@@ -206,6 +206,7 @@ int sqb_ctx_destroy(sqb_ctx* c) {
     c->scratch[0].release();
     c->scratch[1].release();
     c->scratch[2].release();
+    c->scratch[3].release();
     for (int b = 0; b < sqb_ctx::kStage; ++b) {
         if (c->stage_ev[b]) cudaEventDestroy(c->stage_ev[b]);
         if (c->stage[b]) cudaFreeHost(c->stage[b]);

@@ -110,7 +110,7 @@ struct sqb_ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // Large scratch buffers that live as long as the context (GB-sized cudaMalloc/cudaFree per API call would
     // otherwise dominate the host-facing latency).  Work on one ctx is stream ordered, so handles can share them.
-    DevBuf<uint8_t> scratch[3];
+    DevBuf<uint8_t> scratch[4];
     // pinned staging ring for large host-to-device copies of pageable caller memory (sqb_h2d)
     static constexpr int kStage = 16;
     void* stage[kStage] = {};

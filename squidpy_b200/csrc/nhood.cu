@@ -1518,13 +1518,31 @@ __global__ void __launch_bounds__(PIPE_TEAMS * 64) nhood_shuffle_pipe_kernel(LT*
 //                           known), detects position sharing (own-range targets, duplicate targets via a
 //                           shared-memory hash table), swaps conflict-free steps straight in global memory and
 //                           replays the few conflicting ones in step order on staged copies.
+//
+//     PART (shuffle_algo 9): the same targets, stored PARTITIONED BY TARGET REGION for nhood_apply_part_kernel (2j).  A
+//     segment of length m is cut into regions of B positions (sqb_part_regions) and its steps into blocks of
+//     SQB_PART_L consecutive steps; block b (steps [bL, (b+1)L)) keeps its entries in its own slots J[bL, (b+1)L), grouped
+//     by target region (region 0 first) and, inside a region, in step order (descending i).  Entry = ((i - bL) << 18) |
+//     (j - region * B); cnt holds one row of SQB_PART_RMAX u16 counts per (permutation, segment block).  Each warp stages
+//     its current block's targets in shared memory and flushes the block when its last step is generated: a stable
+//     partition by match_any ranks (lower lane = earlier step) and per-region running offsets.
 // ------------------------------------------------------------------------------------------------
-template <int Q>
+#define SQB_PART_L 2048    // steps per block of the partitioned target layout
+#define SQB_PART_RMAX 16   // regions per segment, at most (one u16 count per region and block: a 32-byte row)
+__host__ __device__ __forceinline__ void sqb_part_regions(int m, int cap, int& R, int& B) {
+    R = (m + cap - 1) / cap;
+    B = (((m + R - 1) / R + 15) / 16) * 16;  // balanced regions, <= cap (a multiple of 16)
+}
+
+template <int Q, bool PART>
 __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ J, int64_t stride,
                                                          const uint64_t* __restrict__ states, int64_t n_perms, int nseg,
                                                          const int64_t* __restrict__ seg_start,
-                                                         const int64_t* __restrict__ seg_len, float wfactor) {
+                                                         const int64_t* __restrict__ seg_len, float wfactor,
+                                                         uint16_t* __restrict__ cnt, int64_t nb_total, int region_cap) {
     constexpr int RAW = 64 * Q;
+    constexpr int L = SQB_PART_L;
+    extern __shared__ uint32_t sqb_jgen_smem[];  // PART: per warp [L] staged targets of the current block + [16] region offsets
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t lt_mask = (1u << lane) - 1u;
     // Q independent LCG chains per lane (output q*32 + lane of every batch has its own state, advanced by 32*Q per batch)
@@ -1535,8 +1553,11 @@ __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ 
     pcg_jump_consts((uint64_t)lane + 1, Mt, Ct);
     const int wpb = (int)(blockDim.x >> 5);  // warps per block (1, 2 or 4)
     const int64_t warps_total = (int64_t)gridDim.x * wpb;
+    uint32_t* stage = sqb_jgen_smem + warp * (L + 16);
+    uint32_t* roff = stage + L;
     for (int64_t perm = (int64_t)blockIdx.x * wpb + warp; perm < n_perms; perm += warps_total) {
         uint32_t* __restrict__ Jp = J + perm * stride;
+        int64_t boff = 0;  // PART: count rows of the earlier segments
         const uint64_t* st4 = states + perm * 4;
         const u128 inc = mk128(st4[2], st4[3]);
         u128 st[Q];
@@ -1551,7 +1572,56 @@ __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ 
         int pos = RAW;
         for (int seg = 0; seg < nseg; ++seg) {
             const int64_t base = seg_start[seg];
-            int i_cur = (int)(seg_len[seg] - 1);
+            const int m = (int)seg_len[seg];
+            int i_cur = m - 1;
+            int R = 1, B = 1;
+            if (PART) sqb_part_regions(m, region_cap, R, B);
+            int blk = i_cur / L;  // PART: block of step i_cur
+            // PART: stable partition of block blk (staged entries t in [t0, t1), t = i - blk*L) into its slots of J
+            auto flush = [&]() {
+                const int bL = blk * L;
+                const int t0 = blk == 0 ? 1 : 0, t1 = min(L, m - bL);
+                if (lane < 16) roff[lane] = 0;
+                __syncwarp();
+                for (int c0 = t1 - 1; c0 >= t0; c0 -= 32) {  // per-region counts; the region goes into bits 27.. of the entry
+                    const int t = c0 - lane;
+                    const bool v = t >= t0;
+                    const uint32_t e = v ? stage[t] : 0u;
+                    const uint32_t reg = v ? e / (uint32_t)B : 0xFFFFFFFFu;
+                    const uint32_t peers = __match_any_sync(0xffffffffu, reg);
+                    if (v) {
+                        stage[t] = (reg << 27) | e;
+                        if ((peers & lt_mask) == 0) atomicAdd(&roff[reg], (uint32_t)__popc(peers));
+                    }
+                }
+                __syncwarp();
+                const uint32_t h = lane < 16 ? roff[lane] : 0u;
+                uint32_t incl = h;
+#pragma unroll
+                for (int d = 1; d < 16; d <<= 1) {
+                    const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d);
+                    if (lane >= d) incl += y;
+                }
+                if (lane < 16) {
+                    cnt[((perm * nb_total) + boff + blk) * SQB_PART_RMAX + lane] = (uint16_t)h;
+                    roff[lane] = incl - h;  // running slot of every region
+                }
+                __syncwarp();
+                uint32_t* __restrict__ Jblk = Jp + base + bL;
+                for (int c0 = t1 - 1; c0 >= t0; c0 -= 32) {
+                    const int t = c0 - lane;
+                    const bool v = t >= t0;
+                    const uint32_t e = v ? stage[t] : 0u;
+                    const uint32_t reg = v ? e >> 27 : 0xFFFFFFFFu;
+                    const uint32_t peers = __match_any_sync(0xffffffffu, reg);
+                    const int leader = __ffs(peers) - 1;
+                    uint32_t slot = 0;
+                    if (v && lane == leader) slot = atomicAdd(&roff[reg], (uint32_t)__popc(peers));
+                    slot = __shfl_sync(0xffffffffu, slot, leader) + __popc(peers & lt_mask);
+                    if (v) Jblk[slot] = ((uint32_t)t << 18) | ((e & 0x7FFFFFFu) - reg * (uint32_t)B);
+                }
+                __syncwarp();
+            };
             while (i_cur >= 1) {
                 if (pos >= RAW) {
 #pragma unroll
@@ -1624,14 +1694,31 @@ __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ 
                     S = total;
                     newpos = pos + K;
                 }
-                // target of step i = i_cur - rank, streamed out (read exactly once by the apply kernel)
-                uint32_t* __restrict__ Jtop = Jp + base + i_cur;
+                if (!PART) {
+                    // target of step i = i_cur - rank, streamed out (read exactly once by the apply kernel)
+                    uint32_t* __restrict__ Jtop = Jp + base + i_cur;
 #pragma unroll
-                for (int k = 0; k < 2 * Q; ++k)
-                    if (F[k] && c[k] < S) __stcs(Jtop - c[k], u[k]);
+                    for (int k = 0; k < 2 * Q; ++k)
+                        if (F[k] && c[k] < S) __stcs(Jtop - c[k], u[k]);
+                } else {
+                    // staged per block; a window (S <= RAW < L steps) ends at most one block
+                    const int bL = blk * L;
+#pragma unroll
+                    for (int k = 0; k < 2 * Q; ++k)
+                        if (F[k] && c[k] < S && i_cur - c[k] >= bL) stage[i_cur - c[k] - bL] = u[k];
+                    if (i_cur - S < max(bL, 1)) {
+                        __syncwarp();
+                        flush();
+                        --blk;
+#pragma unroll
+                        for (int k = 0; k < 2 * Q; ++k)
+                            if (F[k] && c[k] < S && i_cur - c[k] < bL) stage[i_cur - c[k] - bL + L] = u[k];
+                    }
+                }
                 i_cur -= S;
                 pos = newpos;
             }
+            if (PART) boff += (m + L - 1) / L;
         }
     }
 }
@@ -2537,6 +2624,313 @@ __global__ void __launch_bounds__(NT, 1) nhood_apply_region_kernel(LT* __restric
 #endif  // SQB_TEST_VARIANTS
 
 // ------------------------------------------------------------------------------------------------
+// 2j. REGION replay over PARTITIONED targets (shuffle_algo 9): the decomposition of 2i (every step applied in the pass of
+//     the region its target falls into, every random access in shared memory), fed by nhood_jgen_kernel<Q, true>, which
+//     stored each block's targets grouped by region.  The pass of region r reads the count rows of the blocks from the
+//     top one down to the block of lo, prefix-sums region r's runs and concatenates them, in step order, into windows of
+//     exactly HS = 2 NT slots (slot s -> thread s % NT): no J re-scan, no compaction, no overflow retry.  Each window is
+//     resolved as in 2i (tests/emu_shuffle.py::_resolve_general_window): filter marks / targeter + owner lists / writes,
+//     three block barriers.  Nothing writes a region before its own pass and every top above it was written by its own
+//     region's pass, so the slab loads straight from the base labels and the label rows need no fill.
+// ------------------------------------------------------------------------------------------------
+template <typename LT, int NT>
+__global__ void __launch_bounds__(NT, 1) nhood_apply_part_kernel(LT* __restrict__ labels, const uint32_t* __restrict__ J,
+                                                                 const uint16_t* __restrict__ cnt, const LT* __restrict__ base_lab,
+                                                                 int64_t stride, int64_t n_perms, int nseg,
+                                                                 const int64_t* __restrict__ seg_start,
+                                                                 const int64_t* __restrict__ seg_len, int64_t nb_total,
+                                                                 int region_cap) {
+    constexpr int L = SQB_PART_L;
+    constexpr uint32_t full_mask = 0xFFFFFFFFu;  // (SQB_CONVERGE)
+    constexpr int HS = 2 * NT;   // slots per window = hash slots per table
+    constexpr int NWB = 2 * HS;  // filter words (16 buckets of 2 bits each)
+    constexpr int LOG_HS = (HS == 1024 ? 10 : HS == 2048 ? 11 : 12);
+    static_assert(HS == (1 << LOG_HS), "HS must be a power of two");
+    constexpr int HS_SHIFT = 32 - LOG_HS;
+    extern __shared__ __align__(16) unsigned char sqb_shuffle_smem[];
+    unsigned long long* s_tabT = reinterpret_cast<unsigned long long*>(sqb_shuffle_smem);  // [HS] (position << 32) | head of its targeter list
+    unsigned long long* s_tabO = s_tabT + HS;                                              // [HS] (position << 32) | slot whose top it is
+    uint32_t* s_bits = reinterpret_cast<uint32_t*>(s_tabO + HS);                            // [NWB] duplicate filter
+    int* s_top = reinterpret_cast<int*>(s_bits + NWB);                                      // [HS] top position of every slot
+    int* s_bpref = s_top + HS;                                                              // [NT + 4] region run prefix per block
+    int* s_bslot = s_bpref + NT + 4;                                                        // [NT] J slot of the run per block
+                                                                                            // (+ 4: the slab stays 16-byte aligned)
+    int* s_wsum = s_bslot + NT;                                                             // [32] scan partials
+    uint16_t* s_next = reinterpret_cast<uint16_t*>(s_wsum + 32);                            // [HS] list links
+    LT* s_otop = reinterpret_cast<LT*>(s_next + HS);                                        // [HS] original top values
+    LT* s_slab = s_otop + HS;                                                               // [region_cap] the region
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int h = tid; h < 2 * HS; h += NT) s_tabT[h] = SQB_EMPTY64;  // both tables
+    for (int w = tid; w < NWB; w += NT) s_bits[w] = 0u;
+    __syncthreads();
+
+    auto mark_pos = [&](uint32_t pl) {
+        const uint32_t sh = (pl & 15u) * 2u;
+        uint32_t* wp = &s_bits[(pl >> 4) & (NWB - 1)];
+        const uint32_t old = atomicOr(wp, 1u << sh);
+        if ((old >> sh) & 1u) atomicOr(wp, 2u << sh);
+    };
+    auto marked_again = [&](uint32_t pl) -> bool { return (s_bits[(pl >> 4) & (NWB - 1)] >> ((pl & 15u) * 2u + 1u)) & 1u; };
+    auto push_targeter = [&](uint32_t pl, int id) -> uint32_t {
+        uint32_t h = (pl * 2654435761u) >> HS_SHIFT;
+        const unsigned long long mine = ((unsigned long long)pl << 32) | (unsigned)id;
+        uint32_t nxt = SQB_NONE16;
+        while (true) {
+            const unsigned long long prev = atomicCAS(&s_tabT[h], SQB_EMPTY64, mine);
+            if (prev == SQB_EMPTY64) break;
+            if ((uint32_t)(prev >> 32) == pl) {  // same position: push in front of the current head
+                if (atomicCAS(&s_tabT[h], prev, mine) == prev) {
+                    nxt = (uint32_t)prev & 0xFFFFu;
+                    break;
+                }
+                continue;
+            }
+            h = (h + 1) & (HS - 1);
+        }
+        s_next[id] = (uint16_t)nxt;
+        return h;
+    };
+    auto insert_owner = [&](uint32_t pl, int id) -> uint32_t {  // tops are distinct: plain insertion
+        uint32_t h = (pl * 2654435761u) >> HS_SHIFT;
+        const unsigned long long mine = ((unsigned long long)pl << 32) | (unsigned)id;
+        while (atomicCAS(&s_tabO[h], SQB_EMPTY64, mine) != SQB_EMPTY64) h = (h + 1) & (HS - 1);
+        return h;
+    };
+    auto find_key = [&](const unsigned long long* tab, uint32_t pl) -> int {
+        uint32_t h = (pl * 2654435761u) >> HS_SHIFT;
+        for (int probes = 0; probes < HS; ++probes) {
+            const unsigned long long e = tab[h];
+            if (e == SQB_EMPTY64) return -1;
+            if ((uint32_t)(e >> 32) == pl) return (int)h;
+            h = (h + 1) & (HS - 1);
+        }
+        return -1;
+    };
+
+    for (int64_t perm = blockIdx.x; perm < n_perms; perm += gridDim.x) {
+        int64_t boff = 0;
+        for (int seg = 0; seg < nseg; ++seg) {
+            const int64_t base = seg_start[seg];
+            const int m = (int)seg_len[seg];  // n < 2^31
+            const int nbs = (m + L - 1) / L;
+            LT* __restrict__ a0 = labels + perm * stride + base;
+            const LT* __restrict__ b0 = base_lab + base;
+            if (m < 2) {  // no steps; the row was not filled
+                if (m == 1 && tid == 0) a0[0] = b0[0];
+                boff += nbs;
+                continue;
+            }
+            const uint32_t* __restrict__ Jb = J + perm * stride + base;
+            const uint16_t* __restrict__ crow = cnt + (perm * nb_total + boff) * SQB_PART_RMAX;
+            boff += nbs;
+            int R, B;
+            sqb_part_regions(m, region_cap, R, B);
+            const int bt = nbs - 1;  // top block
+            for (int r = (m - 1) / B; r >= 0; --r) {
+                const int lo = r * B;
+                const int len = min(B, m - lo);
+                const int hi = lo + len;
+                const int nblk = bt - lo / L + 1;  // <= NT (checked by the host)
+                {  // slab <- base labels [lo, hi)
+                    const LT* __restrict__ src = b0 + lo;
+                    int x0 = 0;
+                    if ((reinterpret_cast<uintptr_t>(src) & 15u) == 0) {
+                        constexpr int EPV = 16 / (int)sizeof(LT);
+                        const int nv = len / EPV;
+                        const uint4* __restrict__ sv = reinterpret_cast<const uint4*>(src);
+                        uint4* dv = reinterpret_cast<uint4*>(s_slab);
+                        for (int x = tid; x < nv; x += NT) dv[x] = __ldg(sv + x);
+                        x0 = nv * EPV;
+                    }
+                    for (int x = x0 + tid; x < len; x += NT) s_slab[x] = src[x];
+                }
+                {  // region r's run in every block (thread t: block bt - t), exclusive prefix over the blocks
+                    int run = 0, slot = 0;
+                    if (tid < nblk) {
+                        const int b = bt - tid;
+                        const uint4* row = reinterpret_cast<const uint4*>(crow + (int64_t)b * SQB_PART_RMAX);
+                        const uint4 q0 = __ldcg(row), q1 = __ldcg(row + 1);
+                        const uint32_t w[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+                        int pre = 0;
+#pragma unroll
+                        for (int k = 0; k < SQB_PART_RMAX; ++k) {
+                            const int c = (int)((w[k >> 1] >> ((k & 1) * 16)) & 0xFFFFu);
+                            if (k < r) pre += c;
+                            if (k == r) run = c;
+                        }
+                        slot = b * L + pre;
+                    }
+                    int incl = run;
+#pragma unroll
+                    for (int d = 1; d < 32; d <<= 1) {
+                        const int y = __shfl_up_sync(0xffffffffu, incl, d);
+                        if (lane >= d) incl += y;
+                    }
+                    if (lane == 31) s_wsum[warp] = incl;
+                    __syncthreads();
+                    if (warp == 0) {
+                        int v = lane < NT / 32 ? s_wsum[lane] : 0;
+#pragma unroll
+                        for (int d = 1; d < 32; d <<= 1) {
+                            const int y = __shfl_up_sync(0xffffffffu, v, d);
+                            if (lane >= d) v += y;
+                        }
+                        s_wsum[lane] = v;  // inclusive over warps
+                    }
+                    __syncthreads();
+                    const int ex = incl - run + (warp > 0 ? s_wsum[warp - 1] : 0);
+                    if (tid < nblk) {
+                        s_bpref[tid] = ex;
+                        s_bslot[tid] = slot;
+                    }
+                    if (tid == nblk - 1) s_bpref[nblk] = ex + run;
+                }
+                __syncthreads();
+                const int total = s_bpref[nblk];
+                // entry of window slot g: binary search for its block (the largest t with s_bpref[t] <= g)
+                auto load_entry = [&](int g, int& top, uint32_t& jl) {
+                    int tl = 0, th = nblk;
+                    while (th - tl > 1) {
+                        const int mid = (tl + th) >> 1;
+                        if (s_bpref[mid] <= g) tl = mid;
+                        else th = mid;
+                    }
+                    const uint32_t e = __ldcs(Jb + s_bslot[tl] + (g - s_bpref[tl]));
+                    top = (bt - tl) * L + (int)(e >> 18);
+                    jl = e & 0x3FFFFu;
+                };
+                int ntop[2];
+                uint32_t njl[2];
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                    ntop[k] = -1, njl[k] = 0;
+                    if (tid + k * NT < total) load_entry(tid + k * NT, ntop[k], njl[k]);
+                }
+                for (int w0 = 0; w0 < total; w0 += HS) {
+                    int top[2];
+                    uint32_t jl[2];
+                    LT vt[2], vj[2];
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {  // originals first (the tops above the region come from global memory)
+                        top[k] = ntop[k], jl[k] = njl[k];
+                        vt[k] = (LT)0, vj[k] = (LT)0;
+                        if (top[k] >= 0) {
+                            vj[k] = s_slab[jl[k]];
+                            vt[k] = (top[k] < hi) ? s_slab[top[k] - lo] : ld_cg<LT>(a0 + top[k]);  // T(i): left there by the pass of i's own region
+                        }
+                    }
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        ntop[k] = -1, njl[k] = 0;
+                        const int g = w0 + HS + tid + k * NT;
+                        if (g < total) load_entry(g, ntop[k], njl[k]);  // the next window's entries
+                    }
+                    // ---- A: stage originals and tops, filter marks ----
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        if (top[k] >= 0) {
+                            const int s = tid + k * NT;
+                            s_otop[s] = vt[k];
+                            s_top[s] = top[k];
+                            mark_pos(jl[k]);
+                            if (top[k] < hi) mark_pos((uint32_t)(top[k] - lo));
+                        }
+                    }
+                    SQB_CONVERGE();
+                    __syncthreads();
+                    // ---- B: slots on multiply-marked positions register in the tables ----
+                    uint32_t slotT[2] = {0, 0}, slotO[2] = {0, 0};
+                    bool stfl[2], sofl[2], sself[2];
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        stfl[k] = sofl[k] = sself[k] = false;
+                        if (top[k] >= 0) {
+                            const int s = tid + k * NT;
+                            const bool inreg = top[k] < hi;
+                            sself[k] = inreg && (uint32_t)(top[k] - lo) == jl[k];
+                            stfl[k] = marked_again(jl[k]);
+                            sofl[k] = inreg && marked_again((uint32_t)(top[k] - lo));
+                            if (stfl[k] && !sself[k]) slotT[k] = push_targeter(jl[k], s);
+                            if (sofl[k]) slotO[k] = insert_owner((uint32_t)(top[k] - lo), s);
+                        }
+                    }
+                    SQB_CONVERGE();
+                    __syncthreads();
+                    // ---- C: writes, from the (now immutable) lists and original values only ----
+                    {
+                        uint4* bz = reinterpret_cast<uint4*>(s_bits);  // nobody reads the filter any more
+#pragma unroll
+                        for (int x = tid; x < NWB / 4; x += NT) bz[x] = make_uint4(0u, 0u, 0u, 0u);
+                    }
+                    // T(x): value of slot x's top just before step x
+                    auto T_of = [&](int x) -> LT {
+                        while (true) {
+                            const int ix = s_top[x];
+                            if (ix >= hi) break;  // tops above the region are never targets
+                            const int h = find_key(s_tabT, (uint32_t)(ix - lo));
+                            if (h < 0) break;
+                            int mx = -1;
+                            for (uint32_t e = (uint32_t)s_tabT[h] & 0xFFFFu; e != SQB_NONE16; e = s_next[e]) mx = max(mx, (int)e);
+                            x = mx;  // the latest targeter of x's top (every targeter of a top precedes its step)
+                        }
+                        return s_otop[x];
+                    };
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        if (top[k] < 0) continue;
+                        const int s = tid + k * NT;
+                        LT val = vj[k];
+                        if (!stfl[k] && !sofl[k]) {
+                            s_slab[jl[k]] = vt[k];
+                        } else {
+                            const LT Ts = sofl[k] ? T_of(s) : vt[k];
+                            if (sself[k]) {
+                                val = Ts;
+                            } else {
+                                bool last = true;  // the only (or the last) slot of this window that targets the position
+                                if (stfl[k]) {
+                                    const uint32_t head = (uint32_t)s_tabT[slotT[k]] & 0xFFFFu;
+                                    int mx;
+                                    const int p = sqb_list_latest_before(s_next, head, s, &mx);
+                                    if (p >= 0) val = T_of(p);
+                                    last = (mx == s);
+                                }
+                                if (last && !(stfl[k] && find_key(s_tabO, jl[k]) >= 0)) s_slab[jl[k]] = Ts;
+                            }
+                        }
+                        if (top[k] < hi) s_slab[top[k] - lo] = val;
+                        else st_cs<LT>(a0 + top[k], val);  // final
+                    }
+                    SQB_CONVERGE();
+                    __syncthreads();
+                    // ---- the table entries of this window are cleared (ordered before the next pushes by its first barrier) ----
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        if (stfl[k] && !sself[k]) s_tabT[slotT[k]] = SQB_EMPTY64;
+                        if (sofl[k]) s_tabO[slotO[k]] = SQB_EMPTY64;
+                    }
+                }
+                __syncthreads();
+                {  // a[lo, hi) <- slab
+                    LT* __restrict__ dst = a0 + lo;
+                    int x0 = 0;
+                    if ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0) {
+                        constexpr int EPV = 16 / (int)sizeof(LT);
+                        const int nv = len / EPV;
+                        uint4* dv = reinterpret_cast<uint4*>(dst);
+                        const uint4* sv = reinterpret_cast<const uint4*>(s_slab);
+                        for (int x = tid; x < nv; x += NT) dv[x] = sv[x];
+                        x0 = nv * EPV;
+                    }
+                    for (int x = x0 + tid; x < len; x += NT) dst[x] = s_slab[x];
+                }
+                __syncthreads();
+            }
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // 3. transpose [P][stride] -> [PB/32][n + 1][32]  (32 permutations x 256 nodes per CTA), optional row scatter through
 //    `order` (library-grouped position k -> original node id)
 // ------------------------------------------------------------------------------------------------
@@ -3166,7 +3560,7 @@ struct sqb_nhood {
     int shuffle_q = 4;     // algo 2: PCG64 outputs per lane per batch (window = 64*q raw values)
     int shuffle_r = 4;     // algo 3: PCG64 outputs per thread per batch (window = 2*r*threads raw values); algo 5: steps per thread
     int64_t shuffle_low = 0;   // algo 5: elements of every label array kept in shared memory (-1 = as much as fits, 0 = off)
-    int64_t shuffle_region = 0;  // algo 8: positions per region (0 = as many as shared memory holds; smaller values are a test hook)
+    int64_t shuffle_region = 0;  // algos 8, 9: positions per region (0 = as many as shared memory holds; smaller values are a test hook)
     int64_t shuffle_stagger_us = 0;  // start-up stagger of the persistent shuffle CTAs / warps (see sqb_stagger)
     int shuffle_threads = 512;
     int64_t perm_chunk = 0;  // 0 = auto
@@ -3424,10 +3818,102 @@ static int launch_apply_region(sqb_nhood* h, LT* lab, const uint32_t* J, int64_t
 #ifndef SQB_TEST_VARIANTS
 static int sqb_variant_unavailable(int algo) {
     sqb_set_error("shuffle_algo %d is a superseded replay variant kept as a cross-check: it is compiled into the test build only "
-                  "(make -C squidpy_b200/csrc testvariants); the product library offers -1 (auto), 1, 2 and 7", algo);
+                  "(make -C squidpy_b200/csrc testvariants); the product library offers -1 (auto), 1, 2, 7 and 9", algo);
     return SQB_ERR_UNSUPPORTED;
 }
 #endif
+
+// swap-target generation (2f) into J; PART: partitioned by target region (2f PART, region_cap and the count rows of 2j)
+template <bool PART>
+static int launch_jgen(sqb_nhood* h, uint32_t* J, const uint64_t* states, int64_t np, uint16_t* cnt, int64_t nb_total,
+                       int region_cap) {
+    sqb_ctx* c = h->ctx;
+    SqbLaunchScope scope(c, SQB_K_MISC);  // J generation is accounted under "misc"
+    // one warp per permutation; small blocks spread the (latency-bound) warps evenly over the SMs
+    const int jt = (int)h->jgen_threads;
+    int64_t ctas = (int64_t)c->sm_count * 8 * (128 / jt);
+    if (ctas > ceil_div64(np, jt / 32)) ctas = ceil_div64(np, jt / 32);
+    const size_t smem = PART ? (size_t)(jt / 32) * (SQB_PART_L + 16) * sizeof(uint32_t) : 0;
+    auto k = h->shuffle_q == 2 ? nhood_jgen_kernel<2, PART> : h->shuffle_q == 8 ? nhood_jgen_kernel<8, PART> : nhood_jgen_kernel<4, PART>;
+    if (PART) SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<(unsigned)ctas, jt, smem, c->stream>>>(J, h->stride, states, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, 4.0f, cnt,
+                                               nb_total, region_cap);
+    SQB_POST_LAUNCH();
+    return SQB_OK;
+}
+
+// shared memory of nhood_apply_part_kernel besides the slab:
+// [tabT, tabO u64 x HS][bits u32 x 2 HS][top int x HS][bpref int x NT + 4][bslot int x NT][wsum int x 32][next u16 x HS][otop LT x HS]
+static size_t part_tables_bytes(int nt, int lt_bytes) {
+    const size_t HS = 2 * (size_t)nt;
+    return 2 * HS * 8 + 2 * HS * 4 + HS * 4 + (2 * (size_t)nt + 4) * 4 + 32 * 4 + HS * 2 + HS * lt_bytes;
+}
+
+// positions per region of shuffle_algo 9 with nt threads (a multiple of 16)
+static int64_t part_region_cap(const sqb_nhood* h, int nt) {
+    const size_t tables = part_tables_bytes(nt, h->lt_bytes);
+    int64_t cap = ((int64_t)h->ctx->smem_optin - (int64_t)tables) / h->lt_bytes;
+    if (cap > (1 << 18) - 16) cap = (1 << 18) - 16;                                 // region offsets are stored in 18 bits
+    if (h->shuffle_region > 0 && cap > h->shuffle_region) cap = h->shuffle_region;  // test hook: small regions
+    cap = (cap / 16) * 16;
+    return cap < 16 ? 16 : cap;
+}
+
+// Threads of the region replay over partitioned targets (shuffle_algo 9) when it runs for np permutations, else 0.  It runs
+// when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that every
+// segment fits SQB_PART_RMAX regions and its step blocks fit one thread each; otherwise the list replay (algo 7) runs.
+// Measured on an H100 80GB HBM3 (400 W), bench.py: at 1M spots x 1000 permutations algo 9 takes 36.7 ms per step against
+// 40.4 ms (apply 19.8 against 32.1 ms, target generation 13.8 against 5.3 ms); at 300 K cells x 10 000 permutations (2
+// regions) the slower partitioning target generation outweighs the apply gain, 118.5 against 86.7 ms, hence the size gate.
+static int part_replay_threads(const sqb_nhood* h, int64_t np) {
+    sqb_ctx* c = h->ctx;
+    int nt = 0;
+    if (h->shuffle_algo == 9) nt = h->shuffle_threads == 512 ? 512 : 1024;
+    else if (h->shuffle_algo < 0 && np > 2 * (int64_t)c->sm_count && h->n >= 524288) nt = 1024;
+    if (nt == 0) return 0;
+    const size_t tables = part_tables_bytes(nt, h->lt_bytes);
+    if (tables + 16 * (size_t)h->lt_bytes > c->smem_optin) return 0;
+    const int cap = (int)part_region_cap(h, nt);
+    for (int64_t m : h->h_seg_len) {
+        int R, B;
+        sqb_part_regions((int)m, cap, R, B);
+        if (R > SQB_PART_RMAX || (m + SQB_PART_L - 1) / SQB_PART_L > nt) return 0;
+    }
+    return nt;
+}
+
+template <typename LT, int NT>
+static int launch_apply_part(sqb_nhood* h, LT* lab, const uint32_t* J, const uint16_t* cnt, int64_t nb_total, int cap, int64_t np) {
+    sqb_ctx* c = h->ctx;
+    auto k = nhood_apply_part_kernel<LT, NT>;
+    const size_t smem = part_tables_bytes(NT, (int)sizeof(LT)) + (size_t)cap * sizeof(LT);
+    SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int64_t grid = h->shuffle_ctas;
+    if (grid <= 0) grid = c->sm_count;  // one CTA per SM (launch bounds), persistent over the permutations
+    if (grid > np) grid = np;
+    k<<<(unsigned)grid, NT, smem, c->stream>>>(lab, J, cnt, reinterpret_cast<const LT*>(h->d_base.p), h->stride, np, h->nseg,
+                                               h->d_seg_start.p, h->d_seg_len.p, nb_total, cap);
+    return SQB_OK;
+}
+
+// shuffle_algo 9: partitioned swap targets + region replay (the label rows are not filled: the replay reads the base labels)
+template <typename LT>
+static int launch_shuffle_part(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, int nt) {
+    sqb_ctx* c = h->ctx;
+    int64_t nb_total = 0;
+    for (int64_t m : h->h_seg_len) nb_total += (m + SQB_PART_L - 1) / SQB_PART_L;
+    SQB_TRY(c->scratch[2].alloc((size_t)np * h->stride * sizeof(uint32_t)));
+    SQB_TRY(c->scratch[3].alloc((size_t)np * nb_total * SQB_PART_RMAX * sizeof(uint16_t)));
+    uint32_t* J = reinterpret_cast<uint32_t*>(c->scratch[2].p);
+    uint16_t* cnt = reinterpret_cast<uint16_t*>(c->scratch[3].p);
+    const int cap = (int)part_region_cap(h, nt);
+    SQB_TRY(launch_jgen<true>(h, J, states, np, cnt, nb_total, cap));
+    SqbLaunchScope scope(c, SQB_K_NHOOD_SHUFFLE);
+    if (nt == 512) SQB_TRY((launch_apply_part<LT, 512>(h, lab, J, cnt, nb_total, cap, np)));
+    else SQB_TRY((launch_apply_part<LT, 1024>(h, lab, J, cnt, nb_total, cap, np)));
+    SQB_POST_LAUNCH();
+    return SQB_OK;
+}
 
 template <typename LT>
 static int launch_shuffle_two_kernel(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, int algo, int nt, int r,
@@ -3436,20 +3922,7 @@ static int launch_shuffle_two_kernel(sqb_nhood* h, LT* lab, const uint64_t* stat
     const float wf = (float)h->shuffle_wfactor_x100 / 100.0f;
     SQB_TRY(c->scratch[2].alloc((size_t)np * h->stride * sizeof(uint32_t)));
     uint32_t* J = reinterpret_cast<uint32_t*>(c->scratch[2].p);
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);  // J generation is accounted under "misc"
-        // one warp per permutation; small blocks spread the (latency-bound) warps evenly over the SMs
-        const int jt = (int)h->jgen_threads;
-        int64_t ctas = (int64_t)c->sm_count * 8 * (128 / jt);
-        if (ctas > ceil_div64(np, jt / 32)) ctas = ceil_div64(np, jt / 32);
-        if (h->shuffle_q == 2)
-            nhood_jgen_kernel<2><<<(unsigned)ctas, jt, 0, c->stream>>>(J, h->stride, states, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, 4.0f);
-        else if (h->shuffle_q == 8)
-            nhood_jgen_kernel<8><<<(unsigned)ctas, jt, 0, c->stream>>>(J, h->stride, states, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, 4.0f);
-        else
-            nhood_jgen_kernel<4><<<(unsigned)ctas, jt, 0, c->stream>>>(J, h->stride, states, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, 4.0f);
-        SQB_POST_LAUNCH();
-    }
+    SQB_TRY(launch_jgen<false>(h, J, states, np, nullptr, 0, 0));
     SqbLaunchScope scope(c, SQB_K_NHOOD_SHUFFLE);
     int rc = SQB_ERR_INVALID;
     if (algo == 8) {  // (shuffle_r is not used by this variant)
@@ -3500,14 +3973,17 @@ static int launch_shuffle_two_kernel(sqb_nhood* h, LT* lab, const uint64_t* stat
 template <typename LT>
 static int launch_shuffle(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np) {
     sqb_ctx* c = h->ctx;
+    if (const int nt = part_replay_threads(h, np)) return launch_shuffle_part<LT>(h, lab, states, np, nt);
     if (h->shuffle_algo == 5 || h->shuffle_algo == 7 || h->shuffle_algo == 8)
         return launch_shuffle_two_kernel<LT>(h, lab, states, np, h->shuffle_algo, h->shuffle_threads, h->shuffle_r, h->shuffle_low,
                                              (uint64_t)h->shuffle_stagger_us * 1000ull);
-    // auto: many permutations of large arrays -> J generation + list apply with the tuned shape (1024 threads, 2048-step
-    // windows, 96 K elements of every array in shared memory, CTAs started about one replay's length apart: ~2.5 ns per
-    // element); few permutations -> one CTA each (finishes sooner); many permutations of small arrays (L1/L2 resident) -> one
-    // warp each.  tools/tune_nhood.py on H100 (1M spots x 1000 permutations) picked the shape, stagger and grid rule.
-    if (h->shuffle_algo < 0 && np > 2 * (int64_t)c->sm_count && h->n >= 65536)
+    // auto: many permutations of large arrays -> partitioned J generation + region replay (algo 9, above) where every segment
+    // fits its region and block limits, else J generation + list apply with the tuned shape (1024 threads, 2048-step windows,
+    // 96 K elements of every array in shared memory, CTAs started about one replay's length apart: ~2.5 ns per element); few
+    // permutations -> one CTA each (finishes sooner); many permutations of small arrays (L1/L2 resident) -> one warp each.
+    // tools/tune_nhood.py on H100 (1M spots x 1000 permutations) picked the list replay's shape, stagger and grid rule.
+    // shuffle_algo 9 outside those limits takes the same list replay.
+    if ((h->shuffle_algo < 0 && np > 2 * (int64_t)c->sm_count && h->n >= 65536) || h->shuffle_algo == 9)
         return launch_shuffle_two_kernel<LT>(h, lab, states, np, 7, 1024, 2, 98304,
                                              h->shuffle_stagger_us > 0 ? (uint64_t)h->shuffle_stagger_us * 1000ull : (uint64_t)h->n * 5 / 2);
     SqbLaunchScope scope(c, SQB_K_NHOOD_SHUFFLE);
@@ -3607,7 +4083,7 @@ static int run_chunk(sqb_nhood* h, int64_t p0, int64_t np, bool do_count) {
     LT* lab = reinterpret_cast<LT*>(c->scratch[0].p);
     LT* labT = reinterpret_cast<LT*>(c->scratch[1].p);
     const int64_t vec_per_row = h->stride * (int64_t)sizeof(LT) / 16;
-    {
+    if (!part_replay_threads(h, np)) {  // the partitioned region replay reads the base labels itself
         SqbLaunchScope scope(c, SQB_K_NHOOD_FILL);
         unsigned gx = (unsigned)ceil_div64(vec_per_row, 256 * 4);
         if (gx < 1) gx = 1;
@@ -4034,7 +4510,7 @@ int sqb_nhood_destroy(sqb_nhood* h) {
 int sqb_nhood_set_option(sqb_nhood* h, const char* key, int64_t value) {
     SQB_CHECK(h && key, SQB_ERR_INVALID, "sqb_nhood_set_option: null argument");
     if (!strcmp(key, "shuffle_algo")) {
-        SQB_CHECK(value >= -1 && value <= 8, SQB_ERR_INVALID, "shuffle_algo must be -1 (auto) or 0..8");
+        SQB_CHECK(value >= -1 && value <= 9, SQB_ERR_INVALID, "shuffle_algo must be -1 (auto) or 0..9");
         h->shuffle_algo = (int)value;
     } else if (!strcmp(key, "jgen_threads")) {
         SQB_CHECK(value == 32 || value == 64 || value == 128, SQB_ERR_INVALID, "jgen_threads must be 32, 64 or 128");

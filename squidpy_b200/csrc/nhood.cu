@@ -1523,27 +1523,156 @@ __global__ void __launch_bounds__(PIPE_TEAMS * 64) nhood_shuffle_pipe_kernel(LT*
 //     segment of length m is cut into regions of B positions (sqb_part_regions) and its steps into blocks of
 //     SQB_PART_L consecutive steps; block b (steps [bL, (b+1)L)) keeps its entries in its own slots J[bL, (b+1)L), grouped
 //     by target region (region 0 first) and, inside a region, in step order (descending i).  Entry = ((i - bL) << 18) |
-//     (j - region * B); cnt holds one row of SQB_PART_RMAX u16 counts per (permutation, segment block).  Each warp stages
-//     its current block's targets in shared memory and flushes the block when its last step is generated: a stable
-//     partition by match_any ranks (lower lane = earlier step) and per-region running offsets.
+//     (j - region * B); cnt holds one row of SQB_PART_RMAX u16 counts per (permutation, segment block).
+//     The partition runs beside the generation, not after it: every generator warp is paired with a partition warp of the
+//     same CTA (nhood_part_warp).  The generator only stores the target of step i at word part_idx(i - bL) of one of two
+//     block buffers and hands a complete block over through an mbarrier pair (full / empty per buffer), so it fills block
+//     b - 1 while block b is being partitioned.  The partition warp walks the same (permutation, segment, block) sequence.
+//     Lane l owns the 64 steps t in [64 l, 64 l + 64) of the block: it counts its entries per region, one 16-region
+//     suffix scan over the lanes turns the counts into slots (higher t = earlier step comes first), it scatters its entries
+//     in step order into an output block in shared memory, and the warp streams that block out to J in whole lines.  The
+//     region of a target is a multiply-high by a per-segment magic number, exact for every j < 2^31 (sqb_part_magic).
 // ------------------------------------------------------------------------------------------------
 #define SQB_PART_L 2048    // steps per block of the partitioned target layout
 #define SQB_PART_RMAX 16   // regions per segment, at most (one u16 count per region and block: a 32-byte row)
+#define SQB_PART_LP (SQB_PART_L + SQB_PART_L / 64)  // words of a block buffer: one pad word per 64 (lane l reads words 65 l + s)
+// shared memory words of a generator / partition pair: mbarriers full[2], empty[2]; two block buffers; the output block;
+// the per-lane region table [SQB_PART_RMAX][32]
+#define SQB_PART_PAIR_WORDS (8 + 2 * SQB_PART_LP + SQB_PART_L + SQB_PART_RMAX * 32)
 __host__ __device__ __forceinline__ void sqb_part_regions(int m, int cap, int& R, int& B) {
     R = (m + cap - 1) / cap;
     B = (((m + R - 1) / R + 15) / 16) * 16;  // balanced regions, <= cap (a multiple of 16)
 }
+// region of target j = __umulhi(j, M) >> sh for 16 <= B < 2^31: sh = floor(log2(B - 1)), M = ceil(2^(32 + sh) / B) < 2^32.
+// With e = M B - 2^(32 + sh) < B <= 2^(sh + 1), j M / 2^(32 + sh) = j / B + j e / (B 2^(32 + sh)) and the excess stays below
+// 1 / B whenever j e < 2^(32 + sh), i.e. for every j < 2^31 (tests/test_part_magic.py checks it for every B <= 2^18).
+__host__ __device__ __forceinline__ void sqb_part_magic(int B, uint32_t& M, int& sh) {
+    sh = 31 - __builtin_clz((unsigned)(B - 1));
+    M = (uint32_t)(((1ull << (32 + sh)) + (uint64_t)B - 1) / (uint64_t)B);
+}
+__device__ __forceinline__ int part_idx(int t) { return t + (t >> 6); }
 
+__device__ __forceinline__ void mbar_init(uint64_t* b, unsigned count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(b)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* b) {
+    asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"((unsigned)__cvta_generic_to_shared(b)) : "memory");
+}
+// waits until the phase of parity `parity` has completed (parity 1 on a fresh barrier: at once)
+__device__ __forceinline__ void mbar_wait(uint64_t* b, unsigned parity) {
+    const unsigned a = (unsigned)__cvta_generic_to_shared(b);
+    unsigned done;
+    do {
+        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.acquire.cta.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+                     : "=r"(done)
+                     : "r"(a), "r"(parity)
+                     : "memory");
+    } while (!done);
+}
+
+// Partition warp of nhood_jgen_kernel<Q, true>: block seq of its generator arrives in buffer seq & 1 (use seq >> 1 of it).
+__device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uint32_t* __restrict__ J, int64_t stride,
+                                                int64_t perm0, int64_t n_perms, int64_t warps_total, int nseg,
+                                                const int64_t* __restrict__ seg_start, const int64_t* __restrict__ seg_len,
+                                                uint16_t* __restrict__ cnt, int64_t nb_total, int region_cap, int lane) {
+    constexpr int L = SQB_PART_L;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(pair);  // full[0], full[1], empty[0], empty[1]
+    uint32_t* __restrict__ out = pair + 8 + 2 * SQB_PART_LP;
+    uint32_t* __restrict__ tab = out + L;  // tab[r * 32 + lane]: this lane's entries of region r, then its next slot
+    unsigned seq = 0;
+    for (int64_t perm = perm0; perm < n_perms; perm += warps_total) {
+        int64_t row = perm * nb_total;  // count row of the current block's segment, block 0
+        for (int seg = 0; seg < nseg; ++seg) {
+            const int m = (int)seg_len[seg];
+            if (m >= 2) {
+                int R, B, sh;
+                uint32_t M;
+                sqb_part_regions(m, region_cap, R, B);
+                sqb_part_magic(B, M, sh);
+                uint32_t* __restrict__ Jseg = J + perm * stride + seg_start[seg];
+                for (int blk = (m - 1) / L; blk >= 0; --blk, ++seq) {
+                    const int bL = blk * L, t0 = blk == 0 ? 1 : 0, t1 = min(L, m - bL);
+                    const int s0 = max(t0 - 64 * lane, 0), s1 = min(t1 - 64 * lane, 64);  // this lane's steps t = 64 lane + s
+                    const uint32_t* __restrict__ in = pair + 8 + (seq & 1) * SQB_PART_LP + 65 * lane;
+#pragma unroll
+                    for (int r = 0; r < SQB_PART_RMAX; ++r) tab[r * 32 + lane] = 0;
+                    mbar_wait(&bar[seq & 1], (seq >> 1) & 1);
+#pragma unroll 4
+                    for (int s = s0; s < s1; ++s) ++tab[(__umulhi(in[s], M) >> sh) * 32 + lane];
+                    // slots: region base + entries of the same region on higher lanes (earlier steps); 16-bit fields, 2 regions a word
+                    uint32_t w[SQB_PART_RMAX / 2], x[SQB_PART_RMAX / 2];
+#pragma unroll
+                    for (int k = 0; k < SQB_PART_RMAX / 2; ++k) x[k] = w[k] = tab[2 * k * 32 + lane] | (tab[(2 * k + 1) * 32 + lane] << 16);
+#pragma unroll
+                    for (int d = 1; d < 32; d <<= 1)
+#pragma unroll
+                        for (int k = 0; k < SQB_PART_RMAX / 2; ++k) {
+                            const uint32_t y = __shfl_down_sync(0xffffffffu, x[k], d);
+                            if (lane + d < 32) x[k] += y;
+                        }
+                    uint32_t run = 0, tot[SQB_PART_RMAX / 2];
+#pragma unroll
+                    for (int k = 0; k < SQB_PART_RMAX / 2; ++k) {
+                        tot[k] = __shfl_sync(0xffffffffu, x[k], 0);
+                        const uint32_t lo = tot[k] & 0xFFFFu;
+                        const uint32_t slot = (run | ((run + lo) << 16)) + x[k] - w[k];
+                        run += lo + (tot[k] >> 16);
+                        tab[2 * k * 32 + lane] = slot & 0xFFFFu;
+                        tab[(2 * k + 1) * 32 + lane] = slot >> 16;
+                    }
+                    if (lane == 0) {  // the count row: u16 counts of regions 0..15, little-endian pairs = tot[]
+                        uint4* crow = reinterpret_cast<uint4*>(cnt + (row + blk) * SQB_PART_RMAX);
+                        crow[0] = make_uint4(tot[0], tot[1], tot[2], tot[3]);
+                        crow[1] = make_uint4(tot[4], tot[5], tot[6], tot[7]);
+                    }
+                    __syncwarp();  // every lane has streamed the previous output block out
+#pragma unroll 4
+                    for (int s = s1 - 1; s >= s0; --s) {  // in step order
+                        const uint32_t j = in[s];
+                        const uint32_t r = __umulhi(j, M) >> sh;
+                        const uint32_t slot = tab[r * 32 + lane];
+                        tab[r * 32 + lane] = slot + 1;
+                        out[slot] = ((uint32_t)(64 * lane + s) << 18) | (j - r * (uint32_t)B);
+                    }
+                    mbar_arrive(&bar[2 + (seq & 1)]);  // the buffer is free for the generator
+                    __syncwarp();
+                    uint32_t* __restrict__ Jblk = Jseg + bL;
+                    for (int k = lane; k < t1 - t0; k += 32) __stcs(Jblk + k, out[k]);
+                }
+            }
+            row += (m + L - 1) / L;
+        }
+    }
+}
+
+// PART: two blocks of 4 pairs per SM (all the shared memory holds); that register bound also keeps ptxas from spilling the
+// generator, which it does at 80 registers without one
 template <int Q, bool PART>
-__global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ J, int64_t stride,
-                                                         const uint64_t* __restrict__ states, int64_t n_perms, int nseg,
-                                                         const int64_t* __restrict__ seg_start,
-                                                         const int64_t* __restrict__ seg_len, float wfactor,
-                                                         uint16_t* __restrict__ cnt, int64_t nb_total, int region_cap) {
+__global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 0) nhood_jgen_kernel(uint32_t* __restrict__ J, int64_t stride,
+                                                                      const uint64_t* __restrict__ states, int64_t n_perms,
+                                                                      int nseg, const int64_t* __restrict__ seg_start,
+                                                                      const int64_t* __restrict__ seg_len, float wfactor,
+                                                                      uint16_t* __restrict__ cnt, int64_t nb_total,
+                                                                      int region_cap) {
     constexpr int RAW = 64 * Q;
     constexpr int L = SQB_PART_L;
-    extern __shared__ uint32_t sqb_jgen_smem[];  // PART: per warp [L] staged targets of the current block + [16] region offsets
+    extern __shared__ uint32_t sqb_jgen_smem[];  // PART: SQB_PART_PAIR_WORDS per generator / partition pair
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // generator warps per block (1, 2 or 4); PART: warps [wpb, 2 wpb) are their partition warps
+    const int wpb = (int)(blockDim.x >> (PART ? 6 : 5));
+    const int64_t warps_total = (int64_t)gridDim.x * wpb;
+    uint32_t* pair = sqb_jgen_smem + (warp % wpb) * SQB_PART_PAIR_WORDS;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(pair);
+    if (PART) {
+        if (warp < wpb && lane < 4) mbar_init(&bar[lane], 32);
+        __syncthreads();
+        if (warp >= wpb) {
+            nhood_part_warp(pair, J, stride, (int64_t)blockIdx.x * wpb + warp - wpb, n_perms, warps_total, nseg, seg_start,
+                            seg_len, cnt, nb_total, region_cap, lane);
+            return;
+        }
+    }
+    unsigned seq = 0;  // PART: blocks handed to the partition warp so far
     const uint32_t lt_mask = (1u << lane) - 1u;
     // Q independent LCG chains per lane (output q*32 + lane of every batch has its own state, advanced by 32*Q per batch)
     // instead of one chain stepped Q times: the 128-bit multiply-adds of a batch no longer depend on each other
@@ -1551,13 +1680,8 @@ __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ 
     pcg_jump_consts(32, M32, C32);
     pcg_jump_consts((uint64_t)32 * Q, MQ, CQ);
     pcg_jump_consts((uint64_t)lane + 1, Mt, Ct);
-    const int wpb = (int)(blockDim.x >> 5);  // warps per block (1, 2 or 4)
-    const int64_t warps_total = (int64_t)gridDim.x * wpb;
-    uint32_t* stage = sqb_jgen_smem + warp * (L + 16);
-    uint32_t* roff = stage + L;
     for (int64_t perm = (int64_t)blockIdx.x * wpb + warp; perm < n_perms; perm += warps_total) {
         uint32_t* __restrict__ Jp = J + perm * stride;
-        int64_t boff = 0;  // PART: count rows of the earlier segments
         const uint64_t* st4 = states + perm * 4;
         const u128 inc = mk128(st4[2], st4[3]);
         u128 st[Q];
@@ -1574,54 +1698,8 @@ __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ 
             const int64_t base = seg_start[seg];
             const int m = (int)seg_len[seg];
             int i_cur = m - 1;
-            int R = 1, B = 1;
-            if (PART) sqb_part_regions(m, region_cap, R, B);
             int blk = i_cur / L;  // PART: block of step i_cur
-            // PART: stable partition of block blk (staged entries t in [t0, t1), t = i - blk*L) into its slots of J
-            auto flush = [&]() {
-                const int bL = blk * L;
-                const int t0 = blk == 0 ? 1 : 0, t1 = min(L, m - bL);
-                if (lane < 16) roff[lane] = 0;
-                __syncwarp();
-                for (int c0 = t1 - 1; c0 >= t0; c0 -= 32) {  // per-region counts; the region goes into bits 27.. of the entry
-                    const int t = c0 - lane;
-                    const bool v = t >= t0;
-                    const uint32_t e = v ? stage[t] : 0u;
-                    const uint32_t reg = v ? e / (uint32_t)B : 0xFFFFFFFFu;
-                    const uint32_t peers = __match_any_sync(0xffffffffu, reg);
-                    if (v) {
-                        stage[t] = (reg << 27) | e;
-                        if ((peers & lt_mask) == 0) atomicAdd(&roff[reg], (uint32_t)__popc(peers));
-                    }
-                }
-                __syncwarp();
-                const uint32_t h = lane < 16 ? roff[lane] : 0u;
-                uint32_t incl = h;
-#pragma unroll
-                for (int d = 1; d < 16; d <<= 1) {
-                    const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d);
-                    if (lane >= d) incl += y;
-                }
-                if (lane < 16) {
-                    cnt[((perm * nb_total) + boff + blk) * SQB_PART_RMAX + lane] = (uint16_t)h;
-                    roff[lane] = incl - h;  // running slot of every region
-                }
-                __syncwarp();
-                uint32_t* __restrict__ Jblk = Jp + base + bL;
-                for (int c0 = t1 - 1; c0 >= t0; c0 -= 32) {
-                    const int t = c0 - lane;
-                    const bool v = t >= t0;
-                    const uint32_t e = v ? stage[t] : 0u;
-                    const uint32_t reg = v ? e >> 27 : 0xFFFFFFFFu;
-                    const uint32_t peers = __match_any_sync(0xffffffffu, reg);
-                    const int leader = __ffs(peers) - 1;
-                    uint32_t slot = 0;
-                    if (v && lane == leader) slot = atomicAdd(&roff[reg], (uint32_t)__popc(peers));
-                    slot = __shfl_sync(0xffffffffu, slot, leader) + __popc(peers & lt_mask);
-                    if (v) Jblk[slot] = ((uint32_t)t << 18) | ((e & 0x7FFFFFFu) - reg * (uint32_t)B);
-                }
-                __syncwarp();
-            };
+            if (PART && i_cur >= 1) mbar_wait(&bar[2 + (seq & 1)], ((seq >> 1) & 1) ^ 1);  // its buffer is free
             while (i_cur >= 1) {
                 if (pos >= RAW) {
 #pragma unroll
@@ -1703,22 +1781,25 @@ __global__ void __launch_bounds__(128) nhood_jgen_kernel(uint32_t* __restrict__ 
                 } else {
                     // staged per block; a window (S <= RAW < L steps) ends at most one block
                     const int bL = blk * L;
+                    uint32_t* stage = pair + 8 + (seq & 1) * SQB_PART_LP;
 #pragma unroll
                     for (int k = 0; k < 2 * Q; ++k)
-                        if (F[k] && c[k] < S && i_cur - c[k] >= bL) stage[i_cur - c[k] - bL] = u[k];
-                    if (i_cur - S < max(bL, 1)) {
-                        __syncwarp();
-                        flush();
-                        --blk;
+                        if (F[k] && c[k] < S && i_cur - c[k] >= bL) stage[part_idx(i_cur - c[k] - bL)] = u[k];
+                    if (i_cur - S < max(bL, 1)) {  // block blk is complete: hand it to the partition warp
+                        mbar_arrive(&bar[seq & 1]);
+                        ++seq;
+                        if (--blk >= 0) {  // the window's lower steps open block blk - 1 in the other buffer
+                            mbar_wait(&bar[2 + (seq & 1)], ((seq >> 1) & 1) ^ 1);
+                            stage = pair + 8 + (seq & 1) * SQB_PART_LP;
 #pragma unroll
-                        for (int k = 0; k < 2 * Q; ++k)
-                            if (F[k] && c[k] < S && i_cur - c[k] < bL) stage[i_cur - c[k] - bL + L] = u[k];
+                            for (int k = 0; k < 2 * Q; ++k)
+                                if (F[k] && c[k] < S && i_cur - c[k] < bL) stage[part_idx(i_cur - c[k] - bL + L)] = u[k];
+                        }
                     }
                 }
                 i_cur -= S;
                 pos = newpos;
             }
-            if (PART) boff += (m + L - 1) / L;
         }
     }
 }
@@ -3530,7 +3611,8 @@ struct sqb_nhood {
     uint32_t n_self = 0;
     bool sym = false;
     int count_sym = -1;  // -1 auto (use the upper CSR when the graph is symmetric), 0 = always the full CSR
-    int jgen_threads = 128;  // block size of the swap-target generation kernel (32 / 64 / 128: 1 / 2 / 4 permutations per block)
+    int jgen_threads = 128;  // generator threads per block of the swap-target generation kernel (32 / 64 / 128: 1 / 2 / 4
+                             // permutations per block; the partitioned variant adds one partition warp per generator warp)
     int count_un = 4;    // records (of three entries) a warp takes per pass in the count kernel (1 / 2 / 3 / 4)
     DevBuf<uint8_t> d_base;   // stride * lt_bytes, library-grouped order
     DevBuf<uint32_t> d_order;  // grouped position -> node id (only with libraries)
@@ -3829,15 +3911,23 @@ static int launch_jgen(sqb_nhood* h, uint32_t* J, const uint64_t* states, int64_
                        int region_cap) {
     sqb_ctx* c = h->ctx;
     SqbLaunchScope scope(c, SQB_K_MISC);  // J generation is accounted under "misc"
-    // one warp per permutation; small blocks spread the (latency-bound) warps evenly over the SMs
+    // one generator warp per permutation; small blocks spread the (latency-bound) warps evenly over the SMs.  jgen_threads =
+    // generator threads per block; PART adds as many partition threads.
     const int jt = (int)h->jgen_threads;
     int64_t ctas = (int64_t)c->sm_count * 8 * (128 / jt);
-    if (ctas > ceil_div64(np, jt / 32)) ctas = ceil_div64(np, jt / 32);
-    const size_t smem = PART ? (size_t)(jt / 32) * (SQB_PART_L + 16) * sizeof(uint32_t) : 0;
+    const size_t smem = PART ? (size_t)(jt / 32) * SQB_PART_PAIR_WORDS * sizeof(uint32_t) : 0;
     auto k = h->shuffle_q == 2 ? nhood_jgen_kernel<2, PART> : h->shuffle_q == 8 ? nhood_jgen_kernel<8, PART> : nhood_jgen_kernel<4, PART>;
-    if (PART) SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<(unsigned)ctas, jt, smem, c->stream>>>(J, h->stride, states, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, 4.0f, cnt,
-                                               nb_total, region_cap);
+    if (PART) {
+        // the pairs' buffers bound the resident blocks: launch exactly those, so that no warp waits for a second wave
+        SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int per_sm = 0;
+        SQB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 2 * jt, smem));
+        SQB_CHECK(per_sm > 0, SQB_ERR_UNSUPPORTED, "partitioned target generation: %zu bytes of shared memory per block do not fit", smem);
+        ctas = (int64_t)c->sm_count * per_sm;
+    }
+    if (ctas > ceil_div64(np, jt / 32)) ctas = ceil_div64(np, jt / 32);
+    k<<<(unsigned)ctas, PART ? 2 * jt : jt, smem, c->stream>>>(J, h->stride, states, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p,
+                                                                4.0f, cnt, nb_total, region_cap);
     SQB_POST_LAUNCH();
     return SQB_OK;
 }
@@ -3862,9 +3952,11 @@ static int64_t part_region_cap(const sqb_nhood* h, int nt) {
 // Threads of the region replay over partitioned targets (shuffle_algo 9) when it runs for np permutations, else 0.  It runs
 // when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that every
 // segment fits SQB_PART_RMAX regions and its step blocks fit one thread each; otherwise the list replay (algo 7) runs.
-// Measured on an H100 80GB HBM3 (400 W), bench.py: at 1M spots x 1000 permutations algo 9 takes 36.7 ms per step against
-// 40.4 ms (apply 19.8 against 32.1 ms, target generation 13.8 against 5.3 ms); at 300 K cells x 10 000 permutations (2
-// regions) the slower partitioning target generation outweighs the apply gain, 118.5 against 86.7 ms, hence the size gate.
+// Measured on an H100 80GB HBM3 (400 W), tools/apply_time.py: at 1M spots x 1000 permutations algo 9 takes 29.6 ms per step
+// (apply 19.9 ms, target generation with the partition warps 7.0 ms against 5.3 ms without); at 300 K cells x 10 000
+// permutations (2 regions, tools/apply_time.py cfg5) it takes 111.1 ms against the list replay's 83.6 ms: its apply is the
+// slower one there (64.5 against 45.5 ms), and its target generation, bound to fewer resident warps by the block buffers,
+// takes 24.0 against 14.6 ms.  Hence the size gate.
 static int part_replay_threads(const sqb_nhood* h, int64_t np) {
     sqb_ctx* c = h->ctx;
     int nt = 0;

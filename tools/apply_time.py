@@ -1,5 +1,6 @@
-"""Exact-mode nhood step at configs[1] (1M spots, 30 clusters, P permutations) for several replay variants: per-kernel-class
-CUDA-event times.  usage: python tools/apply_time.py [P] [algo:threads:r[:key=value...]] ..."""
+"""Exact-mode nhood step at configs[1] (1M spots, 30 clusters, P permutations) or, with cfg5 as the first argument, at the
+nhood shape of configs[4] (300 K MERFISH-shaped cells, kNN(6), 12 clusters, 10 000 permutations by default) for several replay
+variants: per-kernel-class CUDA-event times.  usage: python tools/apply_time.py [cfg5] [P] [algo:threads:r[:key=value...]] ..."""
 import sys
 
 import numpy as np
@@ -10,15 +11,26 @@ from squidpy_b200._rng import spawn_states  # noqa: E402
 from squidpy_b200.gr import NhoodPlan  # noqa: E402
 from tools import synth  # noqa: E402
 
-P = int(sys.argv[1]) if len(sys.argv) > 1 else 1000
-variants = sys.argv[2:] or ["-1:1024:2", "8:1024:2"]
+args = sys.argv[1:]
+cfg5 = bool(args) and args[0] == "cfg5"
+args = args[1:] if cfg5 else args
+P = int(args[0]) if args else (10000 if cfg5 else 1000)
+variants = args[1:] or ["-1:1024:2", "8:1024:2"]
 ctx = sq.default_context(0)
-g = synth.hex_graph(1000, 1000)
-base = synth.categorical_labels(g.shape[0], 30, seed=0).cat.codes.to_numpy().astype(np.uint32)
+if cfg5:
+    from squidpy_b200.gr import KNNBuilder  # noqa: E402
+
+    g, _ = KNNBuilder(n_neighs=6, ctx=ctx).build(synth.thomas_points(300_000, seed=5))
+    n_cls = 12
+    base = synth.dirichlet_labels(300_000, n_cls, seed=5).cat.codes.to_numpy().astype(np.uint32)
+else:
+    g = synth.hex_graph(1000, 1000)
+    n_cls = 30
+    base = synth.categorical_labels(g.shape[0], n_cls, seed=0).cat.codes.to_numpy().astype(np.uint32)
 ref = None
 for v in variants:
     parts = v.split(":")
-    plan = NhoodPlan(g.indptr, g.indices, 30, ctx)
+    plan = NhoodPlan(g.indptr, g.indices, n_cls, ctx)
     plan.set_option("shuffle_algo", int(parts[0]))
     if int(parts[0]) >= 0:
         plan.set_option("shuffle_threads", int(parts[1]))

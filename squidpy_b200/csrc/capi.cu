@@ -162,6 +162,8 @@ int sqb_ctx_create(int device, void* stream, sqb_ctx** out) {
     c->device = device;
     c->sm_count = prop.multiProcessorCount;
     c->smem_optin = prop.sharedMemPerBlockOptin;
+    c->smem_per_sm = prop.sharedMemPerMultiprocessor;
+    c->smem_reserved = prop.reservedSharedMemPerBlock;
     c->l2_bytes = (size_t)prop.l2CacheSize;
     if (stream) {
         c->stream = (cudaStream_t)stream;

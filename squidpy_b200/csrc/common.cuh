@@ -103,6 +103,8 @@ struct sqb_ctx {
     int sm_count = 132;
     size_t l2_bytes = (size_t)50 << 20;
     size_t smem_optin = 0;   // max opt-in dynamic shared memory per block
+    size_t smem_per_sm = 0;  // shared memory per SM, shared by its resident blocks
+    size_t smem_reserved = 0;  // shared memory the system reserves for every resident block
     int64_t launches = 0;
     bool profile = false;
     double k_ms[SQB_K_NCLASS] = {0};

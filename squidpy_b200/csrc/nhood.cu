@@ -2715,12 +2715,13 @@ __global__ void __launch_bounds__(NT, 1) nhood_apply_region_kernel(LT* __restric
 //     region's pass, so the slab loads straight from the base labels and the label rows need no fill.
 // ------------------------------------------------------------------------------------------------
 template <typename LT, int NT>
-__global__ void __launch_bounds__(NT, 1) nhood_apply_part_kernel(LT* __restrict__ labels, const uint32_t* __restrict__ J,
-                                                                 const uint16_t* __restrict__ cnt, const LT* __restrict__ base_lab,
-                                                                 int64_t stride, int64_t n_perms, int nseg,
-                                                                 const int64_t* __restrict__ seg_start,
-                                                                 const int64_t* __restrict__ seg_len, int64_t nb_total,
-                                                                 int region_cap) {
+__global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __restrict__ labels, const uint32_t* __restrict__ J,
+                                                                         const uint16_t* __restrict__ cnt,
+                                                                         const LT* __restrict__ base_lab, int64_t stride,
+                                                                         int64_t n_perms, int nseg,
+                                                                         const int64_t* __restrict__ seg_start,
+                                                                         const int64_t* __restrict__ seg_len, int64_t nb_total,
+                                                                         int region_cap) {
     constexpr int L = SQB_PART_L;
     constexpr uint32_t full_mask = 0xFFFFFFFFu;  // (SQB_CONVERGE)
     constexpr int HS = 2 * NT;   // slots per window = hash slots per table
@@ -3939,58 +3940,95 @@ static size_t part_tables_bytes(int nt, int lt_bytes) {
     return 2 * HS * 8 + 2 * HS * 4 + HS * 4 + (2 * (size_t)nt + 4) * 4 + 32 * 4 + HS * 2 + HS * lt_bytes;
 }
 
-// positions per region of shuffle_algo 9 with nt threads (a multiple of 16)
-static int64_t part_region_cap(const sqb_nhood* h, int nt) {
-    const size_t tables = part_tables_bytes(nt, h->lt_bytes);
-    int64_t cap = ((int64_t)h->ctx->smem_optin - (int64_t)tables) / h->lt_bytes;
+// positions per region of shuffle_algo 9 with nt threads and per_sm resident CTAs per SM (a multiple of 16; 0 = not even 16
+// positions fit): one CTA takes the opt-in limit of a block, two share the SM's shared memory less a block's reservation each
+static int64_t part_region_cap(const sqb_nhood* h, int nt, int per_sm) {
+    const sqb_ctx* c = h->ctx;
+    int64_t budget = (int64_t)c->smem_optin;
+    if (per_sm > 1) budget = std::min(budget, (int64_t)(c->smem_per_sm / per_sm) - (int64_t)c->smem_reserved);
+    int64_t cap = (budget - (int64_t)part_tables_bytes(nt, h->lt_bytes)) / h->lt_bytes;
     if (cap > (1 << 18) - 16) cap = (1 << 18) - 16;                                 // region offsets are stored in 18 bits
     if (h->shuffle_region > 0 && cap > h->shuffle_region) cap = h->shuffle_region;  // test hook: small regions
     cap = (cap / 16) * 16;
-    return cap < 16 ? 16 : cap;
+    return cap < 16 ? 0 : cap;
 }
 
-// Threads of the region replay over partitioned targets (shuffle_algo 9) when it runs for np permutations, else 0.  It runs
-// when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that every
-// segment fits SQB_PART_RMAX regions and its step blocks fit one thread each; otherwise the list replay (algo 7) runs.
-// Measured on an H100 80GB HBM3 (400 W), tools/apply_time.py: at 1M spots x 1000 permutations algo 9 takes 29.6 ms per step
-// (apply 19.9 ms, target generation with the partition warps 7.0 ms against 5.3 ms without); at 300 K cells x 10 000
-// permutations (2 regions, tools/apply_time.py cfg5) it takes 111.1 ms against the list replay's 83.6 ms: its apply is the
-// slower one there (64.5 against 45.5 ms), and its target generation, bound to fewer resident warps by the block buffers,
-// takes 24.0 against 14.6 ms.  Hence the size gate.
-static int part_replay_threads(const sqb_nhood* h, int64_t np) {
+struct PartShape {
+    int nt = 0;      // threads per CTA; 0: the region replay does not run
+    int per_sm = 0;  // resident CTAs per SM
+    int cap = 0;     // positions per region: sets the layout of J and of the count rows that the target generation writes
+};
+
+// dynamic shared memory beyond 48 KB and the largest shared-memory carveout for the region replay's kernel
+template <typename LT, int NT>
+static int part_apply_attributes(size_t smem) {
+    auto k = nhood_apply_part_kernel<LT, NT>;
+    SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    return SQB_OK;
+}
+
+// Shape of the region replay over partitioned targets (shuffle_algo 9) for np permutations; nt = 0 when it does not run.  It
+// runs when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that
+// every segment fits SQB_PART_RMAX regions and its step blocks fit one thread each; otherwise the list replay (algo 7) runs.
+// Its 32 warps spend much of a window waiting at the window's three block barriers, so the first choice is two resident
+// 512-thread CTAs per SM, each with half of the SM's shared memory (1M u8 labels: 13 regions of 76 928 positions).  When a
+// segment does not fit that (u16 labels at 1M, arrays above ~1.05M) or two such CTAs do not fit an SM, one 1024-thread CTA
+// per SM takes a block's opt-in limit (1M u8 labels: 7 regions).  shuffle_threads = 1024 with shuffle_algo 9 asks for the
+// latter.  Measured on an H100 80GB HBM3 (700 W power limit), tools/apply_time.py, 1M spots x 1000 permutations: the apply
+// takes 18.4-18.5 ms with two CTAs per SM against 19.8-19.9 ms with one 1024-thread CTA per SM, and 30.9 ms with the same 13
+// regions but one 512-thread CTA per SM.  At 300 K cells x 10 000 permutations (tools/apply_time.py cfg5) algo 9 still loses
+// to the list replay, so auto keeps the latter below 512 K elements (DESIGN.md §3.1).
+template <typename LT>
+static int part_replay_shape(const sqb_nhood* h, int64_t np, PartShape* out) {
     sqb_ctx* c = h->ctx;
-    int nt = 0;
-    if (h->shuffle_algo == 9) nt = h->shuffle_threads == 512 ? 512 : 1024;
-    else if (h->shuffle_algo < 0 && np > 2 * (int64_t)c->sm_count && h->n >= 524288) nt = 1024;
-    if (nt == 0) return 0;
-    const size_t tables = part_tables_bytes(nt, h->lt_bytes);
-    if (tables + 16 * (size_t)h->lt_bytes > c->smem_optin) return 0;
-    const int cap = (int)part_region_cap(h, nt);
-    for (int64_t m : h->h_seg_len) {
-        int R, B;
-        sqb_part_regions((int)m, cap, R, B);
-        if (R > SQB_PART_RMAX || (m + SQB_PART_L - 1) / SQB_PART_L > nt) return 0;
+    *out = PartShape{};
+    if (h->shuffle_algo != 9 && !(h->shuffle_algo < 0 && np > 2 * (int64_t)c->sm_count && h->n >= 524288)) return SQB_OK;
+    const auto fits = [&](int nt, int cap) {
+        if (cap == 0) return false;
+        for (int64_t m : h->h_seg_len) {
+            int R, B;
+            sqb_part_regions((int)m, cap, R, B);
+            if (R > SQB_PART_RMAX || (m + SQB_PART_L - 1) / SQB_PART_L > nt) return false;
+        }
+        return true;
+    };
+    if (!(h->shuffle_algo == 9 && h->shuffle_threads == 1024)) {
+        const int cap = (int)part_region_cap(h, 512, 2);
+        if (fits(512, cap)) {
+            const size_t smem = part_tables_bytes(512, (int)sizeof(LT)) + (size_t)cap * sizeof(LT);
+            SQB_TRY((part_apply_attributes<LT, 512>(smem)));
+            int per_sm = 0;
+            SQB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nhood_apply_part_kernel<LT, 512>, 512, smem));
+            if (per_sm >= 2) {
+                *out = PartShape{512, 2, cap};
+                return SQB_OK;
+            }
+        }
     }
-    return nt;
+    const int cap = (int)part_region_cap(h, 1024, 1);
+    if (fits(1024, cap)) *out = PartShape{1024, 1, cap};
+    return SQB_OK;
 }
 
 template <typename LT, int NT>
-static int launch_apply_part(sqb_nhood* h, LT* lab, const uint32_t* J, const uint16_t* cnt, int64_t nb_total, int cap, int64_t np) {
+static int launch_apply_part(sqb_nhood* h, LT* lab, const uint32_t* J, const uint16_t* cnt, int64_t nb_total, const PartShape& ps,
+                             int64_t np) {
     sqb_ctx* c = h->ctx;
-    auto k = nhood_apply_part_kernel<LT, NT>;
-    const size_t smem = part_tables_bytes(NT, (int)sizeof(LT)) + (size_t)cap * sizeof(LT);
-    SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = part_tables_bytes(NT, (int)sizeof(LT)) + (size_t)ps.cap * sizeof(LT);
+    SQB_TRY((part_apply_attributes<LT, NT>(smem)));
     int64_t grid = h->shuffle_ctas;
-    if (grid <= 0) grid = c->sm_count;  // one CTA per SM (launch bounds), persistent over the permutations
+    if (grid <= 0) grid = (int64_t)ps.per_sm * c->sm_count;  // every CTA resident, persistent over the permutations
     if (grid > np) grid = np;
-    k<<<(unsigned)grid, NT, smem, c->stream>>>(lab, J, cnt, reinterpret_cast<const LT*>(h->d_base.p), h->stride, np, h->nseg,
-                                               h->d_seg_start.p, h->d_seg_len.p, nb_total, cap);
+    nhood_apply_part_kernel<LT, NT><<<(unsigned)grid, NT, smem, c->stream>>>(
+        lab, J, cnt, reinterpret_cast<const LT*>(h->d_base.p), h->stride, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, nb_total,
+        ps.cap);
     return SQB_OK;
 }
 
 // shuffle_algo 9: partitioned swap targets + region replay (the label rows are not filled: the replay reads the base labels)
 template <typename LT>
-static int launch_shuffle_part(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, int nt) {
+static int launch_shuffle_part(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, const PartShape& ps) {
     sqb_ctx* c = h->ctx;
     int64_t nb_total = 0;
     for (int64_t m : h->h_seg_len) nb_total += (m + SQB_PART_L - 1) / SQB_PART_L;
@@ -3998,11 +4036,10 @@ static int launch_shuffle_part(sqb_nhood* h, LT* lab, const uint64_t* states, in
     SQB_TRY(c->scratch[3].alloc((size_t)np * nb_total * SQB_PART_RMAX * sizeof(uint16_t)));
     uint32_t* J = reinterpret_cast<uint32_t*>(c->scratch[2].p);
     uint16_t* cnt = reinterpret_cast<uint16_t*>(c->scratch[3].p);
-    const int cap = (int)part_region_cap(h, nt);
-    SQB_TRY(launch_jgen<true>(h, J, states, np, cnt, nb_total, cap));
+    SQB_TRY(launch_jgen<true>(h, J, states, np, cnt, nb_total, ps.cap));
     SqbLaunchScope scope(c, SQB_K_NHOOD_SHUFFLE);
-    if (nt == 512) SQB_TRY((launch_apply_part<LT, 512>(h, lab, J, cnt, nb_total, cap, np)));
-    else SQB_TRY((launch_apply_part<LT, 1024>(h, lab, J, cnt, nb_total, cap, np)));
+    if (ps.nt == 512) SQB_TRY((launch_apply_part<LT, 512>(h, lab, J, cnt, nb_total, ps, np)));
+    else SQB_TRY((launch_apply_part<LT, 1024>(h, lab, J, cnt, nb_total, ps, np)));
     SQB_POST_LAUNCH();
     return SQB_OK;
 }
@@ -4063,9 +4100,9 @@ static int launch_shuffle_two_kernel(sqb_nhood* h, LT* lab, const uint64_t* stat
 }
 
 template <typename LT>
-static int launch_shuffle(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np) {
+static int launch_shuffle(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, const PartShape& ps) {
     sqb_ctx* c = h->ctx;
-    if (const int nt = part_replay_threads(h, np)) return launch_shuffle_part<LT>(h, lab, states, np, nt);
+    if (ps.nt) return launch_shuffle_part<LT>(h, lab, states, np, ps);
     if (h->shuffle_algo == 5 || h->shuffle_algo == 7 || h->shuffle_algo == 8)
         return launch_shuffle_two_kernel<LT>(h, lab, states, np, h->shuffle_algo, h->shuffle_threads, h->shuffle_r, h->shuffle_low,
                                              (uint64_t)h->shuffle_stagger_us * 1000ull);
@@ -4175,7 +4212,9 @@ static int run_chunk(sqb_nhood* h, int64_t p0, int64_t np, bool do_count) {
     LT* lab = reinterpret_cast<LT*>(c->scratch[0].p);
     LT* labT = reinterpret_cast<LT*>(c->scratch[1].p);
     const int64_t vec_per_row = h->stride * (int64_t)sizeof(LT) / 16;
-    if (!part_replay_threads(h, np)) {  // the partitioned region replay reads the base labels itself
+    PartShape ps;
+    SQB_TRY(part_replay_shape<LT>(h, np, &ps));
+    if (!ps.nt) {  // the partitioned region replay reads the base labels itself
         SqbLaunchScope scope(c, SQB_K_NHOOD_FILL);
         unsigned gx = (unsigned)ceil_div64(vec_per_row, 256 * 4);
         if (gx < 1) gx = 1;
@@ -4186,7 +4225,7 @@ static int run_chunk(sqb_nhood* h, int64_t p0, int64_t np, bool do_count) {
                                                                   vec_per_row, np);
         SQB_POST_LAUNCH();
     }
-    SQB_TRY(launch_shuffle<LT>(h, lab, h->d_states.p + p0 * 4, np));
+    SQB_TRY(launch_shuffle<LT>(h, lab, h->d_states.p + p0 * 4, np, ps));
     if (!do_count) return SQB_OK;
     const int PB = (int)(((np + 31) / 32) * 32);
     {

@@ -2713,7 +2713,48 @@ __global__ void __launch_bounds__(NT, 1) nhood_apply_region_kernel(LT* __restric
 //     resolved as in 2i (tests/emu_shuffle.py::_resolve_general_window): filter marks / targeter + owner lists / writes,
 //     three block barriers.  Nothing writes a region before its own pass and every top above it was written by its own
 //     region's pass, so the slab loads straight from the base labels and the label rows need no fill.
+//     Nothing global is waited for inside a window: a thread loads its J entries two windows ahead (its block index walks
+//     forward from the one of its slot one window back), decodes them one window ahead and copies that window's tops above
+//     the region into shared memory with cp.async, so the HBM latency of both overlaps a whole window.
 // ------------------------------------------------------------------------------------------------
+// Phase clocks of nhood_apply_part_kernel (test build only, tools/apply_phases.py): thread 0 of every CTA adds the clock64()
+// cycles since its previous mark to the phase's total, so the phases of a window add up to the window's time as warp 0 sees
+// it (a barrier's wait is the time warp 0 waits there for the slowest warp).  A load's latency lands in the phase that first
+// uses its value.  The last two counters count windows and region passes.
+enum SqbPartClk {
+    SQB_PCLK_ENTRY,     // the window's J entries: decode, slot -> block lookup, next J loads issued
+    SQB_PCLK_GATHER,    // original values of the slots' targets and tops (slab; tops above the region from global memory)
+    SQB_PCLK_A,         // phase A: stage originals and tops, filter marks
+    SQB_PCLK_BAR1,      // first barrier
+    SQB_PCLK_B,         // phase B: table registrations
+    SQB_PCLK_BAR2,      // second barrier
+    SQB_PCLK_C,         // phase C: writes
+    SQB_PCLK_BAR3,      // third barrier
+    SQB_PCLK_CLEAR,     // table clear
+    SQB_PCLK_REGION,    // per region: slab load, run scan, first entries, slab store
+    SQB_PCLK_WINDOWS,   // count
+    SQB_PCLK_REGIONS,   // count
+    SQB_PCLK_N
+};
+#ifdef SQB_PART_CLOCKS
+__device__ unsigned long long g_part_clk[SQB_PCLK_N];
+#define SQB_PCLK_START() long long pclk_t = clock64()
+#define SQB_PCLK(ph)                                                                  \
+    do {                                                                              \
+        if (tid == 0) {                                                               \
+            const long long t_ = clock64();                                           \
+            atomicAdd(&g_part_clk[ph], (unsigned long long)(t_ - pclk_t));            \
+            pclk_t = t_;                                                              \
+        }                                                                             \
+    } while (0)
+#define SQB_PCLK_COUNT(ph) \
+    if (tid == 0) atomicAdd(&g_part_clk[ph], 1ull)
+#else
+#define SQB_PCLK_START()
+#define SQB_PCLK(ph)
+#define SQB_PCLK_COUNT(ph)
+#endif
+
 template <typename LT, int NT>
 __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __restrict__ labels, const uint32_t* __restrict__ J,
                                                                          const uint16_t* __restrict__ cnt,
@@ -2739,12 +2780,14 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                                                                                             // (+ 4: the slab stays 16-byte aligned)
     int* s_wsum = s_bslot + NT;                                                             // [32] scan partials
     uint16_t* s_next = reinterpret_cast<uint16_t*>(s_wsum + 32);                            // [HS] list links
-    LT* s_otop = reinterpret_cast<LT*>(s_next + HS);                                        // [HS] original top values
+    uint32_t* s_gath = reinterpret_cast<uint32_t*>(s_next + HS);                            // [HS] next window's tops above
+    LT* s_otop = reinterpret_cast<LT*>(s_gath + HS);                                        // [HS] original top values
     LT* s_slab = s_otop + HS;                                                               // [region_cap] the region
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int h = tid; h < 2 * HS; h += NT) s_tabT[h] = SQB_EMPTY64;  // both tables
     for (int w = tid; w < NWB; w += NT) s_bits[w] = 0u;
     __syncthreads();
+    SQB_PCLK_START();
 
     auto mark_pos = [&](uint32_t pl) {
         const uint32_t sh = (pl & 15u) * 2u;
@@ -2869,44 +2912,80 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                 }
                 __syncthreads();
                 const int total = s_bpref[nblk];
-                // entry of window slot g: binary search for its block (the largest t with s_bpref[t] <= g)
-                auto load_entry = [&](int g, int& top, uint32_t& jl) {
-                    int tl = 0, th = nblk;
-                    while (th - tl > 1) {
-                        const int mid = (tl + th) >> 1;
-                        if (s_bpref[mid] <= g) tl = mid;
-                        else th = mid;
-                    }
-                    const uint32_t e = __ldcs(Jb + s_bslot[tl] + (g - s_bpref[tl]));
-                    top = (bt - tl) * L + (int)(e >> 18);
-                    jl = e & 0x3FFFFu;
+                // Window slot g holds the entry at offset g - s_bpref[t] of block t's run, t = the largest t with
+                // s_bpref[t] <= g (never a block with an empty run).  A thread's slot of the next window, g + HS, lies in
+                // the same block or a later one, so the thread walks its block index forward from the last one it used.
+                auto block_of = [&](int g, int t) {
+                    while (s_bpref[t + 1] <= g) ++t;
+                    return t;
                 };
-                int ntop[2];
-                uint32_t njl[2];
+                auto entry = [&](int g, int t) { return __ldcs(Jb + s_bslot[t] + (g - s_bpref[t])); };
+                // T(i) of a top above the region, left there by the pass of i's own region and not written again before its
+                // own step: copied one window ahead into the thread's word of s_gath (the aligned 4 bytes that hold it)
+                auto gather_top = [&](int s, int i) {
+                    const uintptr_t a = reinterpret_cast<uintptr_t>(a0 + i) & ~(uintptr_t)3;
+                    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(s_gath + s)),
+                                 "l"(a)
+                                 : "memory");
+                };
+                auto gathered = [&](int s, int i) -> LT {
+                    return (LT)(s_gath[s] >> (8u * (unsigned)(reinterpret_cast<uintptr_t>(a0 + i) & 3u)));
+                };
+                // per slot k of the thread: the window's decoded entry (top, jl); the next window's raw entry jn and its block jb
+                int top[2], jb[2];
+                uint32_t jl[2], jn[2];
 #pragma unroll
                 for (int k = 0; k < 2; ++k) {
-                    ntop[k] = -1, njl[k] = 0;
-                    if (tid + k * NT < total) load_entry(tid + k * NT, ntop[k], njl[k]);
+                    const int s = tid + k * NT;
+                    top[k] = -1, jl[k] = 0, jb[k] = 0, jn[k] = 0;
+                    if (s < total) {
+                        jb[k] = block_of(s, 0);
+                        const uint32_t e = entry(s, jb[k]);
+                        top[k] = (bt - jb[k]) * L + (int)(e >> 18);
+                        jl[k] = e & 0x3FFFFu;
+                        if (top[k] >= hi) gather_top(s, top[k]);
+                    }
+                    if (s + HS < total) {
+                        jb[k] = block_of(s + HS, jb[k]);
+                        jn[k] = entry(s + HS, jb[k]);
+                    }
                 }
+                asm volatile("cp.async.commit_group;" ::: "memory");
+                SQB_PCLK(SQB_PCLK_REGION);
                 for (int w0 = 0; w0 < total; w0 += HS) {
-                    int top[2];
-                    uint32_t jl[2];
                     LT vt[2], vj[2];
+                    asm volatile("cp.async.wait_all;" ::: "memory");  // this thread's gathers for this window
 #pragma unroll
-                    for (int k = 0; k < 2; ++k) {  // originals first (the tops above the region come from global memory)
-                        top[k] = ntop[k], jl[k] = njl[k];
+                    for (int k = 0; k < 2; ++k) {  // originals
                         vt[k] = (LT)0, vj[k] = (LT)0;
                         if (top[k] >= 0) {
+                            const int s = tid + k * NT;
                             vj[k] = s_slab[jl[k]];
-                            vt[k] = (top[k] < hi) ? s_slab[top[k] - lo] : ld_cg<LT>(a0 + top[k]);  // T(i): left there by the pass of i's own region
+                            vt[k] = (top[k] < hi) ? s_slab[top[k] - lo] : gathered(s, top[k]);
                         }
                     }
+                    SQB_PCLK(SQB_PCLK_GATHER);
+                    // the next window: decode its entries (loaded one window ago), gather its tops above the region, load
+                    // the entries of the window after it
+                    int ntop[2];
+                    uint32_t njl[2];
 #pragma unroll
                     for (int k = 0; k < 2; ++k) {
+                        const int s = tid + k * NT;
+                        const int g = w0 + HS + s;
                         ntop[k] = -1, njl[k] = 0;
-                        const int g = w0 + HS + tid + k * NT;
-                        if (g < total) load_entry(g, ntop[k], njl[k]);  // the next window's entries
+                        if (g < total) {
+                            ntop[k] = (bt - jb[k]) * L + (int)(jn[k] >> 18);
+                            njl[k] = jn[k] & 0x3FFFFu;
+                            if (ntop[k] >= hi) gather_top(s, ntop[k]);
+                            if (g + HS < total) {
+                                jb[k] = block_of(g + HS, jb[k]);
+                                jn[k] = entry(g + HS, jb[k]);
+                            }
+                        }
                     }
+                    asm volatile("cp.async.commit_group;" ::: "memory");
+                    SQB_PCLK(SQB_PCLK_ENTRY);
                     // ---- A: stage originals and tops, filter marks ----
 #pragma unroll
                     for (int k = 0; k < 2; ++k) {
@@ -2918,8 +2997,10 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                             if (top[k] < hi) mark_pos((uint32_t)(top[k] - lo));
                         }
                     }
+                    SQB_PCLK(SQB_PCLK_A);
                     SQB_CONVERGE();
                     __syncthreads();
+                    SQB_PCLK(SQB_PCLK_BAR1);
                     // ---- B: slots on multiply-marked positions register in the tables ----
                     uint32_t slotT[2] = {0, 0}, slotO[2] = {0, 0};
                     bool stfl[2], sofl[2], sself[2];
@@ -2936,8 +3017,10 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                             if (sofl[k]) slotO[k] = insert_owner((uint32_t)(top[k] - lo), s);
                         }
                     }
+                    SQB_PCLK(SQB_PCLK_B);
                     SQB_CONVERGE();
                     __syncthreads();
+                    SQB_PCLK(SQB_PCLK_BAR2);
                     // ---- C: writes, from the (now immutable) lists and original values only ----
                     {
                         uint4* bz = reinterpret_cast<uint4*>(s_bits);  // nobody reads the filter any more
@@ -2983,14 +3066,20 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                         if (top[k] < hi) s_slab[top[k] - lo] = val;
                         else st_cs<LT>(a0 + top[k], val);  // final
                     }
+                    SQB_PCLK(SQB_PCLK_C);
                     SQB_CONVERGE();
                     __syncthreads();
+                    SQB_PCLK(SQB_PCLK_BAR3);
                     // ---- the table entries of this window are cleared (ordered before the next pushes by its first barrier) ----
 #pragma unroll
                     for (int k = 0; k < 2; ++k) {
                         if (stfl[k] && !sself[k]) s_tabT[slotT[k]] = SQB_EMPTY64;
                         if (sofl[k]) s_tabO[slotO[k]] = SQB_EMPTY64;
                     }
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) top[k] = ntop[k], jl[k] = njl[k];
+                    SQB_PCLK(SQB_PCLK_CLEAR);
+                    SQB_PCLK_COUNT(SQB_PCLK_WINDOWS);
                 }
                 __syncthreads();
                 {  // a[lo, hi) <- slab
@@ -3007,6 +3096,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                     for (int x = x0 + tid; x < len; x += NT) dst[x] = s_slab[x];
                 }
                 __syncthreads();
+                SQB_PCLK(SQB_PCLK_REGION);
+                SQB_PCLK_COUNT(SQB_PCLK_REGIONS);
             }
         }
     }
@@ -3934,10 +4025,11 @@ static int launch_jgen(sqb_nhood* h, uint32_t* J, const uint64_t* states, int64_
 }
 
 // shared memory of nhood_apply_part_kernel besides the slab:
-// [tabT, tabO u64 x HS][bits u32 x 2 HS][top int x HS][bpref int x NT + 4][bslot int x NT][wsum int x 32][next u16 x HS][otop LT x HS]
+// [tabT, tabO u64 x HS][bits u32 x 2 HS][top int x HS][bpref int x NT + 4][bslot int x NT][wsum int x 32][next u16 x HS]
+// [gath u32 x HS][otop LT x HS]
 static size_t part_tables_bytes(int nt, int lt_bytes) {
     const size_t HS = 2 * (size_t)nt;
-    return 2 * HS * 8 + 2 * HS * 4 + HS * 4 + (2 * (size_t)nt + 4) * 4 + 32 * 4 + HS * 2 + HS * lt_bytes;
+    return 2 * HS * 8 + 2 * HS * 4 + HS * 4 + (2 * (size_t)nt + 4) * 4 + 32 * 4 + HS * 2 + HS * 4 + HS * lt_bytes;
 }
 
 // positions per region of shuffle_algo 9 with nt threads and per_sm resident CTAs per SM (a multiple of 16; 0 = not even 16
@@ -3972,13 +4064,15 @@ static int part_apply_attributes(size_t smem) {
 // runs when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that
 // every segment fits SQB_PART_RMAX regions and its step blocks fit one thread each; otherwise the list replay (algo 7) runs.
 // Its 32 warps spend much of a window waiting at the window's three block barriers, so the first choice is two resident
-// 512-thread CTAs per SM, each with half of the SM's shared memory (1M u8 labels: 13 regions of 76 928 positions).  When a
+// 512-thread CTAs per SM, each with half of the SM's shared memory (1M u8 labels: 14 regions of 71 440 positions).  When a
 // segment does not fit that (u16 labels at 1M, arrays above ~1.05M) or two such CTAs do not fit an SM, one 1024-thread CTA
 // per SM takes a block's opt-in limit (1M u8 labels: 7 regions).  shuffle_threads = 1024 with shuffle_algo 9 asks for the
-// latter.  Measured on an H100 80GB HBM3 (700 W power limit), tools/apply_time.py, 1M spots x 1000 permutations: the apply
-// takes 18.4-18.5 ms with two CTAs per SM against 19.8-19.9 ms with one 1024-thread CTA per SM, and 30.9 ms with the same 13
-// regions but one 512-thread CTA per SM.  At 300 K cells x 10 000 permutations (tools/apply_time.py cfg5) algo 9 still loses
-// to the list replay, so auto keeps the latter below 512 K elements (DESIGN.md §3.1).
+// latter.  Measured on an H100 80GB HBM3 (700 W power limit), tools/apply_time.py, 1M spots x 1000 permutations, before the
+// window loop stopped waiting on global memory: the apply took 18.4-18.5 ms with two CTAs per SM against 19.8-19.9 ms with
+// one 1024-thread CTA per SM, and 30.9 ms with 13 regions but one 512-thread CTA per SM.  At 300 K cells x 10 000
+// permutations (tools/apply_time.py cfg5, H100 80GB HBM3, 400 W power limit) algo 9 takes 92.5 ms against 84.2 ms for auto
+// (list replay): its apply now ties (46.2 against 46.0 ms) but its target generation costs 9 ms more, so auto keeps the list
+// replay below 512 K elements (DESIGN.md §3.1).
 template <typename LT>
 static int part_replay_shape(const sqb_nhood* h, int64_t np, PartShape* out) {
     sqb_ctx* c = h->ctx;
@@ -5090,6 +5184,19 @@ int sqb_nhood_permute_var_chain_dev(sqb_nhood* h, const double* d_mean, const do
     SQB_POST_LAUNCH();
     return SQB_OK;
 }
+
+#ifdef SQB_PART_CLOCKS
+// test build only: copies the SQB_PCLK_N phase-clock totals of nhood_apply_part_kernel to out (when out is not null), then
+// zeroes them when reset is set
+int sqb_test_part_clocks(unsigned long long* out, int reset) {
+    if (out) SQB_CUDA(cudaMemcpyFromSymbol(out, g_part_clk, sizeof(g_part_clk)));
+    if (reset) {
+        const unsigned long long zero[SQB_PCLK_N] = {};
+        SQB_CUDA(cudaMemcpyToSymbol(g_part_clk, zero, sizeof(g_part_clk)));
+    }
+    return SQB_OK;
+}
+#endif
 
 }  // extern "C"
 

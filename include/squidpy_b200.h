@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 3
+#define SQB_ABI_VERSION 4
 
 typedef enum {
     SQB_OK = 0,
@@ -72,6 +72,9 @@ int sqb_ctx_profile_get(sqb_ctx* ctx, int kclass, double* ms, int64_t* launches)
 /* page-locked host memory for the host-facing API (so H2D/D2H copies run at full PCIe rate) */
 int sqb_host_alloc(size_t bytes, void** ptr);
 int sqb_host_free(void* ptr);
+
+/* *device = the CUDA device ordinal that owns p (device or managed memory), or -1 for host / unregistered memory. */
+int sqb_pointer_device(const void* p, int* device);
 
 /* ---- nhood_enrichment ------------------------------------------------------------------------------
  * Graph = CSR of obsp['spatial_connectivities'] (data ignored; entries counted as stored; reference dtypes
@@ -201,6 +204,30 @@ int sqb_autocorr_load_csr(sqb_autocorr* h, const int64_t* x_indptr, const int32_
  * as features 0 .. col_hi - col_lo.                                                                          */
 int sqb_autocorr_load_csr_cols(sqb_autocorr* h, const int64_t* x_indptr, const int32_t* x_indices, const void* x_data,
                                int x_dtype, int64_t n_features_total, int64_t col_lo, int64_t col_hi);
+/* Device-resident X (e.g. a cupy / torch array of the caller).  indptr, indices, data and x are DEVICE pointers on the
+ * context's device; everything else is on the host.
+ *   col_map (host, int32, one entry per input feature): the feature's index in [0, n_out) among the loaded features, or -1
+ *           to skip it; every output index must occur exactly once.  One map expresses a gene subset in any order, a mask
+ *           and a multi-GPU shard.
+ *   data_dtype / x_dtype: 0 = f32, 1 = f64, 2 = f16, 3 = int32, 4 = int64.  f32 is loaded as f32, every other type is
+ *           converted to f64 on the device (what the host path does on the host).
+ *   producer_stream: the CUDA Array Interface v3 `stream` of the arrays: 0 = none, 1 = legacy default stream, 2 = per-thread
+ *           default stream, else a cudaStream_t.  The context's stream waits on an event recorded there before it reads X.
+ *   Both calls return after the device has finished reading the caller's buffers: the caller may then free or overwrite them.
+ *   The library never writes caller memory.
+ * CSR: indptr_bits / index_bits 32 or 64; layout as in sqb_autocorr_load_csr (1 = observations x features, AnnData's CSR X;
+ *   0 = features x observations, AnnData's CSC X); n_cols = number of input features.  Indices need not be sorted.  Index
+ *   ranges, indptr monotonicity (checked before anything follows indptr) and duplicates are validated on the device
+ *   (SQB_ERR_INVALID).  The matrix is read in place: no staging copy; the extra device memory is the relaid-out copy of the
+ *   selected features plus one transposition buffer of their entries (layout 1).
+ * Dense: x is rows x cols with element strides stride_row / stride_col (C order, F order or a strided view; any sign);
+ *   layout 1: rows = observations, 0: rows = features.  The selected features are gathered into the layout
+ *   sqb_autocorr_load_dense produces for that layout.                                                          */
+int sqb_autocorr_load_csr_device(sqb_autocorr* h, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                                 const void* data, int data_dtype, int layout, int64_t n_cols, const int32_t* col_map, int64_t n_out,
+                                 uintptr_t producer_stream);
+int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, int64_t rows, int64_t cols, int64_t stride_row,
+                                   int64_t stride_col, int layout, const int32_t* col_map, int64_t n_out, uintptr_t producer_stream);
 int sqb_autocorr_run_async(sqb_autocorr* h, int mode, const int64_t* row_perm);
 int sqb_autocorr_download(sqb_autocorr* h, double* out);
 /* The permutation variant in one call (_score_helper, _ppatterns.py:258-280): row_perms = n_perms x n int64 (row p is

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (the test suite points it at the build that also contains the superseded
 # replay variants, tests/native/libsquidpy_b200_testvariants.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -48,6 +48,7 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_ctx_profile_get": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     "sqb_host_alloc": (C.c_int, [C.c_size_t, c_void_pp]),
     "sqb_host_free": (C.c_int, [C.c_void_p]),
+    "sqb_pointer_device": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
     "sqb_nhood_create": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, c_void_pp]),
     "sqb_nhood_destroy": (C.c_int, [C.c_void_p]),
     "sqb_nhood_count": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -75,6 +76,10 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_autocorr_load_dense": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64]),
     "sqb_autocorr_load_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64]),
     "sqb_autocorr_load_csr_cols": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64]),
+    "sqb_autocorr_load_csr_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64,
+                                                C.c_void_p, C.c_int64, C.c_size_t]),
+    "sqb_autocorr_load_dense_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                                  C.c_int64, C.c_size_t]),
     "sqb_autocorr_run_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "sqb_autocorr_download": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sqb_autocorr_run_perms": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
@@ -142,6 +147,13 @@ def check(rc: int, exc: type[Exception] | None = None) -> None:
     if rc == -4:
         raise NotImplementedError(msg)
     raise SquidpyB200Error(f"[status {rc}] {msg}")
+
+
+def pointer_device(ptr: int) -> int:
+    """CUDA device ordinal owning the address ``ptr`` (device or managed memory), or -1 for host memory."""
+    d = C.c_int(-1)
+    check(load().sqb_pointer_device(C.c_void_p(ptr), C.byref(d)))
+    return d.value
 
 
 def device_count() -> int:

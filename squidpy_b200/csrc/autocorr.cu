@@ -29,6 +29,7 @@
 //   tile, W streamed once per tile.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cuda_fp16.h>
 
 #include <stdlib.h>
 
@@ -196,17 +197,49 @@ __global__ void __launch_bounds__(256) ac_final_kernel(const double* __restrict_
 enum { AC_ERR_INDEX = 1, AC_ERR_DUP = 2, AC_ERR_INDPTR = 4, AC_ERR_PERM = 8 };
 
 // ---- input validation / transposition (load time) ----------------------------------------------------
+// Value conversion of the caller's data type to the device layout's (float16 goes through float32: exact)
+template <typename XT, typename VT>
+struct AcCvt {
+    __device__ __forceinline__ static XT f(VT v) { return (XT)v; }
+};
+template <typename XT>
+struct AcCvt<XT, __half> {
+    __device__ __forceinline__ static XT f(__half v) { return (XT)__half2float(v); }
+};
+
 // indptr must start at 0, be non-decreasing and end at nnz
-__global__ void ac_check_indptr_kernel(const int64_t* __restrict__ ptr, int64_t rows, int64_t nnz, int* __restrict__ err) {
+template <typename IP>
+__global__ void ac_check_indptr_kernel(const IP* __restrict__ ptr, int64_t rows, int64_t nnz, int* __restrict__ err) {
     for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t a = ptr[r], b = ptr[r + 1];
+        const int64_t a = (int64_t)ptr[r], b = (int64_t)ptr[r + 1];
         if (a > b || a < 0 || b > nnz || (r == 0 && a != 0)) atomicOr(err, AC_ERR_INDPTR);
     }
 }
 
+// Output feature of input column c, or -1 to skip it (range errors raise *err unless err is null).  colmap == null: the shard [col_lo, col_lo + n_feat) of the columns,
+// anything outside is an error; else colmap[c] for c in [0, n_cols).
+__device__ __forceinline__ int64_t ac_map_col(int64_t c, int64_t n_feat, int32_t col_lo, const int32_t* __restrict__ colmap,
+                                              int64_t n_cols, int* __restrict__ err) {
+    if (colmap) {
+        if (c < 0 || c >= n_cols) {
+            if (err) atomicOr(err, AC_ERR_INDEX);
+            return -1;
+        }
+        return colmap[c];
+    }
+    c -= col_lo;
+    if (c < 0 || c >= n_feat) {
+        if (err) atomicOr(err, AC_ERR_INDEX);
+        return -1;
+    }
+    return c;
+}
+
 // per-column entry counts of a CSR-by-observation matrix; out-of-range column -> error flag.
 // Shared-memory histogram per CTA when n_feat fits (hist_smem), else global atomics.
-__global__ void ac_colcount_kernel(const int32_t* __restrict__ xi, int64_t nnz, int64_t n_feat, int32_t col_lo, int hist_smem,
+template <typename II>
+__global__ void ac_colcount_kernel(const II* __restrict__ xi, int64_t nnz, int64_t n_feat, int32_t col_lo,
+                                   const int32_t* __restrict__ colmap, int64_t n_cols, int hist_smem,
                                    unsigned int* __restrict__ cnt, int* __restrict__ err) {
     extern __shared__ unsigned int s_hist[];
     if (hist_smem)
@@ -215,11 +248,8 @@ __global__ void ac_colcount_kernel(const int32_t* __restrict__ xi, int64_t nnz, 
     const int64_t per = (nnz + gridDim.x - 1) / gridDim.x;
     const int64_t e0 = blockIdx.x * per, e1 = e0 + per < nnz ? e0 + per : nnz;
     for (int64_t e = e0 + threadIdx.x; e < e1; e += blockDim.x) {
-        const int32_t c = xi[e] - col_lo;
-        if (c < 0 || c >= n_feat) {
-            atomicOr(err, AC_ERR_INDEX);
-            continue;
-        }
+        const int64_t c = ac_map_col((int64_t)xi[e], n_feat, col_lo, colmap, n_cols, err);
+        if (c < 0) continue;
         if (hist_smem)
             atomicAdd(&s_hist[c], 1u);
         else
@@ -303,21 +333,54 @@ __global__ void ac_seglen_kernel(const int64_t* __restrict__ ptr, int64_t n_feat
     }
 }
 
+// segments of the selected features of a caller's CSR by feature: feature k is input row inv[k]
+template <typename IP>
+__global__ void ac_select_segs_kernel(const IP* __restrict__ ptr, const int32_t* __restrict__ inv, int64_t n_out,
+                                      int64_t* __restrict__ beg, int64_t* __restrict__ end, unsigned int* __restrict__ cnt,
+                                      int64_t n, int* __restrict__ err) {
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n_out; k += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t a = (int64_t)ptr[inv[k]], b = (int64_t)ptr[inv[k] + 1];  // validated non-decreasing
+        beg[k] = a;
+        end[k] = b;
+        int64_t d = b - a;
+        if (d > n) {
+            atomicOr(err, AC_ERR_DUP);
+            d = n;
+        }
+        cnt[k] = (unsigned int)d;
+    }
+}
+
 // CSR by observation -> unsorted segments by feature (atomic cursor; the rank sort below orders them)
-template <typename XT>
-__global__ void ac_coltranspose_kernel(const int64_t* __restrict__ xp, const int32_t* __restrict__ xi,
-                                       const XT* __restrict__ xv, int64_t n_obs, int64_t n_feat, int32_t col_lo,
+template <typename IP, typename II, typename VT, typename XT>
+__global__ void ac_coltranspose_kernel(const IP* __restrict__ xp, const II* __restrict__ xi,
+                                       const VT* __restrict__ xv, int64_t n_obs, int64_t n_feat, int32_t col_lo,
+                                       const int32_t* __restrict__ colmap, int64_t n_cols,
                                        unsigned long long* __restrict__ cursor, int32_t* __restrict__ oi, XT* __restrict__ ov) {
     const int lane = threadIdx.x & 31;
     const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; r < n_obs; r += nw) {
-        for (int64_t e = xp[r] + lane; e < xp[r + 1]; e += 32) {
-            const int32_t c = xi[e] - col_lo;
-            if (c < 0 || c >= n_feat) continue;  // flagged by the count kernel
+        const int64_t e1 = (int64_t)xp[r + 1];
+        for (int64_t e = (int64_t)xp[r] + lane; e < e1; e += 32) {
+            const int64_t c = ac_map_col((int64_t)xi[e], n_feat, col_lo, colmap, n_cols, nullptr);  // flagged by the count kernel
+            if (c < 0) continue;
             const unsigned long long pos = atomicAdd(&cursor[c], 1ULL);
             oi[pos] = (int32_t)r;
-            ov[pos] = xv[e];
+            ov[pos] = AcCvt<XT, VT>::f(xv[e]);
         }
+    }
+}
+
+// Dense gather of the selected features of a strided device array (element strides s_obs / s_feat, any sign) into the layout
+// sqb_autocorr_load_dense produces: obs_major = 1 -> [n_obs][n_out], 0 -> [n_out][n_obs]; feature k is input feature inv[k].
+template <typename VT, typename XT>
+__global__ void ac_gather_dense_kernel(const VT* __restrict__ x, int64_t n_obs, int64_t n_out, int64_t s_obs, int64_t s_feat,
+                                       const int32_t* __restrict__ inv, int obs_major, XT* __restrict__ out) {
+    const int64_t total = n_obs * n_out;
+    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = obs_major ? t / n_out : t % n_obs;
+        const int64_t k = obs_major ? t - r * n_out : t / n_obs;
+        out[t] = AcCvt<XT, VT>::f(x[r * s_obs + (int64_t)inv[k] * s_feat]);
     }
 }
 
@@ -369,10 +432,11 @@ __device__ __forceinline__ unsigned int ac_scan_words(uint2* S, int nwords, unsi
 
 // One CTA per feature: order the (observation, value) pairs of a segment by observation (rank = number of stored
 // observations below), write them to the padded segment, pad with index -1 / value 0.  Out-of-range or repeated
-// observation indices raise the error flag.
-template <typename XT>
-__global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __restrict__ in_ptr, const int32_t* __restrict__ in_idx,
-                                                             const XT* __restrict__ in_val, const int64_t* __restrict__ out_start,
+// observation indices raise the error flag.  Segment g is in_idx / in_val [in_beg[g], in_end[g]).
+template <typename II, typename VT, typename XT>
+__global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __restrict__ in_beg, const int64_t* __restrict__ in_end,
+                                                             const II* __restrict__ in_idx, const VT* __restrict__ in_val,
+                                                             const int64_t* __restrict__ out_start,
                                                              int32_t* __restrict__ out_idx, XT* __restrict__ out_val,
                                                              int32_t* __restrict__ seg_len, int64_t n, int64_t n_feat,
                                                              int nwords, uint2* __restrict__ s_global, int* __restrict__ err) {
@@ -382,14 +446,17 @@ __global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __res
     ac_zero_words(S, nwords);
     __syncthreads();
     for (int64_t g = blockIdx.x; g < n_feat; g += gridDim.x) {
-        const int64_t rb = in_ptr[g];
-        int64_t len64 = in_ptr[g + 1] - rb;
+        const int64_t rb = in_beg[g];
+        int64_t len64 = in_end[g] - rb;
         if (len64 < 0) len64 = 0;
-        if (len64 > n) len64 = n;  // flagged by ac_seglen_kernel
+        if (len64 > n) {  // more entries than observations: some observation repeats
+            if (threadIdx.x == 0) atomicOr(err, AC_ERR_DUP);
+            len64 = n;
+        }
         const int len = (int)len64;
         const int64_t os = out_start[g];
         for (int e = threadIdx.x; e < len; e += AC_T) {
-            const int32_t i = in_idx[rb + e];
+            const int64_t i = (int64_t)in_idx[rb + e];
             if (i < 0 || i >= n) {
                 atomicOr(err, AC_ERR_INDEX);
                 continue;
@@ -400,13 +467,13 @@ __global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __res
         __syncthreads();
         ac_scan_words(S, nwords, s_tmp);
         for (int e = threadIdx.x; e < len; e += AC_T) {
-            const int32_t i = in_idx[rb + e];
+            const int64_t i = (int64_t)in_idx[rb + e];
             if (i < 0 || i >= n) continue;
             const uint2 s = S[i >> 5];
             const unsigned int bit = 1u << (i & 31);
             const int64_t pos = os + s.y + __popc(s.x & (bit - 1u));
-            out_idx[pos] = i;
-            out_val[pos] = in_val[rb + e];
+            out_idx[pos] = (int32_t)i;
+            out_val[pos] = AcCvt<XT, VT>::f(in_val[rb + e]);
         }
         const int lenp = (len + 3) & ~3;
         for (int e = len + threadIdx.x; e < lenp; e += AC_T) {
@@ -1002,10 +1069,11 @@ static int ac_check_flags(sqb_autocorr* h, const char* where) {
     return SQB_OK;
 }
 
-// raw segments by feature (ptr / idx / val on the device, any order inside a segment) -> padded, ordered layout
-template <typename XT>
-static int ac_build_segments(sqb_autocorr* h, const int64_t* d_ptr, const unsigned int* d_cnt, int64_t* d_pad,
-                             const int32_t* d_idx, const XT* d_val, int64_t nnz, int64_t n_feat) {
+// raw segments by feature (segment g = [d_beg[g], d_end[g]) of idx / val on the device, any order inside a segment) ->
+// padded, ordered layout; nnz >= the entries of all segments
+template <typename II, typename VT, typename XT>
+static int ac_build_segments(sqb_autocorr* h, const int64_t* d_beg, const int64_t* d_end, const unsigned int* d_cnt, int64_t* d_pad,
+                             const II* d_idx, const VT* d_val, int64_t nnz, int64_t n_feat) {
     sqb_ctx* c = h->ctx;
     const int64_t cap = nnz + 4 * n_feat + 4;
     SQB_TRY(h->d_xi.alloc((size_t)cap));
@@ -1014,16 +1082,15 @@ static int ac_build_segments(sqb_autocorr* h, const int64_t* d_ptr, const unsign
     SQB_TRY(h->d_order.alloc((size_t)n_feat));
     SQB_TRY(h->d_aux.alloc((size_t)5 * n_feat));
     SQB_TRY(h->d_out.alloc((size_t)n_feat));
-    const void* kernel = (const void*)ac_rank_sort_kernel<XT>;
+    const void* kernel = (const void*)ac_rank_sort_kernel<II, VT, XT>;
     AcGeom geo;
     SQB_TRY(ac_geometry(h, kernel, &geo));
     int64_t ctas = geo.ctas < n_feat ? geo.ctas : n_feat;
     {
         SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_rank_sort_kernel<XT><<<(unsigned)ctas, AC_T, geo.smem, c->stream>>>(d_ptr, d_idx, d_val, d_pad, h->d_xi.p,
-                                                                             reinterpret_cast<XT*>(h->d_x.p), h->d_len.p, h->n,
-                                                                             n_feat, geo.nwords, geo.global ? h->d_bitmap.p : nullptr,
-                                                                             h->d_flags.p);
+        ac_rank_sort_kernel<II, VT, XT><<<(unsigned)ctas, AC_T, geo.smem, c->stream>>>(
+            d_beg, d_end, d_idx, d_val, d_pad, h->d_xi.p, reinterpret_cast<XT*>(h->d_x.p), h->d_len.p, h->n, n_feat, geo.nwords,
+            geo.global ? h->d_bitmap.p : nullptr, h->d_flags.p);
         SQB_POST_LAUNCH();
     }
     // features by decreasing length: the queue hands out the long ones first (LPT), the tail of the grid stays short
@@ -1115,7 +1182,12 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
     }
     {
         SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_check_indptr_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(r_ptr.p, rows, nnz, h->d_flags.p);
+        ac_check_indptr_kernel<int64_t><<<c->sm_count * 4, 256, 0, c->stream>>>(r_ptr.p, rows, nnz, h->d_flags.p);
+    }
+    // the kernels below follow indptr: a bad one must stop the load before they read or write outside [0, nnz)
+    if ((rc = ac_check_flags(h, "sqb_autocorr_load_csr"))) {
+        cleanup();
+        return rc;
     }
     const int64_t* seg_ptr;
     const int32_t* seg_idx;
@@ -1139,9 +1211,9 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
             const size_t hist_bytes = (size_t)n_feat * sizeof(unsigned int);
             const int hist_smem = hist_bytes <= 160 * 1024 ? 1 : 0;
             if (hist_smem && hist_bytes > 48 * 1024)
-                cudaFuncSetAttribute(ac_colcount_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_bytes);
-            ac_colcount_kernel<<<c->sm_count * (hist_smem ? 1 : 8), 1024, hist_smem ? hist_bytes : 0, c->stream>>>(r_idx.p, nnz, n_feat, col_lo,
-                                                                                                              hist_smem, cnt.p, h->d_flags.p);
+                cudaFuncSetAttribute(ac_colcount_kernel<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_bytes);
+            ac_colcount_kernel<int32_t><<<c->sm_count * (hist_smem ? 1 : 8), 1024, hist_smem ? hist_bytes : 0, c->stream>>>(
+                r_idx.p, nnz, n_feat, col_lo, nullptr, 0, hist_smem, cnt.p, h->d_flags.p);
         }
     }
     {
@@ -1152,20 +1224,167 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
     }
     if (layout != 0) {
         SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_coltranspose_kernel<XT><<<c->sm_count * 8, 256, 0, c->stream>>>(r_ptr.p, r_idx.p, reinterpret_cast<const XT*>(r_val.p), n, n_feat,
-                                                                           col_lo, cursor.p, t_idx.p, reinterpret_cast<XT*>(t_val.p));
+        ac_coltranspose_kernel<int64_t, int32_t, XT, XT><<<c->sm_count * 8, 256, 0, c->stream>>>(
+            r_ptr.p, r_idx.p, reinterpret_cast<const XT*>(r_val.p), n, n_feat, col_lo, nullptr, 0, cursor.p, t_idx.p,
+            reinterpret_cast<XT*>(t_val.p));
         seg_ptr = t_ptr.p;
         seg_idx = t_idx.p;
         seg_val = reinterpret_cast<const XT*>(t_val.p);
     }
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail(e);
-    rc = ac_build_segments<XT>(h, seg_ptr, cnt.p, pad.p, seg_idx, seg_val, nnz, n_feat);
+    rc = ac_build_segments<int32_t, XT, XT>(h, seg_ptr, seg_ptr + 1, cnt.p, pad.p, seg_idx, seg_val, nnz, n_feat);
     if (rc == SQB_OK) rc = ac_check_flags(h, "sqb_autocorr_load_csr");  // synchronises: the temporaries may go
     else cudaStreamSynchronize(c->stream);
     cleanup();
     h->x_nnz = nnz;
     return rc;
+}
+
+// ---- device-resident input (sqb_autocorr_load_*_device) ------------------------------------------------------------
+// Make the context's stream wait for the caller's producer stream (CUDA Array Interface v3 `stream`: 0 none, 1 legacy
+// default stream, 2 per-thread default stream, else a cudaStream_t).
+static int ac_wait_producer(sqb_ctx* c, uintptr_t producer) {
+    if (producer == 0) return SQB_OK;
+    cudaStream_t s = producer == 1 ? cudaStreamLegacy : producer == 2 ? cudaStreamPerThread : (cudaStream_t)producer;
+    if (s == c->stream) return SQB_OK;
+    cudaEvent_t ev;
+    SQB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    cudaError_t e = cudaEventRecord(ev, s);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->stream, ev, 0);
+    cudaEventDestroy(ev);  // released once the recorded work completes
+    SQB_CUDA(e);
+    return SQB_OK;
+}
+
+// col_map[f] in [0, n_out) or -1 for every input feature f; every output feature must come from exactly one input feature.
+// inv[k] = the input feature of output feature k.
+static int ac_invert_col_map(const int32_t* col_map, int64_t n_cols, int64_t n_out, std::vector<int32_t>& inv, const char* where) {
+    SQB_CHECK(n_cols >= 1 && n_cols < 2147483647LL && n_out >= 1 && n_out <= n_cols, SQB_ERR_INVALID,
+              "%s: n_out=%lld, n_cols=%lld out of range", where, (long long)n_out, (long long)n_cols);
+    inv.assign((size_t)n_out, -1);
+    for (int64_t f = 0; f < n_cols; ++f) {
+        const int32_t k = col_map[f];
+        if (k == -1) continue;
+        SQB_CHECK(k >= 0 && k < n_out && inv[k] < 0, SQB_ERR_INVALID, "%s: col_map[%lld] = %d is not -1 or an unused index in [0, %lld)",
+                  where, (long long)f, k, (long long)n_out);
+        inv[k] = (int32_t)f;
+    }
+    for (int64_t k = 0; k < n_out; ++k)
+        SQB_CHECK(inv[k] >= 0, SQB_ERR_INVALID, "%s: output feature %lld is not in col_map", where, (long long)k);
+    return SQB_OK;
+}
+
+// The caller's CSR (indptr IP, indices II, values VT, all in device memory) -> the padded layout by feature (values XT).
+// Nothing of the caller's is staged: the count / transposition / rank-sort kernels read it in place.  indptr is validated
+// (one synchronisation) before any kernel follows it, so no read leaves [0, nnz).
+template <typename IP, typename II, typename VT, typename XT>
+static int ac_load_csr_device_typed(sqb_autocorr* h, const IP* xp, const II* xi, const VT* xv, int layout, int64_t n_cols,
+                                    const int32_t* col_map, const std::vector<int32_t>& inv, int64_t n_out) {
+    static const char* where = "sqb_autocorr_load_csr_device";
+    sqb_ctx* c = h->ctx;
+    const int64_t n = h->n;
+    const int64_t rows = layout == 0 ? n_cols : n;
+    DevBuf<int32_t> map, t_idx;
+    DevBuf<XT> t_val;
+    DevBuf<int64_t> beg, end, t_ptr, pad;
+    DevBuf<unsigned int> cnt;
+    DevBuf<unsigned long long> cursor;
+    map.bind(c->stream), t_idx.bind(c->stream), t_val.bind(c->stream), beg.bind(c->stream), end.bind(c->stream);
+    t_ptr.bind(c->stream), pad.bind(c->stream), cnt.bind(c->stream), cursor.bind(c->stream);
+    int64_t sel = 0;
+    auto body = [&]() -> int {
+        SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream));
+        IP last = 0;
+        SQB_CUDA(cudaMemcpyAsync(&last, xp + rows, sizeof(IP), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        const int64_t nnz = (int64_t)last;
+        SQB_CHECK(nnz >= 0, SQB_ERR_INVALID, "%s: %s", where, ac_err_text(AC_ERR_INDPTR));
+        SQB_CHECK(nnz == 0 || (xi && xv), SQB_ERR_INVALID, "%s: null X arrays", where);
+        {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_check_indptr_kernel<IP><<<c->sm_count * 4, 256, 0, c->stream>>>(xp, rows, nnz, h->d_flags.p);
+            SQB_POST_LAUNCH();
+        }
+        SQB_TRY(ac_check_flags(h, where));
+        SQB_TRY(cnt.alloc(n_out + 1));
+        SQB_TRY(pad.alloc(n_out + 1));
+        SQB_TRY(t_ptr.alloc(n_out + 1));
+        if (layout == 0) {
+            SQB_TRY(map.alloc(n_out));
+            SQB_TRY(beg.alloc(n_out));
+            SQB_TRY(end.alloc(n_out));
+            SQB_CUDA(cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_select_segs_kernel<IP><<<c->sm_count * 2, 256, 0, c->stream>>>(xp, map.p, n_out, beg.p, end.p, cnt.p, n, h->d_flags.p);
+            SQB_POST_LAUNCH();
+        } else {
+            SQB_TRY(map.alloc(n_cols));
+            SQB_TRY(cursor.alloc(n_out + 1));
+            SQB_CUDA(cudaMemcpyAsync(map.p, col_map, n_cols * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+            SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_out + 1) * sizeof(unsigned int), c->stream));
+            if (nnz > 0) {
+                SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+                const size_t hist_bytes = (size_t)n_out * sizeof(unsigned int);
+                const int hist_smem = hist_bytes <= 160 * 1024 ? 1 : 0;
+                if (hist_smem && hist_bytes > 48 * 1024)
+                    SQB_CUDA(cudaFuncSetAttribute(ac_colcount_kernel<II>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_bytes));
+                ac_colcount_kernel<II><<<c->sm_count * (hist_smem ? 1 : 8), 1024, hist_smem ? hist_bytes : 0, c->stream>>>(
+                    xi, nnz, n_out, 0, map.p, n_cols, hist_smem, cnt.p, h->d_flags.p);
+                SQB_POST_LAUNCH();
+            }
+        }
+        {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_scan_counts_kernel<<<1, 1024, 0, c->stream>>>(cnt.p, n_out, t_ptr.p, pad.p, layout == 0 ? nullptr : cursor.p);
+            SQB_POST_LAUNCH();
+        }
+        // entries of the selected features: the relaid-out copy is sized by them, not by the whole matrix
+        SQB_CUDA(cudaMemcpyAsync(&sel, t_ptr.p + n_out, sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        if (layout == 0) return ac_build_segments<II, VT, XT>(h, beg.p, end.p, cnt.p, pad.p, xi, xv, sel, n_out);
+        SQB_TRY(t_idx.alloc(sel));
+        SQB_TRY(t_val.alloc(sel));
+        if (sel > 0) {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_coltranspose_kernel<IP, II, VT, XT><<<c->sm_count * 8, 256, 0, c->stream>>>(xp, xi, xv, n, n_out, 0, map.p, n_cols, cursor.p,
+                                                                                          t_idx.p, t_val.p);
+            SQB_POST_LAUNCH();
+        }
+        return ac_build_segments<int32_t, XT, XT>(h, t_ptr.p, t_ptr.p + 1, cnt.p, pad.p, t_idx.p, t_val.p, sel, n_out);
+    };
+    int rc = body();
+    if (rc == SQB_OK) rc = ac_check_flags(h, where);  // synchronises: the caller's buffers are no longer read
+    else cudaStreamSynchronize(c->stream);
+    map.release(), t_idx.release(), t_val.release(), beg.release(), end.release(), t_ptr.release(), pad.release(), cnt.release();
+    cursor.release();
+    h->x_nnz = sel;
+    return rc;
+}
+
+template <typename IP, typename II>
+static int ac_load_csr_device_v(sqb_autocorr* h, const void* xp, const void* xi, const void* xv, int data_dtype, int layout,
+                                int64_t n_cols, const int32_t* col_map, const std::vector<int32_t>& inv, int64_t n_out) {
+    const IP* p = reinterpret_cast<const IP*>(xp);
+    const II* i = reinterpret_cast<const II*>(xi);
+    switch (data_dtype) {  // float32 stays float32, everything else becomes float64 (the host path's dtype rule)
+        case 0: return ac_load_csr_device_typed<IP, II, float, float>(h, p, i, (const float*)xv, layout, n_cols, col_map, inv, n_out);
+        case 1: return ac_load_csr_device_typed<IP, II, double, double>(h, p, i, (const double*)xv, layout, n_cols, col_map, inv, n_out);
+        case 2: return ac_load_csr_device_typed<IP, II, __half, double>(h, p, i, (const __half*)xv, layout, n_cols, col_map, inv, n_out);
+        case 3: return ac_load_csr_device_typed<IP, II, int32_t, double>(h, p, i, (const int32_t*)xv, layout, n_cols, col_map, inv, n_out);
+        default: return ac_load_csr_device_typed<IP, II, int64_t, double>(h, p, i, (const int64_t*)xv, layout, n_cols, col_map, inv, n_out);
+    }
+}
+
+template <typename VT, typename XT>
+static int ac_gather_dense(sqb_autocorr* h, const void* x, int64_t n_out, int64_t s_obs, int64_t s_feat, const int32_t* d_inv,
+                           int obs_major) {
+    sqb_ctx* c = h->ctx;
+    SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+    ac_gather_dense_kernel<VT, XT><<<c->sm_count * 8, 256, 0, c->stream>>>((const VT*)x, h->n, n_out, s_obs, s_feat, d_inv, obs_major,
+                                                                          reinterpret_cast<XT*>(h->d_x.p));
+    SQB_POST_LAUNCH();
+    return SQB_OK;
 }
 
 extern "C" {
@@ -1388,6 +1607,86 @@ int sqb_autocorr_load_csr_cols(sqb_autocorr* h, const int64_t* x_indptr, const i
     h->kind = 3;
     h->x_dtype = x_dtype;
     h->n_feat = nf;
+    return SQB_OK;
+}
+
+int sqb_autocorr_load_csr_device(sqb_autocorr* h, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                                 const void* data, int data_dtype, int layout, int64_t n_cols, const int32_t* col_map, int64_t n_out,
+                                 uintptr_t producer_stream) {
+    static const char* where = "sqb_autocorr_load_csr_device";
+    SQB_CHECK(h && indptr && col_map, SQB_ERR_INVALID, "%s: null argument", where);
+    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
+              "%s: indptr_bits / index_bits must be 32 or 64", where);
+    SQB_CHECK(data_dtype >= 0 && data_dtype <= 4, SQB_ERR_INVALID, "%s: data_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32) or 4 (i64)",
+              where);
+    SQB_CHECK(layout == 0 || layout == 1, SQB_ERR_INVALID, "%s: layout must be 0 or 1", where);
+    std::vector<int32_t> inv;
+    SQB_TRY(ac_invert_col_map(col_map, n_cols, n_out, inv, where));
+    sqb_ctx* c = h->ctx;
+    SQB_CUDA(cudaSetDevice(c->device));
+    SQB_TRY(ac_wait_producer(c, producer_stream));
+    h->kind = 0;
+    h->aux_valid = false;
+    h->ran = false;
+    int rc;
+    if (indptr_bits == 32)
+        rc = index_bits == 32 ? ac_load_csr_device_v<int32_t, int32_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out)
+                              : ac_load_csr_device_v<int32_t, int64_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out);
+    else
+        rc = index_bits == 32 ? ac_load_csr_device_v<int64_t, int32_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out)
+                              : ac_load_csr_device_v<int64_t, int64_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out);
+    SQB_TRY(rc);
+    h->kind = 3;
+    h->x_dtype = data_dtype == 0 ? 0 : 1;
+    h->n_feat = n_out;
+    return SQB_OK;
+}
+
+int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, int64_t rows, int64_t cols, int64_t stride_row,
+                                   int64_t stride_col, int layout, const int32_t* col_map, int64_t n_out, uintptr_t producer_stream) {
+    static const char* where = "sqb_autocorr_load_dense_device";
+    SQB_CHECK(h && x && col_map, SQB_ERR_INVALID, "%s: null argument", where);
+    SQB_CHECK(x_dtype >= 0 && x_dtype <= 4, SQB_ERR_INVALID, "%s: x_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32) or 4 (i64)", where);
+    SQB_CHECK(layout == 0 || layout == 1, SQB_ERR_INVALID, "%s: layout must be 0 or 1", where);
+    const int64_t n_obs = layout == 1 ? rows : cols, n_cols = layout == 1 ? cols : rows;
+    SQB_CHECK(n_obs == h->n, SQB_ERR_INVALID, "%s: expected %lld observations, found %lld", where, (long long)h->n, (long long)n_obs);
+    const int64_t s_obs = layout == 1 ? stride_row : stride_col, s_feat = layout == 1 ? stride_col : stride_row;
+    std::vector<int32_t> inv;
+    SQB_TRY(ac_invert_col_map(col_map, n_cols, n_out, inv, where));
+    sqb_ctx* c = h->ctx;
+    SQB_CUDA(cudaSetDevice(c->device));
+    SQB_TRY(ac_wait_producer(c, producer_stream));
+    h->kind = 0;
+    h->aux_valid = false;
+    h->ran = false;
+    const int xt = x_dtype == 0 ? 0 : 1;
+    // zero-copy tiles read up to 31 elements past the last feature of a row: pad the allocation (as sqb_autocorr_load_dense)
+    SQB_TRY(h->d_x.alloc((size_t)n_out * h->n * xsize(xt) + 64 * 8));
+    SQB_TRY(h->d_out.alloc((size_t)n_out));
+    DevBuf<int32_t> map;
+    map.bind(c->stream);
+    SQB_TRY(map.alloc(n_out));
+    int rc = SQB_OK;
+    cudaError_t e = cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) {
+        sqb_set_error("%s: %s", where, cudaGetErrorString(e));
+        rc = SQB_ERR_CUDA;
+    } else {
+        switch (x_dtype) {
+            case 0: rc = ac_gather_dense<float, float>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
+            case 1: rc = ac_gather_dense<double, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
+            case 2: rc = ac_gather_dense<__half, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
+            case 3: rc = ac_gather_dense<int32_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
+            default: rc = ac_gather_dense<int64_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
+        }
+    }
+    map.release();
+    e = cudaStreamSynchronize(c->stream);  // the caller's buffer is no longer read
+    SQB_TRY(rc);
+    SQB_CUDA(e);
+    h->kind = layout == 0 ? 1 : 2;
+    h->x_dtype = xt;
+    h->n_feat = n_out;
     return SQB_OK;
 }
 

@@ -277,4 +277,18 @@ int sqb_host_free(void* ptr) {
     return SQB_OK;
 }
 
+int sqb_pointer_device(const void* p, int* device) {
+    SQB_CHECK(device, SQB_ERR_INVALID, "sqb_pointer_device: null argument");
+    cudaPointerAttributes attr;
+    const cudaError_t e = cudaPointerGetAttributes(&attr, p);
+    if (e == cudaErrorInvalidValue) {  // a host pointer CUDA has never seen
+        cudaGetLastError();
+        *device = -1;
+        return SQB_OK;
+    }
+    SQB_CUDA(e);
+    *device = (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) ? attr.device : -1;
+    return SQB_OK;
+}
+
 }  // extern "C"

@@ -23,8 +23,9 @@ from scipy import stats
 from scipy.sparse import issparse, spmatrix
 
 from .._constants import Key, SpatialAutocorr
+from .._device import DevArray, DevSparse, array_device, common_stream, device_matrix, dtype_code, feature_map, index_bits, to_host_matrix
 from .._dist import all_gather_rows, all_reduce_sum, shard_range, shared_seed, world
-from .._lib import Context, check, default_context, load
+from .._lib import Context, check, default_context, load, pointer_device
 from .._rng import spawn_generators
 from .._validators import (
     assert_categorical_obs,
@@ -73,14 +74,23 @@ class AutocorrPlan:
             return np.ascontiguousarray(a), 0
         return np.ascontiguousarray(a, dtype=np.float64), 1  # ints, float16, float64 ... -> float64 like scanpy's astype
 
-    def load(self, m: Any, *, obs_major: bool, cols: tuple[int, int] | None = None) -> None:
-        """``m``: observations x features if ``obs_major`` else features x observations; dense or scipy sparse.
+    def load(self, m: Any, *, obs_major: bool, cols: tuple[int, int] | None = None, col_map: np.ndarray | None = None) -> None:
+        """``m``: observations x features if ``obs_major`` else features x observations; dense or scipy sparse, or resident
+        in device memory (see :mod:`squidpy_b200._device`): then it is read in place on the device and never copied to the host.
         ``cols=(lo, hi)`` loads only features ``lo..hi`` (the shard of one rank): for CSR-by-observation input the slice is
-        cut while the matrix is staged for the upload (``sqb_autocorr_load_csr_cols``), nothing is copied on the host."""
-        n_feat = m.shape[1] if obs_major else m.shape[0]
-        n_obs = m.shape[0] if obs_major else m.shape[1]
+        cut while the matrix is staged for the upload (``sqb_autocorr_load_csr_cols``), nothing is copied on the host.
+        ``col_map`` (device input only, instead of ``cols``): int32 per input feature, its index among the loaded features
+        or -1 to skip it."""
+        n_feat = int(m.shape[1] if obs_major else m.shape[0])
+        n_obs = int(m.shape[0] if obs_major else m.shape[1])
         if n_obs != self.n:
             raise ValueError(f"Expected `{self.n}` observations, found `{n_obs}`.")
+        dev = device_matrix(m)
+        if dev is not None:
+            self._load_device(dev, obs_major, n_feat, cols, col_map)
+            return
+        if col_map is not None:
+            raise ValueError("`col_map` applies to device-resident input only.")
         if cols is not None and tuple(cols) == (0, n_feat):
             cols = None
         if issparse(m):
@@ -116,6 +126,35 @@ class AutocorrPlan:
             a, dt = self._dt(a)
             check(self._lib.sqb_autocorr_load_dense(self._h, a.ctypes.data, dt, int(obs_major), n_feat))
         self.n_features = int(n_feat)
+
+    def _load_device(self, d: DevArray | DevSparse, obs_major: bool, n_feat: int, cols: tuple[int, int] | None,
+                     col_map: np.ndarray | None) -> None:
+        if col_map is None:
+            lo, hi = cols if cols is not None else (0, n_feat)
+            col_map, n_out, _ = feature_map(n_feat, np.arange(lo, hi))
+        else:
+            col_map = np.ascontiguousarray(col_map, dtype=np.int32)
+            if col_map.shape != (n_feat,):
+                raise ValueError(f"Expected `col_map` of length `{n_feat}`, found shape `{col_map.shape}`.")
+            n_out = int(col_map.max(initial=-1)) + 1
+        if n_out < 1:
+            raise ValueError("No feature selected.")
+        dev = array_device(d, pointer_device)
+        if dev != self.ctx.device:
+            raise ValueError(f"The matrix lives on cuda:{dev}, but this plan's context is on cuda:{self.ctx.device}.")
+        stream = common_stream(d)
+        if isinstance(d, DevSparse):
+            # CSC of (a x b) == CSR of (b x a): the orientation flips instead of a conversion
+            layout = int(obs_major) if d.format == "csr" else int(not obs_major)
+            check(self._lib.sqb_autocorr_load_csr_device(self._h, d.indptr.ptr, index_bits(d.indptr, "indptr"), d.indices.ptr,
+                                                         index_bits(d.indices, "indices"), d.data.ptr, dtype_code(d.data), layout, n_feat,
+                                                         col_map.ctypes.data, n_out, stream))
+        else:
+            if len(d.shape) != 2:
+                raise ValueError(f"Expected a 2-D device array, found shape `{d.shape}`.")
+            check(self._lib.sqb_autocorr_load_dense_device(self._h, d.ptr, dtype_code(d), d.shape[0], d.shape[1], d.strides[0], d.strides[1],
+                                                           int(obs_major), col_map.ctypes.data, n_out, stream))
+        self.n_features = n_out
 
     def run_async(self, mode: SpatialAutocorr | str, row_perm: np.ndarray | None = None) -> None:
         mode = SpatialAutocorr(mode)
@@ -183,19 +222,31 @@ def spatial_autocorr(
     Returns / writes ``adata.uns['moranI' | 'gearyC']``: DataFrame indexed by feature with columns ``I``|``C``,
     ``pval_norm``, ``var_norm``, (with ``n_perms``) ``pval_z_sim``, ``pval_sim``, ``var_sim``, and
     ``{pval}_{corr_method}``; sorted by the statistic.  Under ``torch.distributed`` the features are sharded over
-    ranks (one all-gather of the scores)."""
+    ranks (one all-gather of the scores).
+
+    ``adata.X`` / ``layers[layer]`` / ``raw.X`` / ``obsm[layer]`` may be resident in device memory (cupy / cupyx.scipy.sparse,
+    torch CUDA tensors, anything exposing ``__cuda_array_interface__``): the features are then selected and scored on the
+    array's own device (``device`` must match it), and the matrix is never copied to the host.  A device-resident
+    ``obsp[connectivity_key]`` is copied to the host once (it is small; its moments and row normalisation are computed there)."""
     adata = extract_adata_if_sdata(adata, table_key=table_key)
     assert_connectivity_key(adata, connectivity_key)
 
     # ---- feature matrix, observations x features (the reference builds the transpose, :154-194) ----
-    def extract_X(genes):
+    def select_genes(genes):  # the feature list and its order, for host and device matrices alike
         if genes is None:
             if "highly_variable" in adata.var:
-                genes = adata[:, adata.var["highly_variable"]].var_names.values
+                genes = adata.var_names[np.asarray(adata.var["highly_variable"], dtype=bool)].values
             else:
                 genes = adata.var_names.values
         elif isinstance(genes, str):
             genes = [genes]
+        if use_raw:
+            if adata.raw is None:
+                raise AttributeError("No `.raw` attribute found. Try specifying `use_raw=False`.")
+            genes = list(set(genes) & set(adata.raw.var_names))
+        return genes
+
+    def extract_X(genes):
         if not use_raw:
             if len(genes) == adata.shape[1] and np.array_equal(np.asarray(genes), np.asarray(adata.var_names)):
                 # all variables in their own order: the subset is the matrix itself (the reference's adata[:, genes] copies it
@@ -203,10 +254,16 @@ def spatial_autocorr(
                 return (adata.X if layer is None else adata.layers[layer]), genes
             subset = adata[:, genes]
             return (subset.X if layer is None else subset.layers[layer]), genes
-        if adata.raw is None:
-            raise AttributeError("No `.raw` attribute found. Try specifying `use_raw=False`.")
-        genes = list(set(genes) & set(adata.raw.var_names))
         return adata.raw[:, genes].X, genes
+
+    def var_positions(var_names, genes):  # adata[:, genes] as column positions (names, or integer positions)
+        sel = np.asarray(genes)
+        if sel.dtype.kind in "iu":
+            return sel.astype(np.int64)
+        ix = pd.Index(var_names).get_indexer(sel)
+        if (ix < 0).any():
+            raise KeyError(f"Values {[str(s) for s, i in zip(sel, ix) if i < 0]} are not valid var names or indices.")
+        return ix.astype(np.int64)
 
     def extract_obs(cols):
         if cols is None:
@@ -216,19 +273,33 @@ def spatial_autocorr(
             cols = [cols]
         return adata.obs[cols].to_numpy(), cols
 
-    def extract_obsm(ixs):
+    def obsm_columns(ixs):
         assert_key_in_adata(adata, layer, attr="obsm")
         if ixs is None:
             ixs = list(np.arange(adata.obsm[layer].shape[1]))
-        ixs = list(np.ravel([ixs]))
-        return adata.obsm[layer][:, ixs], ixs
+        return list(np.ravel([ixs]))
 
+    # device-resident matrix: `src` (every feature) and the column `positions` of the selected ones; X is not touched here
+    src, positions = None, None
     if attr == "X":
-        mat, index = extract_X(genes)
+        genes = select_genes(genes)
+        src = adata.raw.X if use_raw else (adata.X if layer is None else adata.layers[layer])
+        if device_matrix(src) is None:
+            src = None
+            mat, index = extract_X(genes)
+        else:
+            index = genes
+            positions = var_positions(adata.raw.var_names if use_raw else adata.var_names, genes)
     elif attr == "obs":
         mat, index = extract_obs(genes)
     elif attr == "obsm":
-        mat, index = extract_obsm(genes)
+        index = obsm_columns(genes)
+        src = adata.obsm[layer]
+        if device_matrix(src) is None:
+            src = None
+            mat = adata.obsm[layer][:, index]
+        else:
+            positions = np.asarray(index, dtype=np.int64)
     else:
         raise NotImplementedError(f"Extracting from `adata.{attr}` is not yet implemented.")
 
@@ -239,22 +310,33 @@ def spatial_autocorr(
     else:
         params.update(stat="C", expected=1.0, ascending=True)
 
-    g = adata.obsp[connectivity_key].copy()
+    g = adata.obsp[connectivity_key]
+    g = g.copy() if device_matrix(g) is None else to_host_matrix(g)
     if transformation:  # row-normalise in place, dtype preserved (float32 stays float32), :212-214
         from sklearn.preprocessing import normalize
 
         normalize(g, norm="l1", axis=1, copy=False)
 
     start = time.perf_counter()
-    n_feat = mat.shape[1]
+    n_feat = mat.shape[1] if src is None else len(positions)
     rank, ws = world()
     lo, hi = shard_range(n_feat, rank, ws)
+    expand = None  # device input: scores of the shard = loaded scores[expand] (duplicate features are loaded once)
+    if src is not None:
+        on = array_device(device_matrix(src), pointer_device)
+        if device is not None and int(device) != on:
+            raise ValueError(f"`device={device}` does not match the device of the feature matrix, cuda:{on}.")
+        device = on
     ctx = default_context(device)
     logg.info("Calculating %s's statistic for `%s` permutations on cuda:%d (rank %d/%d, features %d..%d)", mode, n_perms, ctx.device, rank, ws, lo, hi)
     with ctx.lock:
         plan = AutocorrPlan(g, ctx)
         try:
-            if hi > lo:
+            if hi > lo and src is not None:
+                col_map, _, expand = feature_map(src.shape[1], positions, lo, hi)
+                plan.load(src, obs_major=True, col_map=col_map)
+                score_local = plan.score(mode)[expand]
+            elif hi > lo:
                 plan.load(mat, obs_major=True, cols=(lo, hi))
                 score_local = plan.score(mode)
             else:
@@ -279,7 +361,8 @@ def spatial_autocorr(
                         if k + 1 < len(starts):
                             nxt = pool.submit(draw, starts[k + 1])
                         if hi > lo:
-                            sp_local[p0 : p0 + idx.shape[0]] = plan.score_perms(mode, idx)
+                            sp = plan.score_perms(mode, idx)
+                            sp_local[p0 : p0 + idx.shape[0]] = sp if expand is None else sp[:, expand]
                 score_perms = np.ascontiguousarray(all_gather_rows(np.ascontiguousarray(sp_local.T), n_feat).T)
         finally:
             plan.close()

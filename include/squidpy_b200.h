@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 4
+#define SQB_ABI_VERSION 5
 
 typedef enum {
     SQB_OK = 0,
@@ -81,6 +81,15 @@ int sqb_pointer_device(const void* p, int* device);
  * uint32, _nhood.py:52,205).  n_cls = number of categories (labels in [0, n_cls)).                       */
 int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indptr, const uint32_t* indices,
                      int n_cls, sqb_nhood** out);
+/* The same from a graph already in device memory (e.g. a cupy / torch CSR of the caller): indptr (n + 1 entries) and
+ * indices (nnz) are DEVICE pointers on the context's device with indptr_bits / index_bits 32 or 64 (signed).  The handle
+ * converts them into its own uint32 copy on the device (the caller may free its buffers once the call returns; the library
+ * never writes them); from there the graph is prepared exactly as by sqb_nhood_create.  indptr must run from 0 to nnz
+ * without decreasing and every index must lie in [0, n) (negative ones included): both are checked on the device before
+ * anything follows the arrays (SQB_ERR_INVALID).  producer_stream: as in sqb_autocorr_load_csr_device.  A CSC graph
+ * passed here is the CSR of its transpose: every count it yields is the transpose of the graph's.                      */
+int sqb_nhood_create_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
+                            int index_bits, int n_cls, uintptr_t producer_stream, sqb_nhood** out);
 int sqb_nhood_destroy(sqb_nhood* h);
 
 /* observed count: out[a*n_cls+b] = #stored entries (i->j) with labels[i]=a, labels[j]=b   (uint32)       */
@@ -171,6 +180,15 @@ int sqb_nhood_bytes_per_perm(sqb_nhood* h, int64_t* bytes);
 int sqb_interaction_matrix(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indptr, const uint32_t* indices,
                            const void* data, int data_dtype, const int32_t* codes, int n_cls, double* out_weighted,
                            int64_t* out_counts);
+/* The same from a graph in device memory, read in place (no copy): indptr / indices / data are DEVICE pointers on the
+ * context's device, indptr_bits / index_bits 32 or 64; codes and the outputs stay on the host.  weights=True is selected by
+ * out_weighted != NULL (out_counts otherwise); data_dtype 0 = f32, 1 = f64, 2 = f16, 3 = int32, 4 = int64, 5 = bool (one
+ * byte), every value summed in float64.  indptr is checked on the device before anything follows it; column indices outside
+ * [0, n) and codes >= n_cls are detected by the kernel (SQB_ERR_INVALID, no result).  producer_stream: as in
+ * sqb_autocorr_load_csr_device.  Returns after the device has stopped reading the caller's buffers.                   */
+int sqb_interaction_matrix_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
+                                  int index_bits, const void* data, int data_dtype, const int32_t* codes, int n_cls,
+                                  double* out_weighted, int64_t* out_counts, uintptr_t producer_stream);
 
 /* ---- ligrec permutation test ------------------------------------------------------------------------------
  * _score_permutations of the reference (src/squidpy/gr/_ligrec.py:616-676) for a handle whose base labels are the cells'

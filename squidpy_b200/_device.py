@@ -158,6 +158,63 @@ def index_bits(a: DevArray, what: str) -> int:
     return 8 * a.dtype.itemsize
 
 
+@dataclass
+class DevGraph:
+    """The ABI arguments of a device neighbour graph (``sqb_nhood_create_device`` / ``sqb_interaction_matrix_device``).
+
+    The arrays are handed over as given.  For a CSC graph they are the CSR of the transpose, so every C x C result computed
+    from them is the transpose of the graph's: ``transposed`` tells the caller to transpose it back."""
+
+    sparse: DevSparse
+    n: int
+    nnz: int
+    indptr_bits: int
+    index_bits: int
+    transposed: bool
+    stream: int
+
+    @property
+    def indptr(self) -> int:
+        return self.sparse.indptr.ptr
+
+    @property
+    def indices(self) -> int:
+        return self.sparse.indices.ptr
+
+
+def device_graph(m: Any) -> DevSparse | None:
+    """The device description of a neighbour graph (``obsp[key]``), or ``None`` for a host graph.  Graphs are sparse: a
+    dense device array raises ``NotImplementedError``."""
+    d = device_matrix(m)
+    if isinstance(d, DevArray):
+        raise NotImplementedError(f"Dense device graphs are not supported; supported formats: {', '.join(SPARSE_FORMATS)}.")
+    return d
+
+
+def graph_args(d: DevSparse, n_obs: int) -> DevGraph:
+    """Check that ``d`` is an ``n_obs x n_obs`` graph with int32 / int64 index arrays and describe it for the C ABI."""
+    if tuple(d.shape) != (n_obs, n_obs):
+        raise ValueError(f"Expected the connectivity graph to be of shape `{(n_obs, n_obs)}`, found `{tuple(d.shape)}`.")
+    ip_bits, ix_bits = index_bits(d.indptr, "indptr"), index_bits(d.indices, "indices")
+    if d.indptr.shape[0] != n_obs + 1:
+        raise ValueError(f"Expected `indptr` of length `{n_obs + 1}`, found `{d.indptr.shape[0]}`.")
+    nnz = int(d.indices.shape[0])
+    return DevGraph(d, n_obs, nnz, ip_bits, ix_bits, d.format == "csc", common_stream(d))
+
+
+# value dtype code of sqb_interaction_matrix_device: the autocorr codes plus bool (one byte per value)
+GRAPH_VALUE_CODES = {**DTYPE_CODES, np.dtype(np.bool_): 5}
+
+
+def graph_value_code(a: DevArray, nnz: int) -> int:
+    code = GRAPH_VALUE_CODES.get(a.dtype)
+    if code is None:
+        raise TypeError(f"Device graph values of dtype `{a.dtype}` are not supported; use float32, float64, float16, int32, int64 or bool.")
+    if len(a.shape) != 1 or a.shape[0] != nnz or (nnz > 1 and a.strides[0] != 1):
+        raise ValueError(f"The graph's values must be a contiguous 1-D array of `{nnz}` entries.")
+    return code
+
+
 def feature_map(n_cols: int, positions: Any, lo: int = 0, hi: int | None = None) -> tuple[np.ndarray, int, np.ndarray]:
     """``col_map`` of ``sqb_autocorr_load_*_device`` for the selected features ``positions[lo:hi]`` (input feature of every
     selected feature, in output order; duplicates allowed).  Every distinct feature is loaded once, in order of first

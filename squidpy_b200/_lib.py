@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (the test suite points it at the build that also contains the superseded
 # replay variants, tests/native/libsquidpy_b200_testvariants.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -50,6 +50,8 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_host_free": (C.c_int, [C.c_void_p]),
     "sqb_pointer_device": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
     "sqb_nhood_create": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, c_void_pp]),
+    "sqb_nhood_create_device": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_size_t,
+                                           c_void_pp]),
     "sqb_nhood_destroy": (C.c_int, [C.c_void_p]),
     "sqb_nhood_count": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "sqb_nhood_set_base": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
@@ -61,6 +63,8 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_nhood_permute_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "sqb_interaction_matrix": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                           C.c_int, C.c_void_p, C.c_void_p]),
+    "sqb_interaction_matrix_device": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                                 C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sqb_nhood_permute_sums": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sqb_nhood_permute_var_chain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sqb_nhood_permute_stats_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -1242,21 +1242,6 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
 }
 
 // ---- device-resident input (sqb_autocorr_load_*_device) ------------------------------------------------------------
-// Make the context's stream wait for the caller's producer stream (CUDA Array Interface v3 `stream`: 0 none, 1 legacy
-// default stream, 2 per-thread default stream, else a cudaStream_t).
-static int ac_wait_producer(sqb_ctx* c, uintptr_t producer) {
-    if (producer == 0) return SQB_OK;
-    cudaStream_t s = producer == 1 ? cudaStreamLegacy : producer == 2 ? cudaStreamPerThread : (cudaStream_t)producer;
-    if (s == c->stream) return SQB_OK;
-    cudaEvent_t ev;
-    SQB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    cudaError_t e = cudaEventRecord(ev, s);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->stream, ev, 0);
-    cudaEventDestroy(ev);  // released once the recorded work completes
-    SQB_CUDA(e);
-    return SQB_OK;
-}
-
 // col_map[f] in [0, n_out) or -1 for every input feature f; every output feature must come from exactly one input feature.
 // inv[k] = the input feature of output feature k.
 static int ac_invert_col_map(const int32_t* col_map, int64_t n_cols, int64_t n_out, std::vector<int32_t>& inv, const char* where) {
@@ -1624,7 +1609,7 @@ int sqb_autocorr_load_csr_device(sqb_autocorr* h, const void* indptr, int indptr
     SQB_TRY(ac_invert_col_map(col_map, n_cols, n_out, inv, where));
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    SQB_TRY(ac_wait_producer(c, producer_stream));
+    SQB_TRY(sqb_wait_producer(c, producer_stream));
     h->kind = 0;
     h->aux_valid = false;
     h->ran = false;
@@ -1655,7 +1640,7 @@ int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, 
     SQB_TRY(ac_invert_col_map(col_map, n_cols, n_out, inv, where));
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    SQB_TRY(ac_wait_producer(c, producer_stream));
+    SQB_TRY(sqb_wait_producer(c, producer_stream));
     h->kind = 0;
     h->aux_valid = false;
     h->ran = false;

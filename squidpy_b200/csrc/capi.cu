@@ -132,6 +132,19 @@ int sqb_h2d_gather(sqb_ctx* c, void* dst, const void* src, size_t elem, const in
     return SQB_OK;
 }
 
+int sqb_wait_producer(sqb_ctx* c, uintptr_t producer) {
+    if (producer == 0) return SQB_OK;
+    cudaStream_t s = producer == 1 ? cudaStreamLegacy : producer == 2 ? cudaStreamPerThread : (cudaStream_t)producer;
+    if (s == c->stream) return SQB_OK;
+    cudaEvent_t ev;
+    SQB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    cudaError_t e = cudaEventRecord(ev, s);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->stream, ev, 0);
+    cudaEventDestroy(ev);  // released once the recorded work completes
+    SQB_CUDA(e);
+    return SQB_OK;
+}
+
 extern "C" {
 
 int sqb_abi_version(void) { return SQB_ABI_VERSION; }

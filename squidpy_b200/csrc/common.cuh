@@ -128,6 +128,10 @@ int sqb_h2d(sqb_ctx* c, void* dst, const void* src, size_t bytes);
 int sqb_h2d_gather(sqb_ctx* c, void* dst, const void* src, size_t elem, const int64_t* start, const int64_t* cnt,
                    const int64_t* out_ptr, int64_t rows);
 
+// Device-resident caller arrays: make the context's stream wait for the caller's producer stream before it reads them
+// (CUDA Array Interface v3 `stream`: 0 none, 1 legacy default stream, 2 per-thread default stream, else a cudaStream_t).
+int sqb_wait_producer(sqb_ctx* c, uintptr_t producer);
+
 // Launch accounting.  In profile mode each launch is bracketed by events on the ctx stream and the elapsed
 // time accumulated per kernel class (the launch is synchronised; never used inside a timed bench region
 // except for the dedicated roofline pass).
@@ -161,3 +165,21 @@ struct SqbLaunchScope {
     } while (0)
 
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// The indptr (n + 1 entries, int32 or int64) of a caller's device CSR must run from 0 at row 0 to nnz at row n without
+// decreasing; bit 1 of *err otherwise.  Kernels that follow it may run only after *err has been read back as 0.
+// dst (or null) receives the validated indptr as uint32 (nnz < 2^32 - 1; an invalid entry is written as 0).
+template <typename IP>
+__global__ void sqb_check_indptr_kernel(const IP* __restrict__ ptr, int64_t n, int64_t nnz, uint32_t* __restrict__ dst,
+                                        unsigned* __restrict__ err) {
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r <= n; r += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t v = (int64_t)ptr[r];
+        const bool bad = v < 0 || v > nnz || (r == 0 && v != 0) || (r == n && v != nnz) || (r < n && (int64_t)ptr[r + 1] < v);
+        if (bad) atomicOr(err, 1u);
+        if (dst) dst[r] = bad ? 0u : (uint32_t)v;
+    }
+}
+static inline unsigned sqb_grid_rows(const sqb_ctx* c, int64_t rows, int threads) {
+    const int64_t b = ceil_div64(rows, threads), cap = (int64_t)c->sm_count * 8;
+    return (unsigned)(b < 1 ? 1 : b > cap ? cap : b);
+}

@@ -7,13 +7,26 @@
 //   weights = true : out[a][b] = sum of their values, accumulated in float64                             (order free:
 //                    exact for integer-valued weights, |rel err| ~1e-16 * entries otherwise)
 // HBM-bound: the CSR is streamed once (8-12 bytes per stored entry); the label gather hits L2.
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
-template <typename VT, bool WEIGHTED>
-__global__ void __launch_bounds__(256) interaction_kernel(const uint32_t* __restrict__ indptr, const uint32_t* __restrict__ indices,
+// value of a stored entry as float64 (float16 through float32: exact; bool arrives as one byte, any non-zero byte is true)
+__device__ __forceinline__ double inter_f64(float v) { return (double)v; }
+__device__ __forceinline__ double inter_f64(double v) { return v; }
+__device__ __forceinline__ double inter_f64(__half v) { return (double)__half2float(v); }
+__device__ __forceinline__ double inter_f64(int32_t v) { return (double)v; }
+__device__ __forceinline__ double inter_f64(int64_t v) { return (double)v; }
+__device__ __forceinline__ double inter_f64(uint8_t v) { return v != 0 ? 1.0 : 0.0; }
+
+// IP / II: index types of indptr / indices (uint32 for the host path's staged copy, int32 / int64 for a caller's device
+// CSR read in place).  A column index outside [0, n) is skipped and raises bit 2 of *err (null: host input, validated on
+// the host); a code >= C is skipped too (bit 4).  indptr must have been validated: the kernel follows it.
+template <typename IP, typename II, typename VT, bool WEIGHTED>
+__global__ void __launch_bounds__(256) interaction_kernel(const IP* __restrict__ indptr, const II* __restrict__ indices,
                                                           const VT* __restrict__ data, const int32_t* __restrict__ codes, int64_t n,
                                                           int C, int use_smem, double* __restrict__ out_w,
-                                                          unsigned long long* __restrict__ out_c) {
+                                                          unsigned long long* __restrict__ out_c, unsigned* __restrict__ err) {
     extern __shared__ unsigned char sqb_inter_smem[];
     double* s_w = reinterpret_cast<double*>(sqb_inter_smem);
     unsigned long long* s_c = reinterpret_cast<unsigned long long*>(sqb_inter_smem);
@@ -32,15 +45,25 @@ __global__ void __launch_bounds__(256) interaction_kernel(const uint32_t* __rest
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t i = warp; i < n; i += nwarps) {
-        const int32_t a = codes[i];
-        if (a < 0) continue;  // warp uniform
-        const uint32_t beg = indptr[i], end = indptr[i + 1];
-        for (uint32_t e = beg + lane; e < end; e += 32) {
-            const int32_t b = codes[indices[e]];
-            if (b < 0) continue;
+        const int32_t a = codes[i];  // warp uniform
+        if (a >= C) {
+            if (err && lane == 0) atomicOr(err, 4u);
+            continue;
+        }
+        if (a < 0 && !err) continue;  // unlabelled row; device input still has its column indices validated
+        const int64_t beg = (int64_t)indptr[i], end = (int64_t)indptr[i + 1];
+        for (int64_t e = beg + lane; e < end; e += 32) {
+            const int64_t j = (int64_t)indices[e];
+            if (j < 0 || j >= n) {
+                if (err) atomicOr(err, 2u);
+                continue;
+            }
+            if (a < 0) continue;
+            const int32_t b = codes[j];
+            if ((unsigned)b >= (unsigned)C) continue;  // no label (< 0); >= C is flagged by row j
             const int bin = a * C + b;
             if (WEIGHTED) {
-                const double v = (double)data[e];
+                const double v = inter_f64(data[e]);
                 if (use_smem)
                     atomicAdd(&s_w[bin], v);
                 else
@@ -66,6 +89,23 @@ __global__ void __launch_bounds__(256) interaction_kernel(const uint32_t* __rest
         }
     }
 }
+
+// grid / shared memory of interaction_kernel for n rows and C classes
+struct InterLaunch {
+    unsigned blocks;
+    size_t smem;
+    int use_smem;
+    InterLaunch(const sqb_ctx* c, int64_t n, int C) {
+        const size_t CC = (size_t)C * C;
+        use_smem = CC * 8 <= 48 * 1024;
+        smem = use_smem ? CC * 8 : 0;
+        int64_t b = ceil_div64(n * 32, 256);
+        const int64_t max_blocks = (int64_t)c->sm_count * 8;
+        if (b > max_blocks) b = max_blocks;
+        if (b < 1) b = 1;
+        blocks = (unsigned)b;
+    }
+};
 
 extern "C" int sqb_interaction_matrix(sqb_ctx* c, int64_t n, int64_t nnz, const uint32_t* indptr, const uint32_t* indices,
                                       const void* data, int data_dtype, const int32_t* codes, int n_cls, double* out_weighted,
@@ -117,20 +157,15 @@ extern "C" int sqb_interaction_matrix(sqb_ctx* c, int64_t n, int64_t nnz, const 
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_codes.p, codes, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_out.p, 0, (size_t)CC * 8, c->stream);
     if (e == cudaSuccess) {
-        const int use_smem = (size_t)CC * 8 <= 48 * 1024;
-        const size_t smem = use_smem ? (size_t)CC * 8 : 0;
-        int64_t blocks = ceil_div64(n * 32, 256);
-        const int64_t max_blocks = (int64_t)c->sm_count * 8;
-        if (blocks > max_blocks) blocks = max_blocks;
-        if (blocks < 1) blocks = 1;
+        const InterLaunch L(c, n, n_cls);
         SqbLaunchScope scope(c, SQB_K_MISC);
         double* ow = reinterpret_cast<double*>(d_out.p);
         if (!weighted)
-            interaction_kernel<float, false><<<(unsigned)blocks, 256, smem, c->stream>>>(d_ptr.p, d_idx.p, nullptr, d_codes.p, n, n_cls, use_smem, ow, d_out.p);
+            interaction_kernel<uint32_t, uint32_t, float, false><<<L.blocks, 256, L.smem, c->stream>>>(d_ptr.p, d_idx.p, nullptr, d_codes.p, n, n_cls, L.use_smem, ow, d_out.p, nullptr);
         else if (data_dtype == 0)
-            interaction_kernel<float, true><<<(unsigned)blocks, 256, smem, c->stream>>>(d_ptr.p, d_idx.p, reinterpret_cast<const float*>(d_val.p), d_codes.p, n, n_cls, use_smem, ow, d_out.p);
+            interaction_kernel<uint32_t, uint32_t, float, true><<<L.blocks, 256, L.smem, c->stream>>>(d_ptr.p, d_idx.p, reinterpret_cast<const float*>(d_val.p), d_codes.p, n, n_cls, L.use_smem, ow, d_out.p, nullptr);
         else
-            interaction_kernel<double, true><<<(unsigned)blocks, 256, smem, c->stream>>>(d_ptr.p, d_idx.p, reinterpret_cast<const double*>(d_val.p), d_codes.p, n, n_cls, use_smem, ow, d_out.p);
+            interaction_kernel<uint32_t, uint32_t, double, true><<<L.blocks, 256, L.smem, c->stream>>>(d_ptr.p, d_idx.p, reinterpret_cast<const double*>(d_val.p), d_codes.p, n, n_cls, L.use_smem, ow, d_out.p, nullptr);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess)
@@ -142,4 +177,93 @@ extern "C" int sqb_interaction_matrix(sqb_ctx* c, int64_t n, int64_t nnz, const 
         return SQB_ERR_CUDA;
     }
     return SQB_OK;
+}
+
+// ---- device-resident graph (sqb_interaction_matrix_device) ----------------------------------------------------------
+// The caller's CSR is read in place by interaction_kernel<IP, II, VT>: no copy.  indptr is validated first (one
+// synchronisation); column indices and codes are validated by the kernel as it goes, and a flagged result is discarded.
+template <typename IP, typename II>
+static int inter_device_typed(sqb_ctx* c, int64_t n, int64_t nnz, const void* indptr, const void* indices, bool weighted, const void* data,
+                              int data_dtype, const int32_t* d_codes, int n_cls, unsigned long long* d_out, unsigned* d_err) {
+    static const char* where = "sqb_interaction_matrix_device";
+    const IP* ip = reinterpret_cast<const IP*>(indptr);
+    const II* ix = reinterpret_cast<const II*>(indices);
+    unsigned flag = 0;
+    {
+        SqbLaunchScope scope(c, SQB_K_MISC);
+        sqb_check_indptr_kernel<IP><<<sqb_grid_rows(c, n + 1, 256), 256, 0, c->stream>>>(ip, n, nnz, nullptr, d_err);
+        SQB_POST_LAUNCH();
+    }
+    SQB_CUDA(cudaMemcpyAsync(&flag, d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    SQB_CHECK(flag == 0, SQB_ERR_INVALID, "%s: indptr inconsistent with nnz=%lld (it must run from 0 to nnz without decreasing)", where,
+              (long long)nnz);
+    const InterLaunch L(c, n, n_cls);
+    double* ow = reinterpret_cast<double*>(d_out);
+    SqbLaunchScope scope(c, SQB_K_MISC);
+#define SQB_INTER(VT, W) \
+    interaction_kernel<IP, II, VT, W><<<L.blocks, 256, L.smem, c->stream>>>(ip, ix, reinterpret_cast<const VT*>(data), d_codes, n, n_cls, L.use_smem, ow, d_out, d_err)
+    if (!weighted) SQB_INTER(float, false);
+    else switch (data_dtype) {
+        case 0: SQB_INTER(float, true); break;
+        case 1: SQB_INTER(double, true); break;
+        case 2: SQB_INTER(__half, true); break;
+        case 3: SQB_INTER(int32_t, true); break;
+        case 4: SQB_INTER(int64_t, true); break;
+        default: SQB_INTER(uint8_t, true); break;
+    }
+#undef SQB_INTER
+    SQB_POST_LAUNCH();
+    return SQB_OK;
+}
+
+extern "C" int sqb_interaction_matrix_device(sqb_ctx* c, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
+                                             int index_bits, const void* data, int data_dtype, const int32_t* codes, int n_cls,
+                                             double* out_weighted, int64_t* out_counts, uintptr_t producer_stream) {
+    static const char* where = "sqb_interaction_matrix_device";
+    SQB_CHECK(c, SQB_ERR_INVALID, "%s: null ctx", where);
+    SQB_CHECK(n >= 1 && n < 0x7FFFFFFFLL, SQB_ERR_INVALID, "%s: n=%lld out of range", where, (long long)n);
+    SQB_CHECK(nnz >= 0 && nnz < 0xFFFFFFFFLL, SQB_ERR_INVALID, "%s: nnz=%lld does not fit uint32", where, (long long)nnz);
+    SQB_CHECK(indptr && (indices || nnz == 0) && codes, SQB_ERR_INVALID, "%s: null argument", where);
+    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
+              "%s: indptr_bits / index_bits must be 32 or 64", where);
+    SQB_CHECK(n_cls >= 1 && n_cls <= 4096, SQB_ERR_INVALID, "%s: n_cls=%d out of range [1, 4096]", where, n_cls);
+    const bool weighted = out_weighted != nullptr;  // data may be null only when there are no entries
+    SQB_CHECK(!weighted || ((data || nnz == 0) && data_dtype >= 0 && data_dtype <= 5), SQB_ERR_INVALID,
+              "%s: data_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32), 4 (i64) or 5 (bool)", where);
+    SQB_CHECK(weighted || out_counts != nullptr, SQB_ERR_INVALID, "%s: null output", where);
+    SQB_CUDA(cudaSetDevice(c->device));
+    SQB_TRY(sqb_wait_producer(c, producer_stream));
+    const int CC = n_cls * n_cls;
+    DevBuf<int32_t> d_codes;
+    DevBuf<unsigned long long> d_out;  // 8 bytes per bin: double or uint64
+    DevBuf<unsigned> d_err;
+    d_codes.bind(c->stream), d_out.bind(c->stream), d_err.bind(c->stream);
+    unsigned flag = 0;
+    auto body = [&]() -> int {
+        SQB_TRY(d_codes.alloc(n));
+        SQB_TRY(d_out.alloc(CC));
+        SQB_TRY(d_err.alloc(1));
+        SQB_CUDA(cudaMemcpyAsync(d_codes.p, codes, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        SQB_CUDA(cudaMemsetAsync(d_out.p, 0, (size_t)CC * 8, c->stream));
+        SQB_CUDA(cudaMemsetAsync(d_err.p, 0, sizeof(unsigned), c->stream));
+        int rc;
+        if (indptr_bits == 32)
+            rc = index_bits == 32 ? inter_device_typed<int32_t, int32_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p)
+                                  : inter_device_typed<int32_t, int64_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p);
+        else
+            rc = index_bits == 32 ? inter_device_typed<int64_t, int32_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p)
+                                  : inter_device_typed<int64_t, int64_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p);
+        SQB_TRY(rc);
+        SQB_CUDA(cudaMemcpyAsync(weighted ? (void*)out_weighted : (void*)out_counts, d_out.p, (size_t)CC * 8, cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(&flag, d_err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffers are no longer read
+        SQB_CHECK(!(flag & 2u), SQB_ERR_INVALID, "%s: column index out of range [0, %lld)", where, (long long)n);
+        SQB_CHECK(!(flag & 4u), SQB_ERR_INVALID, "%s: a code is >= n_cls=%d", where, n_cls);
+        return SQB_OK;
+    };
+    const int rc = body();
+    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);
+    d_codes.release(), d_out.release(), d_err.release();
+    return rc;
 }

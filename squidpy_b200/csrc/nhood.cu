@@ -4581,22 +4581,18 @@ static int nhood_build_records(sqb_nhood* h, const uint32_t* ptr, const uint32_t
     return SQB_OK;
 }
 
-extern "C" {
-
-int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indptr, const uint32_t* indices, int n_cls,
-                     sqb_nhood** out) {
-    SQB_CHECK(ctx && out, SQB_ERR_INVALID, "sqb_nhood_create: null ctx/out");
-    SQB_CHECK(n >= 1 && n < 0x7FFFFFFFLL, SQB_ERR_INVALID, "sqb_nhood_create: n=%lld out of range [1, 2^31-1)", (long long)n);
-    SQB_CHECK(nnz >= 0 && nnz < 0xFFFFFFFFLL, SQB_ERR_INVALID, "sqb_nhood_create: nnz=%lld does not fit uint32",
-              (long long)nnz);
+static int nhood_check_args(const char* where, sqb_ctx* ctx, int64_t n, int64_t nnz, int n_cls, sqb_nhood** out) {
+    SQB_CHECK(ctx && out, SQB_ERR_INVALID, "%s: null ctx/out", where);
+    SQB_CHECK(n >= 1 && n < 0x7FFFFFFFLL, SQB_ERR_INVALID, "%s: n=%lld out of range [1, 2^31-1)", where, (long long)n);
+    SQB_CHECK(nnz >= 0 && nnz < 0xFFFFFFFFLL, SQB_ERR_INVALID, "%s: nnz=%lld does not fit uint32", where, (long long)nnz);
     // same message as the reference (_nhood.py:107-108)
     SQB_CHECK(n_cls >= 2, SQB_ERR_INVALID, "Expected at least `2` clusters, found `%d`.", n_cls);
-    SQB_CHECK(n_cls <= 65535, SQB_ERR_UNSUPPORTED, "sqb_nhood_create: n_cls=%d > 65535 unsupported", n_cls);
-    SQB_CHECK(indptr && (indices || nnz == 0), SQB_ERR_INVALID, "sqb_nhood_create: null CSR arrays");
-    SQB_CHECK(indptr[0] == 0 && (int64_t)indptr[n] == nnz, SQB_ERR_INVALID,
-              "sqb_nhood_create: indptr[0]=%u indptr[n]=%u inconsistent with nnz=%lld", indptr[0], indptr[n],
-              (long long)nnz);
-    SQB_CUDA(cudaSetDevice(ctx->device));
+    SQB_CHECK(n_cls <= 65535, SQB_ERR_UNSUPPORTED, "%s: n_cls=%d > 65535 unsupported", where, n_cls);
+    return SQB_OK;
+}
+
+// A handle whose buffers live in ctx->stream order, with the uint32 CSR (d_indptr, d_indices) allocated but not filled.
+static int nhood_new(sqb_ctx* ctx, int64_t n, int64_t nnz, int n_cls, sqb_nhood** out) {
     sqb_nhood* h = new sqb_nhood();
     h->ctx = ctx;
     // all handle buffers are allocated, used and freed in ctx->stream order
@@ -4625,9 +4621,17 @@ int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indpt
         sqb_nhood_destroy(h);
         return rc;
     }
-    SQB_CUDA(cudaMemcpyAsync(h->d_indptr.p, indptr, (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    if (nnz > 0)
-        SQB_TRY(sqb_h2d(ctx, h->d_indices.p, indices, nnz * sizeof(uint32_t)));
+    *out = h;
+    return SQB_OK;
+}
+
+// The graph in h->d_indptr / d_indices (indptr[0] = 0 and indptr[n] = nnz already checked) -> symmetric check, upper CSR
+// and row records.  Destroys h on failure.
+static int nhood_prepare(sqb_nhood* h, const char* where) {
+    sqb_ctx* ctx = h->ctx;
+    const int64_t n = h->n, nnz = h->nnz;
+    const int n_cls = h->n_cls;
+    int rc = SQB_OK;
     // symmetric structure? then keep the entries with j >= i as a second CSR (3b)
     if (nnz > 0) {
         DevBuf<uint32_t> flag, ucnt;
@@ -4662,7 +4666,7 @@ int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indpt
         if (e == cudaSuccess && (hflag & 2u)) {  // the kernels index the label arrays with these values: refuse
             cleanup();
             sqb_nhood_destroy(h);
-            sqb_set_error("sqb_nhood_create: invalid CSR (column index outside [0, %lld) or indptr not monotone)", (long long)n);
+            sqb_set_error("%s: invalid CSR (column index outside [0, %lld) or indptr not monotone)", where, (long long)n);
             return SQB_ERR_INVALID;
         }
         if (e == cudaSuccess && hflag == 0) {
@@ -4689,7 +4693,7 @@ int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indpt
         }
         cleanup();
         if (e != cudaSuccess || rc != SQB_OK) {
-            if (e != cudaSuccess) sqb_set_error("sqb_nhood_create: symmetric-graph preparation failed: %s", cudaGetErrorString(e));
+            if (e != cudaSuccess) sqb_set_error("%s: symmetric-graph preparation failed: %s", where, cudaGetErrorString(e));
             sqb_nhood_destroy(h);
             return e != cudaSuccess ? SQB_ERR_CUDA : rc;
         }
@@ -4705,7 +4709,104 @@ int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indpt
             }
         }
     }
-    SQB_CUDA(cudaStreamSynchronize(ctx->stream));
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        sqb_set_error("%s: %s", where, cudaGetErrorString(e));
+        sqb_nhood_destroy(h);
+        return SQB_ERR_CUDA;
+    }
+    return SQB_OK;
+}
+
+// Device graph (sqb_nhood_create_device): column indices of a caller's CSR (int32 or int64) -> the handle's uint32 copy.
+// An index outside [0, n) becomes 0xFFFFFFFF (>= n, since n < 2^31 - 1), which nhood_symcheck_kernel rejects (flag bit 2)
+// exactly like a negative int32 index of the host path; an int64 index cannot wrap into range.
+template <typename II>
+__global__ void nhood_cvt_indices_kernel(const II* __restrict__ src, int64_t nnz, int64_t n, uint32_t* __restrict__ dst) {
+    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t j = (int64_t)src[e];
+        dst[e] = (j < 0 || j >= n) ? 0xFFFFFFFFu : (uint32_t)j;
+    }
+}
+
+template <typename IP, typename II>
+static int nhood_fill_device(sqb_nhood* h, const void* indptr, const void* indices, unsigned* d_err) {
+    sqb_ctx* ctx = h->ctx;
+    unsigned flag = 0;
+    {
+        SqbLaunchScope scope(ctx, SQB_K_NHOOD_FILL);
+        sqb_check_indptr_kernel<IP><<<sqb_grid_rows(ctx, h->n + 1, 256), 256, 0, ctx->stream>>>(
+            reinterpret_cast<const IP*>(indptr), h->n, h->nnz, h->d_indptr.p, d_err);
+        SQB_POST_LAUNCH();
+    }
+    if (h->nnz > 0) {
+        SqbLaunchScope scope(ctx, SQB_K_NHOOD_FILL);
+        nhood_cvt_indices_kernel<II><<<sqb_grid_rows(ctx, h->nnz, 256), 256, 0, ctx->stream>>>(reinterpret_cast<const II*>(indices), h->nnz,
+                                                                                               h->n, h->d_indices.p);
+        SQB_POST_LAUNCH();
+    }
+    SQB_CUDA(cudaMemcpyAsync(&flag, d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    SQB_CUDA(cudaStreamSynchronize(ctx->stream));  // the caller's buffers are no longer read
+    SQB_CHECK(flag == 0, SQB_ERR_INVALID, "sqb_nhood_create_device: indptr inconsistent with nnz=%lld (it must run from 0 to nnz without decreasing)",
+              (long long)h->nnz);
+    return SQB_OK;
+}
+
+extern "C" {
+
+int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indptr, const uint32_t* indices, int n_cls,
+                     sqb_nhood** out) {
+    SQB_TRY(nhood_check_args("sqb_nhood_create", ctx, n, nnz, n_cls, out));
+    SQB_CHECK(indptr && (indices || nnz == 0), SQB_ERR_INVALID, "sqb_nhood_create: null CSR arrays");
+    SQB_CHECK(indptr[0] == 0 && (int64_t)indptr[n] == nnz, SQB_ERR_INVALID,
+              "sqb_nhood_create: indptr[0]=%u indptr[n]=%u inconsistent with nnz=%lld", indptr[0], indptr[n],
+              (long long)nnz);
+    SQB_CUDA(cudaSetDevice(ctx->device));
+    sqb_nhood* h = nullptr;
+    SQB_TRY(nhood_new(ctx, n, nnz, n_cls, &h));
+    SQB_CUDA(cudaMemcpyAsync(h->d_indptr.p, indptr, (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    if (nnz > 0)
+        SQB_TRY(sqb_h2d(ctx, h->d_indices.p, indices, nnz * sizeof(uint32_t)));
+    SQB_TRY(nhood_prepare(h, "sqb_nhood_create"));
+    *out = h;
+    return SQB_OK;
+}
+
+int sqb_nhood_create_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                            int n_cls, uintptr_t producer_stream, sqb_nhood** out) {
+    static const char* where = "sqb_nhood_create_device";
+    SQB_TRY(nhood_check_args(where, ctx, n, nnz, n_cls, out));
+    SQB_CHECK(indptr && (indices || nnz == 0), SQB_ERR_INVALID, "%s: null CSR arrays", where);
+    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
+              "%s: indptr_bits / index_bits must be 32 or 64", where);
+    SQB_CUDA(cudaSetDevice(ctx->device));
+    SQB_TRY(sqb_wait_producer(ctx, producer_stream));
+    sqb_nhood* h = nullptr;
+    SQB_TRY(nhood_new(ctx, n, nnz, n_cls, &h));
+    DevBuf<unsigned> err;
+    err.bind(ctx->stream);
+    int rc = err.alloc(1);
+    if (rc == SQB_OK) {
+        const cudaError_t e = cudaMemsetAsync(err.p, 0, sizeof(unsigned), ctx->stream);
+        if (e != cudaSuccess) {
+            sqb_set_error("%s: %s", where, cudaGetErrorString(e));
+            rc = SQB_ERR_CUDA;
+        }
+    }
+    if (rc == SQB_OK) {
+        if (indptr_bits == 32)
+            rc = index_bits == 32 ? nhood_fill_device<int32_t, int32_t>(h, indptr, indices, err.p) : nhood_fill_device<int32_t, int64_t>(h, indptr, indices, err.p);
+        else
+            rc = index_bits == 32 ? nhood_fill_device<int64_t, int32_t>(h, indptr, indices, err.p) : nhood_fill_device<int64_t, int64_t>(h, indptr, indices, err.p);
+    }
+    if (rc != SQB_OK) cudaStreamSynchronize(ctx->stream);  // the caller's buffers are no longer read
+    err.release();
+    if (rc != SQB_OK) {
+        sqb_nhood_destroy(h);
+        return rc;
+    }
+    // from here on the handle's own copy is all that is read: the chain of the host path
+    SQB_TRY(nhood_prepare(h, where));
     *out = h;
     return SQB_OK;
 }

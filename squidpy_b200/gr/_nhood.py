@@ -18,8 +18,9 @@ from typing import Any, NamedTuple
 import numpy as np
 
 from .._constants import Key
+from .._device import DevGraph, DevSparse, array_device, device_graph, graph_args, graph_value_code
 from .._dist import nccl_cuda, sequential_stats, shard_range, shared_seed, stats_device, world
-from .._lib import Context, check, default_context, load
+from .._lib import Context, check, default_context, load, pointer_device
 from .._rng import spawn_states
 from .._validators import assert_categorical_obs, assert_connectivity_key, assert_positive, extract_adata_if_sdata
 from ._utils import _save_data, as_csr, category_codes, logg
@@ -65,6 +66,28 @@ class NhoodPlan:
         )
         self._h = h
         self.n_perms = 0
+
+    @classmethod
+    def from_device(cls, graph: DevGraph, n_cls: int, ctx: Context | None = None) -> "NhoodPlan":
+        """Plan over a neighbour graph already in GPU memory (``graph_args`` of a cupy-style or torch CSR / CSC).  The library
+        converts and validates it into its own copy on the device and never reads it on the host.  The caller may free the
+        graph when this returns.  For a CSC graph the plan holds the transpose: its counts are the transposes of the
+        graph's (``graph.transposed``)."""
+        self = cls.__new__(cls)
+        self._h = None
+        self._lib = load()
+        self.ctx = ctx or default_context()
+        self.indptr = self.indices = None  # no host copy
+        self.n = graph.n
+        self.n_cls = int(n_cls)
+        h = C.c_void_p()
+        check(
+            self._lib.sqb_nhood_create_device(self.ctx.handle, graph.n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None,
+                                              graph.index_bits, self.n_cls, graph.stream, C.byref(h))
+        )
+        self._h = h
+        self.n_perms = 0
+        return self
 
     def set_option(self, key: str, value: int) -> None:
         check(self._lib.sqb_nhood_set_option(self._h, key.encode(), int(value)))
@@ -173,6 +196,14 @@ class NhoodPlan:
             pass
 
 
+def _graph_device(d: DevSparse, device: int | None) -> int:
+    """The CUDA device holding a device graph; an explicit ``device`` must name it."""
+    on = array_device(d, pointer_device)
+    if device is not None and int(device) != on:
+        raise ValueError(f"`device={device}` does not match the device of the connectivity graph, cuda:{on}.")
+    return on
+
+
 def nhood_enrichment(
     adata: Any,
     cluster_key: str,
@@ -207,7 +238,11 @@ def nhood_enrichment(
     assert_connectivity_key(adata, connectivity_key)
     assert_positive(n_perms, name="n_perms")
 
-    adj = as_csr(adata.obsp[connectivity_key])
+    # a graph in GPU memory is read there (converted into the plan's own copy); a host graph goes through scipy as before
+    dev = device_graph(adata.obsp[connectivity_key])
+    graph = None if dev is None else graph_args(dev, adata.shape[0])
+    if dev is None:
+        adj = as_csr(adata.obsp[connectivity_key])
     int_clust, n_cls = category_codes(adata.obs[cluster_key], dtype=np.uint32)
     if n_cls <= 1:
         raise ValueError(f"Expected at least `2` clusters, found `{n_cls}`.")  # _nhood.py:107-108
@@ -222,6 +257,8 @@ def nhood_enrichment(
     if rng not in ("numpy", "philox"):
         raise ValueError(f"Expected `rng` to be 'numpy' or 'philox', found `{rng!r}`.")
     start = time.perf_counter()
+    if graph is not None:
+        device = _graph_device(dev, device)
     ctx = default_context(device)
     rank, ws = world()
     lo, hi = shard_range(int(n_perms), rank, ws)
@@ -234,7 +271,7 @@ def nhood_enrichment(
         spawner = threading.Thread(target=lambda: states_box.append(spawn_states(seed, int(n_perms), lo, hi)), daemon=True)
         spawner.start()
     with ctx.lock:
-        plan = NhoodPlan(adj.indptr, adj.indices, n_cls, ctx)
+        plan = NhoodPlan(adj.indptr, adj.indices, n_cls, ctx) if graph is None else NhoodPlan.from_device(graph, n_cls, ctx)
         try:
             count = plan.count(int_clust)
             logg.info("Calculating neighborhood enrichment on cuda:%d (rank %d/%d, permutations %d..%d)", ctx.device, rank, ws, lo, hi)
@@ -266,6 +303,10 @@ def nhood_enrichment(
                 mean, std = sequential_stats(sums_local, step, int(n_perms))
         finally:
             plan.close()
+    if graph is not None and graph.transposed:
+        # the plan held the CSC graph's transpose: every per-permutation count is transposed, hence count, mean and std
+        # bin for bin
+        count, mean, std = (np.ascontiguousarray(a.T) for a in (count, mean, std))
     with np.errstate(divide="ignore", invalid="ignore"):
         zscore = (count - mean) / std  # _nhood.py:231 (no zero-std guard there either)
 
@@ -304,27 +345,41 @@ def interaction_matrix(
     codes = np.ascontiguousarray(cats.array.codes, dtype=np.int32)  # -1 == NaN label
     if not (codes >= 0).any():
         raise RuntimeError(f"After removing NaNs in `adata.obs[{cluster_key!r}]`, none remain.")  # _nhood.py:391-392
-    g = as_csr(adata.obsp[connectivity_key])
+    dev = device_graph(adata.obsp[connectivity_key])
+    if dev is None:
+        g = as_csr(adata.obsp[connectivity_key])
+        value_dtype = g.dtype
+    else:  # read in place on the device
+        graph = graph_args(dev, adata.shape[0])
+        value_dtype = dev.data.dtype
+        device = _graph_device(dev, device)
     n_cats = len(cats.cat.categories)
-    int_graph = bool(pd.api.types.is_bool_dtype(g.dtype) or pd.api.types.is_integer_dtype(g.dtype))
+    int_graph = bool(pd.api.types.is_bool_dtype(value_dtype) or pd.api.types.is_integer_dtype(value_dtype))
 
     ctx = default_context(device)
     lib = load()
-    indptr, indices = _as_u32(g.indptr), _as_u32(g.indices)
     if weights:
-        data = g.data
-        if data.dtype not in (np.float32, np.float64):
-            data = data.astype(np.float64)  # integer / bool weights are summed exactly in float64 (< 2^53)
-        data = np.ascontiguousarray(data)
         out = np.zeros((n_cats, n_cats), dtype=np.float64)
-        check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
-                                         data.ctypes.data, 0 if data.dtype == np.float32 else 1, codes.ctypes.data, n_cats,
-                                         out.ctypes.data, None))
+        if dev is not None:
+            _interaction_device(lib, ctx, graph, codes, n_cats, out, None)
+        else:
+            indptr, indices = _as_u32(g.indptr), _as_u32(g.indices)
+            data = g.data
+            if data.dtype not in (np.float32, np.float64):
+                data = data.astype(np.float64)  # integer / bool weights are summed exactly in float64 (< 2^53)
+            data = np.ascontiguousarray(data)
+            check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
+                                             data.ctypes.data, 0 if data.dtype == np.float32 else 1, codes.ctypes.data, n_cats,
+                                             out.ctypes.data, None))
         output = np.rint(out).astype(np.int64) if int_graph else out
     else:
         cnt = np.zeros((n_cats, n_cats), dtype=np.int64)
-        check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
-                                         None, 0, codes.ctypes.data, n_cats, None, cnt.ctypes.data))
+        if dev is not None:
+            _interaction_device(lib, ctx, graph, codes, n_cats, None, cnt)
+        else:
+            indptr, indices = _as_u32(g.indptr), _as_u32(g.indices)
+            check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
+                                             None, 0, codes.ctypes.data, n_cats, None, cnt.ctypes.data))
         output = cnt if int_graph else cnt.astype(np.float64)
     if normalized:
         with np.errstate(divide="ignore", invalid="ignore"):
@@ -333,3 +388,19 @@ def interaction_matrix(
         return output
     _save_data(adata, attr="uns", key=Key.uns.interaction_matrix(cluster_key), data=output)
     return None
+
+
+def _interaction_device(lib, ctx: Context, graph: DevGraph, codes: np.ndarray, n_cats: int, out_w: np.ndarray | None,
+                        out_c: np.ndarray | None) -> None:
+    """Sums (``out_w``, float64) or counts (``out_c``, int64) of a device graph into the host matrix given, read in place by
+    ``sqb_interaction_matrix_device``; transposed back for a CSC graph."""
+    vals = graph.sparse.data
+    code = graph_value_code(vals, graph.nnz) if out_w is not None else 0
+    out = out_w if out_w is not None else out_c
+    with ctx.lock:
+        check(lib.sqb_interaction_matrix_device(ctx.handle, graph.n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None,
+                                                graph.index_bits, (vals.ptr or None) if out_w is not None else None, code,
+                                                codes.ctypes.data, n_cats, None if out_w is None else out_w.ctypes.data,
+                                                None if out_c is None else out_c.ctypes.data, graph.stream))
+    if graph.transposed:
+        out[...] = out.T.copy()

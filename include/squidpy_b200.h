@@ -153,14 +153,11 @@ int sqb_nhood_shuffled_labels(sqb_nhood* h, int64_t p0, int64_t p1, uint32_t* ou
  *                    1 CTA per permutation; 2 warp per permutation; 7 two kernels (swap-target generation + list apply);
  *                    9 two kernels (swap targets partitioned by region of the array + region replay in shared memory; a
  *                    segment needing more than 16 regions or 2048-step blocks than threads makes the call use 7 instead).
- *                    0 (serial), 3 (large windows), 4 (two-warp pipeline), 5 (two kernels, ordered replay), 6 (fused list
- *                    kernel) and 8 (region replay: every random access in shared memory, one region of the array per pass)
- *                    are superseded / slower cross-check variants compiled into the TEST build only (make testvariants);
- *                    the product library answers SQB_ERR_UNSUPPORTED for them.
+ *                    Any other value is refused with SQB_ERR_INVALID.
  *   "shuffle_threads" 128/256/512/1024 (algos 1, 7), 512/1024 (9), "shuffle_r" 2/4/8 steps per thread (7),
  *   "shuffle_q"      1/2/4/8 PCG64 outputs per lane and batch (2, and the target generation of 7),
  *   "shuffle_low"    elements of every label array kept in shared memory by the apply kernel of 7 (-1 all that fits, 0 off),
- *   "shuffle_region" positions per region of 8 and 9 (0 = as many as shared memory holds; smaller values are a test hook),
+ *   "shuffle_region" positions per region of 9 (0 = as many as shared memory holds; smaller values are a test hook),
  *   "shuffle_ctas"   persistent grid size = permutations in flight (0 = occupancy x SM count),
  *   "shuffle_stagger_us" start-up stagger of the persistent CTAs, "shuffle_wfactor_x100" window = min(i/4, f*sqrt(i)),
  *   "perm_chunk"     permutations resident at once (read at the next upload), "count_algo" 0 auto / 1 shared-memory histograms /

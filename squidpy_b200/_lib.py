@@ -13,8 +13,8 @@ import threading
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# $SQB_LIB_PATH: another build of the same C ABI (the test suite points it at the build that also contains the superseded
-# replay variants, tests/native/libsquidpy_b200_testvariants.so); the package itself only ever ships libsquidpy_b200.so
+# $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
+# phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
 ABI_VERSION = 5
 

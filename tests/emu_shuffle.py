@@ -4,8 +4,9 @@ It mirrors the device algorithm phase by phase (RNG batch by jump-ahead, windowe
 hash-based conflict detection, parallel swaps + ordered serial pass) so the *algorithm* can be validated on
 the CPU against numpy's ``Generator.shuffle`` (tests/test_shuffle_emulation.py).  Not used by the product.
 
-Also here: ``resolve_window_lists`` (the serial-pass-free conflict resolution of shuffle_algo 6 / 7) and ``emu_targets``
-(nhood_jgen_kernel: batch-sized windows, one-pass acceptance), each the executable specification of its kernel.
+Also here: ``resolve_window_lists`` (the serial-pass-free conflict resolution of shuffle_algo 7), ``emu_targets``
+(nhood_jgen_kernel: batch-sized windows, one-pass acceptance) and ``_resolve_general_window`` (one window of the region replay
+of shuffle_algo 9), each the executable specification of its kernel.
 """
 from __future__ import annotations
 
@@ -43,7 +44,7 @@ def window_size(i_cur, raw_left, raw_total):
 
 
 def resolve_window_lists(a, base, i_cur, sj, rng):
-    """Conflict resolution WITHOUT a serial pass (shuffle_algo 6, nhood_shuffle_list_kernel): applies the window's steps
+    """Conflict resolution WITHOUT a serial pass (shuffle_algo 7, nhood_apply_list_kernel): applies the window's steps
     s = 0..S-1 (swap positions i_cur-s and sj[s]) to `a` in place.  Every step pushes itself on the list of the position
     it targets (arbitrary push order = thread interleaving); afterwards each step derives what it has to write from the
     lists alone, reading only ORIGINAL values:
@@ -325,7 +326,8 @@ def serial_targets(state, inc, segs):
 
 
 # ------------------------------------------------------------------------------------------------
-# Region replay (shuffle_algo 8, nhood_apply_region_kernel): executable specification
+# Region replay (shuffle_algo 9, nhood_apply_part_kernel): one window, executable specification (tests/emu_partition.py
+# feeds it the windows of every region pass)
 # ------------------------------------------------------------------------------------------------
 def _resolve_general_window(slab, a, lo, hi, tops, tgts, rng):
     """One window of the region replay: compacted steps in step order (slot s: top position tops[s], strictly descending;
@@ -373,47 +375,3 @@ def _resolve_general_window(slab, a, lo, hi, tops, tgts, rng):
     for pos, v in ws:
         slab[pos] = v
 
-
-def region_replay(arr, J, cap, NT=8, WL=4, CAPW=12, KMAX=16, rng=None, stats=None):
-    """Applies the Fisher-Yates steps i = m-1 .. 1 (swap positions i and J[i] <= i) to a copy of `arr`, one region of at most
-    `cap` positions at a time, top region first (see nhood.cu 2i): the pass of region [lo, hi) scans all steps i >= lo and
-    applies those whose TARGET lies in the region (a step whose target lies below is left to a later pass: its top then
-    still holds T(step), the value it had just before the step).  Mirrors the kernel's chunking: NT*K steps are scanned per
-    window, "warp" w (WL lanes) takes the w-th run of WL*K of them; K is sized for ~0.58 CAPW expected matches per warp and
-    halved when a warp finds more than CAPW or the window more than HS = 2*NT."""
-    rng = rng or random.Random(0)
-    a = list(arr)
-    m = len(a)
-    if m < 2:
-        return a
-    HS = 2 * NT
-    ETGT = max(1, (CAPW * 56) // 96)
-    assert 2 * WL <= CAPW
-    R = (m + cap - 1) // cap
-    B = (((m + R - 1) // R + 15) // 16) * 16
-    for r in range((m - 1) // B, -1, -1):
-        lo = r * B
-        ln = min(B, m - lo)
-        hi = lo + ln
-        slab = a[lo:hi]
-        i_min = max(lo, 1)
-        i_cur = m - 1
-        while i_cur >= i_min:
-            avail = i_cur - i_min + 1
-            K = min(KMAX, max(2, (ETGT * (i_cur + 1)) // (WL * min(ln, i_cur - lo + 1))))
-            while True:
-                SC = min(NT * K, avail)
-                match = [lo <= J[i_cur - s] < hi for s in range(SC)]
-                per_warp = [sum(match[w * WL * K:(w + 1) * WL * K]) for w in range(NT // WL)]
-                if max(per_warp) <= CAPW and sum(per_warp) <= HS:
-                    break
-                K = max(2, K >> 1)
-                if stats is not None:
-                    stats["overflow"] = stats.get("overflow", 0) + 1
-            steps = [i_cur - s for s in range(SC) if match[s]]
-            _resolve_general_window(slab, a, lo, hi, steps, [J[i] for i in steps], rng)
-            if stats is not None:
-                stats["xwin"] = stats.get("xwin", 0) + 1
-            i_cur -= SC
-        a[lo:hi] = slab
-    return a

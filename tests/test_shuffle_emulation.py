@@ -47,7 +47,7 @@ def test_emulated_cta_shuffle_segments():
 
 
 def test_list_resolution_equals_serial_swaps():
-    """The serial-pass-free conflict resolution of shuffle_algo 6 (tests/emu_shuffle.resolve_window_lists) against the
+    """The serial-pass-free conflict resolution of shuffle_algo 7 (tests/emu_shuffle.resolve_window_lists) against the
     plain in-order application of the same swaps, on windows far denser in conflicts than the device ever sees."""
     from tests.emu_shuffle import resolve_window_lists
 
@@ -136,41 +136,3 @@ def test_emulated_target_generation_segments_and_wrong_shortcut():
         wrong += emu_targets(state, inc, [(0, n)], Q=4, shortcut="flags") != serial_targets(state, inc, [(0, n)])
     assert wrong > 0
 
-
-def _fisher_yates(arr, J):
-    a = list(arr)
-    for i in range(len(a) - 1, 0, -1):
-        j = J[i]
-        a[i], a[j] = a[j], a[i]
-    return a
-
-
-def test_region_replay_equals_fisher_yates():
-    """shuffle_algo 8 (tests/emu_shuffle.region_replay = the specification of nhood_apply_region_kernel): applying every step in
-    the pass of the region its TARGET falls into -- tops above the region through compacted windows, tops inside through
-    consecutive windows, targets below deferred with T(step) left at the top -- equals the plain Fisher-Yates sweep, for any
-    region size, window size and target distribution (uniform like the real stream, and adversarial: many duplicates, many
-    own-range targets, all targets in one region)."""
-    from tests.emu_shuffle import region_replay
-
-    rnd = random.Random(5)
-    stats = {}
-    for trial in range(1500):
-        m = rnd.choice([2, 3, 5, 17, 40, 97, 200, 333])
-        mode = trial % 4
-        J = [0] * m
-        for i in range(1, m):
-            if mode == 0:
-                J[i] = rnd.randrange(i + 1)
-            elif mode == 1:  # few distinct targets: long duplicate lists
-                J[i] = min(i, rnd.choice([0, 1, 2, m // 3, m // 2]))
-            elif mode == 2:  # targets close to the top: own-range chains
-                J[i] = max(0, i - rnd.randrange(0, 4))
-            else:  # everything aims at the lowest positions: every region defers almost all of its steps
-                J[i] = rnd.randrange(min(i + 1, 6))
-        arr = [rnd.randrange(1000) for _ in range(m)]
-        cap = rnd.choice([16, 32, 48, 64, 128, 1024])
-        nt = rnd.choice([4, 8, 16])
-        got = region_replay(arr, J, cap, NT=nt, WL=rnd.choice([2, 4]), CAPW=rnd.choice([8, 12]), KMAX=rnd.choice([2, 16]), rng=rnd, stats=stats)
-        assert got == _fisher_yates(arr, J), (trial, m, cap, nt, mode)
-    assert stats.get("xwin", 0) > 1000 and stats.get("overflow", 0) > 0  # compacted windows and the halving path were exercised

@@ -1,7 +1,7 @@
 """Where a window of the region replay (shuffle_algo 9) spends its time: the phase clocks of nhood_apply_part_kernel at
 configs[1] (1M spots, 30 clusters, P permutations), in cycles per window as warp 0 of a CTA sees them.  They exist in the
-test build only (make -C squidpy_b200/csrc testvariants), which this script loads unless $SQB_LIB_PATH names another
-build with the clocks.  usage: python tools/apply_phases.py [P] [algo:threads:r[:key=value...]] ..."""
+clocks build only (tools/native/libsquidpy_b200_clocks.so, make -C squidpy_b200/csrc clocks), which this script loads unless
+$SQB_LIB_PATH names another build with the clocks.  usage: python tools/apply_phases.py [P] [algo:threads:r[:key=value...]] ..."""
 import ctypes as C
 import os
 import sys
@@ -9,7 +9,7 @@ import sys
 import numpy as np
 
 sys.path.insert(0, ".")
-os.environ.setdefault("SQB_LIB_PATH", os.path.abspath("tests/native/libsquidpy_b200_testvariants.so"))
+os.environ.setdefault("SQB_LIB_PATH", os.path.abspath("tools/native/libsquidpy_b200_clocks.so"))
 import squidpy_b200 as sq  # noqa: E402
 from squidpy_b200 import _lib  # noqa: E402
 from squidpy_b200._rng import spawn_states  # noqa: E402

@@ -43,9 +43,6 @@ def main():
                 for stagger in (0, 1500, 2500, 4000):
                     variants.append({**base, "shuffle_algo": 7, "shuffle_threads": nt, "shuffle_r": r, "shuffle_low": low,
                                      "shuffle_ctas": ctas, "shuffle_stagger_us": stagger})
-    if os.environ.get("SQB_LIB_PATH", "").endswith("testvariants.so"):  # superseded variants exist in the test build only
-        variants.append({**base, "shuffle_algo": 6, "shuffle_threads": 1024, "shuffle_r": 2, "shuffle_wfactor_x100": 1600})
-        variants.append({**base, "shuffle_algo": 5, "shuffle_threads": 512, "shuffle_r": 2})
     variants.append({**base, "shuffle_algo": 2})
     variants.append({**base, "shuffle_algo": 1, "shuffle_threads": 1024})
     for v in variants:

@@ -23,6 +23,7 @@
  *   sqb_ligrec_counts          <- _score_permutations(data, clustering, generators, ...)  src/squidpy/gr/_ligrec.py:616-676
  *   sqb_sepal                  <- _diffusion(conc, use_hex, n_iter, sat, sat_idx, unsat, unsat_idx, dt, thresh)  src/squidpy/gr/_sepal.py:186-233
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
+ *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
  */
 #ifndef SQUIDPY_B200_H
@@ -35,7 +36,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 5
+#define SQB_ABI_VERSION 6
 
 typedef enum {
     SQB_OK = 0,
@@ -292,6 +293,34 @@ int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_id
  * `capacity` >= nnz entries the rows are filled in ascending column order.                                                 */
 int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int64_t* out_indptr, int32_t* out_idx,
                   double* out_dist, int64_t capacity, int64_t* nnz_out);
+
+/* ---- spatial neighbour graphs from coordinates in GPU memory, kept there ---------------------------------------------
+ * The whole builder on the device: search, cut, ring expansion, diagonals, interval / percentile pruning, eliminate_zeros,
+ * transform and the library block diagonal of KNNBuilder / GridBuilder / RadiusBuilder.build and GraphBuilderCSR.combine
+ * (src/squidpy/gr/neighbors.py:80-156, :192-209, :253-270, :365-419, :423-477).  The result equals the host builders' after
+ * sort_indices(), bit for bit.
+ *   xy: DEVICE pointer on the context's device to n x 2 coordinates, xy_dtype 0 float32 / 1 float64, element strides
+ *   stride_row / stride_col (any); never read on the host.  producer_stream: as in sqb_autocorr_load_csr_device.
+ *   kind 0 kNN (n_neighbors in [1, 64]), 1 grid (n_neighbors, n_rings >= 1, 1.3 x median cut), 2 radius (radius; interval != 0
+ *   prunes to [radius_min, radius_max] like a tuple radius).  set_diag as the builders'.  percentile: NaN for none (kNN /
+ *   radius).  transform 0 none, 1 spectral, 2 cosine.
+ *   lib_ptr / lib_rows (HOST, or NULL with n_libs = 0): library b is the ascending rows lib_rows[lib_ptr[b] .. lib_ptr[b+1]) of
+ *   the coordinates; each is built as its own block, the blocks are combined in the order of the rows.
+ * Returns a handle with *n_out rows (n, or the rows the libraries list), the entry counts of the connectivities (float32
+ * values) and the distances (float64 values if *dst_f64, else float32).  Errors (non-finite coordinates, k >= n, ...) carry
+ * the host path's messages and leave the context usable.                                                              */
+typedef struct sqb_graph sqb_graph;
+int sqb_graph_build_device(sqb_ctx* ctx, const void* xy, int xy_dtype, int64_t n, int64_t stride_row, int64_t stride_col,
+                           uintptr_t producer_stream, int kind, int n_neighbors, int n_rings, double radius, int interval,
+                           double radius_min, double radius_max, int set_diag, double percentile, int transform,
+                           const int64_t* lib_ptr, const int32_t* lib_rows, int n_libs, sqb_graph** out, int64_t* n_out,
+                           int64_t* adj_nnz, int64_t* dst_nnz, int* dst_f64);
+/* Writes both CSR matrices into caller-allocated DEVICE buffers: indptr n_out + 1 int32, indices nnz int32, data nnz values.
+ * consumer_stream (CUDA Array Interface convention) is the stream that allocated the buffers; it is waited on before the
+ * copies.  The buffers are complete when the call returns.                                                             */
+int sqb_graph_export(sqb_graph* g, int32_t* adj_indptr, int32_t* adj_indices, float* adj_data, int32_t* dst_indptr,
+                     int32_t* dst_indices, void* dst_data, uintptr_t consumer_stream);
+int sqb_graph_free(sqb_graph* g);
 
 #ifdef __cplusplus
 }

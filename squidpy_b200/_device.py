@@ -242,6 +242,12 @@ def _host_array(a: Any) -> np.ndarray:
     return torch.as_tensor(a, device="cuda").cpu().numpy()
 
 
+def on_host(m: Any) -> Any:
+    """``m`` itself when it is a host object, else its host copy (``to_host_matrix``): for the readers of ``obsm`` / ``obsp``
+    that stage small arrays (coordinates, a neighbour graph) on the host anyway."""
+    return m if device_matrix(m) is None else to_host_matrix(m)
+
+
 def to_host_matrix(m: Any) -> Any:
     """Host copy of a device-resident matrix (numpy for dense, scipy CSR / CSC for sparse): for the weight matrix, which is
     small next to X and whose moments, S0 and row normalisation are computed on the host."""

@@ -17,12 +17,7 @@
 #include <cub/device/device_scan.cuh>
 #include <math.h>
 
-#include "common.cuh"
-
-struct GridGeom {
-    double x0, y0, inv_cell, cell;
-    int gx, gy;
-};
+#include "graph.cuh"
 
 __device__ __forceinline__ int grid_cell_coord(double v, double v0, double inv, int g) {
     int c = (int)floor((v - v0) * inv);
@@ -189,27 +184,7 @@ __global__ void __launch_bounds__(128) graph_radius_kernel(const double2* __rest
 }
 
 // ================================================================================================
-struct PointGrid {
-    GridGeom gm;
-    DevBuf<double> d_xy;
-    DevBuf<double2> d_pts;
-    DevBuf<int32_t> d_idx_sorted, d_cell_start;
-    void release() {
-        d_xy.release();
-        d_pts.release();
-        d_idx_sorted.release();
-        d_cell_start.release();
-    }
-};
-
-// bucket n points into square cells of edge `cell` (clamped so that the grid has at most ~4n + 16 cells)
-static int build_grid(sqb_ctx* c, const double* xy, int64_t n, double cell_hint, double pts_per_cell, PointGrid* g) {
-    double x0 = INFINITY, y0 = INFINITY, x1 = -INFINITY, y1 = -INFINITY;
-    for (int64_t i = 0; i < n; ++i) {
-        const double x = xy[2 * i], y = xy[2 * i + 1];
-        SQB_CHECK(isfinite(x) && isfinite(y), SQB_ERR_INVALID, "coordinates of observation %lld are not finite", (long long)i);
-        x0 = x < x0 ? x : x0, x1 = x > x1 ? x : x1, y0 = y < y0 ? y : y0, y1 = y > y1 ? y : y1;
-    }
+GridGeom grid_geometry(double x0, double y0, double x1, double y1, int64_t n, double cell_hint, double pts_per_cell) {
     const double w = x1 - x0, h = y1 - y0;
     double cell = cell_hint;
     if (!(cell > 0.0)) {
@@ -227,7 +202,11 @@ static int build_grid(sqb_ctx* c, const double* xy, int64_t n, double cell_hint,
     GridGeom gm;
     gm.x0 = x0, gm.y0 = y0, gm.cell = cell, gm.inv_cell = 1.0 / cell;
     gm.gx = (int)(floor(w / cell) + 1.0), gm.gy = (int)(floor(h / cell) + 1.0);
-    g->gm = gm;
+    return gm;
+}
+
+int grid_bucket(sqb_ctx* c, int64_t n, PointGrid* g) {
+    const GridGeom gm = g->gm;
     const int64_t n_cells = (int64_t)gm.gx * gm.gy;
     DevBuf<uint32_t> cell_a, cell_b;
     DevBuf<int32_t> idx_a;
@@ -235,17 +214,14 @@ static int build_grid(sqb_ctx* c, const double* xy, int64_t n, double cell_hint,
     cell_a.bind(c->stream), cell_b.bind(c->stream), idx_a.bind(c->stream), tmp.bind(c->stream);
     auto cleanup = [&]() { cell_a.release(), cell_b.release(), idx_a.release(), tmp.release(); };
     int rc;
-    if ((rc = g->d_xy.alloc(2 * n)) || (rc = g->d_pts.alloc(n)) || (rc = g->d_idx_sorted.alloc(n)) || (rc = g->d_cell_start.alloc(n_cells + 1)) ||
-        (rc = cell_a.alloc(n)) || (rc = cell_b.alloc(n)) || (rc = idx_a.alloc(n))) {
+    if ((rc = g->d_pts.alloc(n)) || (rc = g->d_idx_sorted.alloc(n)) || (rc = g->d_cell_start.alloc(n_cells + 1)) || (rc = cell_a.alloc(n)) ||
+        (rc = cell_b.alloc(n)) || (rc = idx_a.alloc(n))) {
         cleanup();
         return rc;
     }
-    cudaError_t e = cudaMemcpyAsync(g->d_xy.p, xy, 2 * n * sizeof(double), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        c->launches += 1;
-        graph_cell_id_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, c->stream>>>(g->d_xy.p, n, gm, cell_a.p, idx_a.p);
-        e = cudaGetLastError();
-    }
+    c->launches += 1;
+    graph_cell_id_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, c->stream>>>(g->d_xy.p, n, gm, cell_a.p, idx_a.p);
+    cudaError_t e = cudaGetLastError();
     int bits = 1;
     while (bits < 32 && ((uint64_t)(n_cells - 1) >> bits) != 0) ++bits;
     size_t tmp_bytes = 0;
@@ -265,6 +241,60 @@ static int build_grid(sqb_ctx* c, const double* xy, int64_t n, double cell_hint,
     return SQB_OK;
 }
 
+// host coordinates: bounding box and finiteness on the host, then upload and bucket
+static int build_grid(sqb_ctx* c, const double* xy, int64_t n, double cell_hint, double pts_per_cell, PointGrid* g) {
+    double x0 = INFINITY, y0 = INFINITY, x1 = -INFINITY, y1 = -INFINITY;
+    for (int64_t i = 0; i < n; ++i) {
+        const double x = xy[2 * i], y = xy[2 * i + 1];
+        SQB_CHECK(isfinite(x) && isfinite(y), SQB_ERR_INVALID, "coordinates of observation %lld are not finite", (long long)i);
+        x0 = x < x0 ? x : x0, x1 = x > x1 ? x : x1, y0 = y < y0 ? y : y0, y1 = y > y1 ? y : y1;
+    }
+    g->gm = grid_geometry(x0, y0, x1, y1, n, cell_hint, pts_per_cell);
+    SQB_TRY(g->d_xy.alloc(2 * n));
+    cudaError_t e = cudaMemcpyAsync(g->d_xy.p, xy, 2 * n * sizeof(double), cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) {
+        sqb_set_error("spatial grid: %s", cudaGetErrorString(e));
+        return SQB_ERR_CUDA;
+    }
+    return grid_bucket(c, n, g);
+}
+
+cudaError_t knn_launch(sqb_ctx* c, const PointGrid& g, int64_t n, int k, int32_t* idx, double* dist) {
+    SqbLaunchScope scope(c, SQB_K_MISC);
+    const unsigned grid = (unsigned)ceil_div64(n, 128);
+    if (k <= 8)
+        graph_knn_kernel<8><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, idx, dist);
+    else if (k <= 16)
+        graph_knn_kernel<16><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, idx, dist);
+    else if (k <= 32)
+        graph_knn_kernel<32><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, idx, dist);
+    else
+        graph_knn_kernel<64><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, idx, dist);
+    return cudaGetLastError();
+}
+
+cudaError_t median_enqueue(sqb_ctx* c, const double* dist, int64_t m, DevBuf<double>& sorted, DevBuf<uint8_t>& tmp, double* med) {
+    // np.median of all m distances: radix sort, the middle element (odd count) or the mean of the two middle ones
+    cudaError_t e = cudaSuccess;
+    size_t tmp_bytes = 0;
+    if (sorted.alloc((size_t)m) != SQB_OK) e = cudaErrorMemoryAllocation;
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, dist, sorted.p, (int)m, 0, 64, c->stream);
+    if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, dist, sorted.p, (int)m, 0, 64, c->stream);
+    c->launches += 1;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&med[0], sorted.p + (m - 1) / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&med[1], sorted.p + m / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream);
+    return e;
+}
+
+cudaError_t radius_launch(sqb_ctx* c, const PointGrid& g, int64_t n, double radius, int64_t* counts, const int64_t* indptr, int32_t* idx,
+                          double* dist) {
+    SqbLaunchScope scope(c, SQB_K_MISC);
+    graph_radius_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, radius,
+                                                                             radius_reach(radius, g.gm), counts, indptr, idx, dist);
+    return cudaGetLastError();
+}
+
 extern "C" {
 
 int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_idx, double* out_dist, double* median_out) {
@@ -278,8 +308,8 @@ int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_id
     sqb_ctx* c = ctx;
     SQB_CUDA(cudaSetDevice(c->device));
     PointGrid g;
-    g.d_xy.bind(c->stream), g.d_pts.bind(c->stream), g.d_idx_sorted.bind(c->stream), g.d_cell_start.bind(c->stream);
-    int rc = build_grid(c, xy, n, 0.0, k <= 8 ? 2.5 : (double)k / 3.0, &g);
+    g.bind(c->stream);
+    int rc = build_grid(c, xy, n, 0.0, knn_pts_per_cell(k), &g);
     if (rc != SQB_OK) {
         g.release();
         return rc;
@@ -293,32 +323,9 @@ int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_id
         cleanup();
         return rc;
     }
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        const unsigned grid = (unsigned)ceil_div64(n, 128);
-        if (k <= 8)
-            graph_knn_kernel<8><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, d_idx.p, d_dist.p);
-        else if (k <= 16)
-            graph_knn_kernel<16><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, d_idx.p, d_dist.p);
-        else if (k <= 32)
-            graph_knn_kernel<32><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, d_idx.p, d_dist.p);
-        else
-            graph_knn_kernel<64><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, d_idx.p, d_dist.p);
-    }
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = knn_launch(c, g, n, k, d_idx.p, d_dist.p);
     double med[2] = {0.0, 0.0};
-    if (e == cudaSuccess && median_out) {
-        // np.median of all n*k distances: radix sort, the middle element (odd count) or the mean of the two middle ones
-        const int64_t m = n * k;
-        size_t tmp_bytes = 0;
-        if (d_sorted.alloc((size_t)m) != SQB_OK) e = cudaErrorMemoryAllocation;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, d_dist.p, d_sorted.p, (int)m, 0, 64, c->stream);
-        if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, d_dist.p, d_sorted.p, (int)m, 0, 64, c->stream);
-        c->launches += 1;
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&med[0], d_sorted.p + (m - 1) / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&med[1], d_sorted.p + m / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    }
+    if (e == cudaSuccess && median_out) e = median_enqueue(c, d_dist.p, n * k, d_sorted, tmp, med);
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_idx, d_idx.p, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, d_dist.p, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -339,14 +346,12 @@ int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int6
     sqb_ctx* c = ctx;
     SQB_CUDA(cudaSetDevice(c->device));
     PointGrid g;
-    g.d_xy.bind(c->stream), g.d_pts.bind(c->stream), g.d_idx_sorted.bind(c->stream), g.d_cell_start.bind(c->stream);
+    g.bind(c->stream);
     int rc = build_grid(c, xy, n, radius > 0.0 ? radius : 0.0, 2.5, &g);
     if (rc != SQB_OK) {
         g.release();
         return rc;
     }
-    // the grid may have been coarsened (cell >= radius) or not (cell hint 0): cells to look at on every side
-    const int reach = (int)ceil(radius / g.gm.cell * (1.0 + 1e-12));
     DevBuf<int64_t> d_cnt, d_ptr;
     DevBuf<int32_t> d_idx;
     DevBuf<double> d_dist;
@@ -358,12 +363,7 @@ int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int6
         return rc;
     }
     cudaError_t e = cudaMemsetAsync(d_cnt.p, 0, (n + 1) * sizeof(int64_t), c->stream);
-    const unsigned grid = (unsigned)ceil_div64(n, 128);
-    if (e == cudaSuccess) {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        graph_radius_kernel<<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, radius, reach, d_cnt.p, nullptr, nullptr, nullptr);
-        e = cudaGetLastError();
-    }
+    if (e == cudaSuccess) e = radius_launch(c, g, n, radius, d_cnt.p, nullptr, nullptr, nullptr);
     size_t tmp_bytes = 0;
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_cnt.p, d_ptr.p, (int)(n + 1), c->stream);
     if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
@@ -386,11 +386,7 @@ int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int6
             cleanup();
             return rc;
         }
-        {
-            SqbLaunchScope scope(c, SQB_K_MISC);
-            graph_radius_kernel<<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, radius, reach, nullptr, d_ptr.p, d_idx.p, d_dist.p);
-            e = cudaGetLastError();
-        }
+        e = radius_launch(c, g, n, radius, nullptr, d_ptr.p, d_idx.p, d_dist.p);
         if (e == cudaSuccess) e = cudaMemcpyAsync(out_idx, d_idx.p, (size_t)nnz * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, d_dist.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);

@@ -9,6 +9,11 @@ seconds where the statistics now cost milliseconds.  The neighbour search runs o
 reference's scipy code on the host.  Output contract as in the reference: ``obsp['{key}_connectivities']`` CSR float32,
 ``obsp['{key}_distances']`` CSR, ``uns['{key}_neighbors']`` with the parameters.  Delaunay-based graphs are not offered
 (Qhull has no counterpart here); they raise ``NotImplementedError``.
+
+Coordinates already in GPU memory (a torch CUDA tensor or any ``__cuda_array_interface__`` exporter of shape (n, 2), float32
+or float64, any strides) take the device path instead (``sqb_graph_build_device``): search AND post-processing run on the
+GPU and both matrices are returned as torch ``sparse_csr`` CUDA tensors (int32 indices, ascending columns) that equal the
+host path's result after ``sort_indices()`` bit for bit.  The coordinates are never read on the host.
 """
 
 from __future__ import annotations
@@ -21,7 +26,8 @@ import numpy as np
 from scipy.sparse import block_diag, csr_matrix
 
 from .._constants import CoordType, Key, Transform
-from .._lib import Context, check, default_context, load
+from .._device import DevArray, _torch_stream, array_device, device_matrix
+from .._lib import Context, check, default_context, load, pointer_device
 from .._validators import assert_categorical_obs, assert_positive, assert_spatial_basis, extract_adata_if_sdata
 from ._utils import _save_data, logg
 
@@ -75,6 +81,23 @@ def radius_2d(coords, radius: float, *, ctx: Context | None = None):
         dist = np.empty(max(nnz.value, 1), dtype=np.float64)
         check(lib.sqb_radius_2d(ctx.handle, xy.ctypes.data, n, float(radius), indptr.ctypes.data, idx.ctypes.data, dist.ctypes.data, idx.size, C.byref(nnz)))
     return indptr, idx[: nnz.value], dist[: nnz.value]
+
+
+def _device_coords(coords) -> DevArray | None:
+    """The device description of coordinates in GPU memory, or ``None`` for host coordinates."""
+    d = device_matrix(coords)
+    if d is None:
+        return None
+    if not isinstance(d, DevArray):
+        raise NotImplementedError("Spatial coordinates must be a dense (n, 2) array, found a sparse device matrix.")
+    if len(d.shape) != 2 or d.shape[1] != 2:
+        raise ValueError(f"Expected device coordinates of shape `(n, 2)`, found `{d.shape}`.")
+    if d.dtype not in (np.dtype(np.float32), np.dtype(np.float64)):
+        raise TypeError(f"Device coordinates of dtype `{d.dtype}` are not supported; use float32 or float64.")
+    return d
+
+
+_TRANSFORM_CODES = {Transform.NONE: 0, Transform.SPECTRAL: 1, Transform.COSINE: 2}
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -148,7 +171,50 @@ class _Builder:
             adj.setdiag(1.0 if self.set_diag else adj.diagonal())
             dst.setdiag(0.0)
 
+    def _device_args(self) -> tuple[int, int, int, float, tuple[float, float] | None]:  # pragma: no cover
+        """(kind, n_neighbors, n_rings, radius, interval) of ``sqb_graph_build_device``."""
+        raise NotImplementedError
+
+    def build_device(self, d: DevArray, device: int | None = None, libraries: tuple[np.ndarray, np.ndarray] | None = None):
+        """The graph of device coordinates ``d`` on their device (an explicit ``device`` must name it) as torch ``sparse_csr``
+        CUDA tensors; ``libraries = (ptr int64, rows int32)`` builds every library's rows as its own block."""
+        import torch
+
+        on = array_device(d, pointer_device)
+        if device is not None and int(device) != on:
+            raise ValueError(f"`device={device}` does not match the device of the spatial coordinates, cuda:{on}.")
+        ctx = self.ctx if self.ctx is not None and self.ctx.device == on else default_context(on)
+        kind, k, n_rings, radius, interval = self._device_args()
+        lo, hi = interval if interval is not None else (0.0, 0.0)
+        pct = np.nan if self.percentile is None else float(self.percentile)
+        lp, lr, n_libs = (None, None, 0) if libraries is None else (libraries[0].ctypes.data, libraries[1].ctypes.data, libraries[0].size - 1)
+        lib = load()
+        h, n_out, nnz_a, nnz_d, f64 = C.c_void_p(), C.c_int64(), C.c_int64(), C.c_int64(), C.c_int()
+        with ctx.lock:
+            check(lib.sqb_graph_build_device(ctx.handle, d.ptr, int(d.dtype == np.float64), d.shape[0], d.strides[0], d.strides[1], d.stream, kind, k,
+                                             n_rings, float(radius), int(interval is not None), float(lo), float(hi), int(bool(self.set_diag)), pct,
+                                             _TRANSFORM_CODES[self.transform], lp, lr, n_libs, C.byref(h), C.byref(n_out), C.byref(nnz_a),
+                                             C.byref(nnz_d), C.byref(f64)))
+            try:
+                n, dev = n_out.value, torch.device("cuda", on)
+                parts = [torch.empty(n + 1, dtype=torch.int32, device=dev), torch.empty(nnz_a.value, dtype=torch.int32, device=dev),
+                         torch.empty(nnz_a.value, dtype=torch.float32, device=dev), torch.empty(n + 1, dtype=torch.int32, device=dev),
+                         torch.empty(nnz_d.value, dtype=torch.int32, device=dev),
+                         torch.empty(nnz_d.value, dtype=torch.float64 if f64.value else torch.float32, device=dev)]
+                check(lib.sqb_graph_export(h, *(t.data_ptr() or None for t in parts), _torch_stream(parts[0])))
+            finally:
+                lib.sqb_graph_free(h)
+        adj = torch.sparse_csr_tensor(parts[0], parts[1], parts[2], size=(n, n))
+        dst = torch.sparse_csr_tensor(parts[3], parts[4], parts[5], size=(n, n))
+        return adj, dst
+
     def build(self, coords) -> tuple[csr_matrix, csr_matrix]:
+        d = _device_coords(coords)
+        if d is not None:
+            return self.build_device(d, None if self.ctx is None else self.ctx.device)
+        return self._build_host(coords)
+
+    def _build_host(self, coords) -> tuple[csr_matrix, csr_matrix]:
         import warnings
 
         from scipy.sparse import SparseEfficiencyWarning
@@ -199,6 +265,9 @@ class KNNBuilder(_Builder):
     def uns_params(self) -> dict[str, Any]:
         return {"coord_type": CoordType.GENERIC.v, "n_neighbors": self.n_neighs, "transform": self.transform.v}
 
+    def _device_args(self):
+        return 0, int(self.n_neighs), 1, 0.0, None
+
     def build_graph(self, coords):
         dist, idx = knn_2d(coords, self.n_neighs, ctx=self.ctx)
         n = idx.shape[0]
@@ -220,6 +289,10 @@ class RadiusBuilder(_Builder):
 
     def uns_params(self) -> dict[str, Any]:
         return {"coord_type": CoordType.GENERIC.v, "radius": self.radius, "transform": self.transform.v}
+
+    def _device_args(self):
+        r = self.radius if isinstance(self.radius, int | float) else max(self.radius)
+        return 2, 0, 1, r, self._interval()
 
     def build_graph(self, coords):
         r = self.radius if isinstance(self.radius, int | float) else max(self.radius)
@@ -248,6 +321,9 @@ class GridBuilder(_Builder):
     def uns_params(self) -> dict[str, Any]:
         return {"coord_type": CoordType.GRID.v, "n_neighbors": self.n_neighs, "n_rings": self.n_rings, "delaunay": self.delaunay,
                 "transform": self.transform.v}
+
+    def _device_args(self):
+        return 1, int(self.n_neighs), int(self.n_rings), 0.0, None
 
     def _base_adjacency(self, coords, *, set_diag: bool) -> csr_matrix:
         dist, idx, med = knn_2d(coords, self.n_neighs, median=True, ctx=self.ctx)
@@ -283,10 +359,30 @@ class GridBuilder(_Builder):
 # ---------------------------------------------------------------------------------------------------------
 # public functions
 # ---------------------------------------------------------------------------------------------------------
-def _run(adata, builder: _Builder, *, spatial_key: str, library_key: str | None, key_added: str, copy: bool):
+def _library_rows(adata, library_key: str | None) -> tuple[np.ndarray, np.ndarray] | None:
+    """The observations of every library (the host path's ``np.where(codes == code)``) as (ptr int64, rows int32)."""
+    if library_key is None:
+        return None
+    assert_categorical_obs(adata, key=library_key)
+    codes = np.asarray(adata.obs[library_key].array.codes)
+    n_libs = len(adata.obs[library_key].cat.categories)
+    if n_libs == 0:
+        raise ValueError(f"`adata.obs[{library_key!r}]` has no categories.")
+    rows = np.argsort(codes, kind="stable").astype(np.int32)
+    counts = np.bincount(codes[codes >= 0], minlength=n_libs)
+    ptr = np.zeros(n_libs + 1, dtype=np.int64)
+    np.cumsum(counts, out=ptr[1:])
+    skip = int((codes < 0).sum())  # observations without a library belong to no block
+    return ptr, np.ascontiguousarray(rows[skip:])
+
+
+def _run(adata, builder: _Builder, *, spatial_key: str, library_key: str | None, key_added: str, copy: bool, device: int | None = None):
     """``_run_spatial_neighbors`` (``_build.py:789-850``)."""
     start = time.perf_counter()
-    if library_key is not None:
+    dev = _device_coords(adata.obsm[spatial_key])
+    if dev is not None:
+        adj, dst = builder.build_device(dev, device, _library_rows(adata, library_key))
+    elif library_key is not None:
         assert_categorical_obs(adata, key=library_key)
         libs = adata.obs[library_key].cat.categories
         codes = np.asarray(adata.obs[library_key].array.codes)
@@ -312,6 +408,11 @@ def _run(adata, builder: _Builder, *, spatial_key: str, library_key: str | None,
     return None
 
 
+def _host_context(adata, spatial_key: str, device: int | None) -> Context | None:
+    """The context of the host path; device coordinates are built on their own device (``_Builder.build_device``)."""
+    return None if _device_coords(adata.obsm[spatial_key]) is not None else default_context(device)
+
+
 def _prepare(data, spatial_key, table_key):
     adata = extract_adata_if_sdata(data, table_key=table_key)
     assert_spatial_basis(adata, spatial_key)
@@ -323,8 +424,10 @@ def spatial_neighbors_knn(data: Any, *, spatial_key: str = Key.obsm.spatial, ele
                           transform=None, set_diag: bool = False, key_added: str = "spatial", copy: bool = False, n_jobs: int = 1,
                           device: int | None = None) -> SpatialNeighborsResult | None:
     """k-nearest-neighbour graph from spatial coordinates (``_build.py:484-549``); ``n_jobs`` is accepted and ignored."""
-    builder = KNNBuilder(n_neighs=n_neighs, percentile=percentile, transform=transform, set_diag=set_diag, ctx=default_context(device))
-    return _run(_prepare(data, spatial_key, table_key), builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy)
+    adata = _prepare(data, spatial_key, table_key)
+    builder = KNNBuilder(n_neighs=n_neighs, percentile=percentile, transform=transform, set_diag=set_diag, ctx=_host_context(adata, spatial_key, device))
+    return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy,
+                device=device)
 
 
 def spatial_neighbors_radius(data: Any, *, spatial_key: str = Key.obsm.spatial, elements_to_coordinate_systems: dict[str, str] | None = None,
@@ -332,8 +435,10 @@ def spatial_neighbors_radius(data: Any, *, spatial_key: str = Key.obsm.spatial, 
                              percentile: float | None = None, transform=None, set_diag: bool = False, key_added: str = "spatial",
                              copy: bool = False, n_jobs: int = 1, device: int | None = None) -> SpatialNeighborsResult | None:
     """Radius graph from spatial coordinates (``_build.py:553-620``)."""
-    builder = RadiusBuilder(radius=radius, percentile=percentile, transform=transform, set_diag=set_diag, ctx=default_context(device))
-    return _run(_prepare(data, spatial_key, table_key), builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy)
+    adata = _prepare(data, spatial_key, table_key)
+    builder = RadiusBuilder(radius=radius, percentile=percentile, transform=transform, set_diag=set_diag, ctx=_host_context(adata, spatial_key, device))
+    return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy,
+                device=device)
 
 
 def spatial_neighbors_grid(data: Any, *, spatial_key: str = Key.obsm.spatial, elements_to_coordinate_systems: dict[str, str] | None = None,
@@ -343,5 +448,8 @@ def spatial_neighbors_grid(data: Any, *, spatial_key: str = Key.obsm.spatial, el
     """Grid graph for Visium-like coordinates (``_build.py:701-786``)."""
     assert_positive(n_rings, name="n_rings")
     assert_positive(n_neighs, name="n_neighs")
-    builder = GridBuilder(n_neighs=n_neighs, n_rings=n_rings, delaunay=delaunay, transform=transform, set_diag=set_diag, ctx=default_context(device))
-    return _run(_prepare(data, spatial_key, table_key), builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy)
+    adata = _prepare(data, spatial_key, table_key)
+    builder = GridBuilder(n_neighs=n_neighs, n_rings=n_rings, delaunay=delaunay, transform=transform, set_diag=set_diag,
+                          ctx=_host_context(adata, spatial_key, device))
+    return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy,
+                device=device)

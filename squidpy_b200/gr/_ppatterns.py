@@ -23,7 +23,8 @@ from scipy import stats
 from scipy.sparse import issparse, spmatrix
 
 from .._constants import Key, SpatialAutocorr
-from .._device import DevArray, DevSparse, array_device, common_stream, device_matrix, dtype_code, feature_map, index_bits, to_host_matrix
+from .._device import (DevArray, DevSparse, array_device, common_stream, device_matrix, dtype_code, feature_map, index_bits, on_host,
+                       to_host_matrix)
 from .._dist import all_gather_rows, all_reduce_sum, shard_range, shared_seed, world
 from .._lib import Context, check, default_context, load, pointer_device
 from .._rng import spawn_generators
@@ -559,7 +560,7 @@ def co_occurrence(
     assert_categorical_obs(adata, key=cluster_key)
     assert_spatial_basis(adata, key=spatial_key)
 
-    spatial = np.asarray(adata.obsm[spatial_key]).astype(fp)
+    spatial = np.asarray(on_host(adata.obsm[spatial_key])).astype(fp)
     labs, _ = category_codes(adata.obs[cluster_key], dtype=ip)
 
     if isinstance(interval, int):

@@ -16,6 +16,7 @@ import numpy as np
 import pandas as pd
 
 from .._constants import Key, RipleyStat
+from .._device import on_host
 from .._dist import all_reduce_sum, world, shared_seed
 from .._lib import Context, check, default_context, load
 from .._rng import spawn_generators
@@ -69,7 +70,7 @@ def ripley(
     adata = extract_adata_if_sdata(adata, table_key=table_key)
     assert_categorical_obs(adata, key=cluster_key)
     assert_spatial_basis(adata, key=spatial_key)
-    coordinates = np.asarray(adata.obsm[spatial_key])
+    coordinates = np.asarray(on_host(adata.obsm[spatial_key]))
     clusters = adata.obs[cluster_key].values
     mode = RipleyStat(mode)
 

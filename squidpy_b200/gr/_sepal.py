@@ -14,6 +14,7 @@ import pandas as pd
 from scipy.sparse import csr_matrix, issparse
 
 from .._constants import Key
+from .._device import on_host
 from .._lib import Context, check, default_context, load
 from .._validators import assert_connectivity_key, assert_spatial_basis, extract_adata_if_sdata
 from ._utils import _save_data, logg
@@ -83,7 +84,7 @@ def sepal(adata: Any, max_neighs: int, genes: str | Sequence[str] | None = None,
     assert_spatial_basis(adata, key=spatial_key)
     if max_neighs not in (4, 6):
         raise ValueError(f"Expected `max_neighs` to be either `4` or `6`, found `{max_neighs}`.")
-    spatial = np.asarray(adata.obsm[spatial_key]).astype(np.float64)
+    spatial = np.asarray(on_host(adata.obsm[spatial_key])).astype(np.float64)
     if genes is None:
         genes = adata.var_names.values
         if "highly_variable" in adata.var.columns:
@@ -92,7 +93,7 @@ def sepal(adata: Any, max_neighs: int, genes: str | Sequence[str] | None = None,
     if not genes:
         raise ValueError("No genes have been selected.")
 
-    g = adata.obsp[connectivity_key]
+    g = on_host(adata.obsp[connectivity_key])
     g = g.copy() if (issparse(g) and g.format == "csr") else csr_matrix(g)
     g.eliminate_zeros()
     max_n = np.diff(g.indptr).max()

@@ -42,11 +42,20 @@ __constant__ uint64_t c_jump_C[SQB_PCG_JUMP_BITS][2] = SQB_PCG_JUMP_C_INIT;
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ u128 mk128(uint64_t hi, uint64_t lo) { return ((u128)hi << 64) | (u128)lo; }
 
+// XSL-RR output of the state held as four 32-bit limbs (little-endian): the 64-bit rotate is a half swap for rot >= 32 and
+// two 32-bit funnel shifts by rot mod 32
+__device__ __forceinline__ void pcg_output_limbs(const uint32_t (&s)[4], uint32_t& lo, uint32_t& hi) {
+    const uint32_t a = s[0] ^ s[2], b = s[1] ^ s[3], rot = s[3] >> 26;
+    const uint32_t xl = (rot & 32u) ? b : a, xh = (rot & 32u) ? a : b;
+    lo = __funnelshift_r(xl, xh, rot);
+    hi = __funnelshift_r(xh, xl, rot);
+}
+
 __device__ __forceinline__ uint64_t pcg_output(u128 s) {
-    uint64_t hi = (uint64_t)(s >> 64), lo = (uint64_t)s;
-    uint64_t x = hi ^ lo;
-    unsigned rot = (unsigned)(hi >> 58);
-    return (x >> rot) | (x << ((64u - rot) & 63u));
+    const uint32_t l[4] = {(uint32_t)s, (uint32_t)(s >> 32), (uint32_t)(s >> 64), (uint32_t)(s >> 96)};
+    uint32_t lo, hi;
+    pcg_output_limbs(l, lo, hi);
+    return ((uint64_t)hi << 32) | lo;
 }
 
 // state_{k+d} = M * state_k + C * inc
@@ -748,10 +757,24 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
     }
 }
 
+// J[top - c] = u when u <= i (an accepted value), streamed (evict-first): one multiply-add from the window's base address
+// and a predicated store, which is what the compiler does not emit for the same C++ (it rebuilds the 64-bit address of every
+// element under a branch)
+__device__ __forceinline__ void st_cs_target(uint32_t* top, int c, uint32_t u, int i) {
+    asm volatile(
+        "{ .reg .pred p; .reg .u64 a;\n\t"
+        "setp.le.u32 p, %2, %3;\n\t"
+        "mad.wide.s32 a, %1, -4, %0;\n\t"
+        "@p st.global.cs.u32 [a], %2; }" ::"l"(top),
+        "r"(c), "r"(u), "r"(i)
+        : "memory");
+}
+
 // PART: two blocks of 4 pairs per SM (all the shared memory holds); that register bound also keeps ptxas from spilling the
-// generator, which it does at 80 registers without one
+// generator, which it does at 80 registers without one.  Plain: an explicit minimum of one block, without which ptxas caps
+// the registers on its own (80 for Q = 4, 128 for Q = 8) and spills the jump-ahead set-up
 template <int Q, bool PART>
-__global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 0) nhood_jgen_kernel(uint32_t* __restrict__ J, int64_t stride,
+__global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_kernel(uint32_t* __restrict__ J, int64_t stride,
                                                                       const uint64_t* __restrict__ states, int64_t n_perms,
                                                                       int nseg, const int64_t* __restrict__ seg_start,
                                                                       const int64_t* __restrict__ seg_len, float wfactor,
@@ -817,6 +840,49 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 0) nhood_jgen_ker
                 const uint32_t mask = 0xFFFFFFFFu >> __clz(i_cur);
                 const int i_lo = (int)(mask >> 1) + 1;
                 const int n_ph = i_cur - i_lo + 1;
+                // The common window, tested once per window with warp-uniform conditions: the whole fresh batch (pos = 0,
+                // K = RAW), no candidate whose acceptance depends on its rank (below), the phase goes on past the window
+                // (every accepted value is the target of a step of this phase) and, PART, the window stays inside block blk
+                // without completing it.  Only u and the ranks are live here; the acceptance flag of a value is u <= i_cur,
+                // re-tested where it is needed, and the stores are predicated on it.  Every other window (refills in
+                // mid-batch, ends of a phase or of a block, the small-i end where K = i/4) takes the general path below.
+                if (pos == 0 && (i_cur >> 2) >= RAW) {
+                    uint32_t u[2 * Q];
+                    bool uncertain = false;
+#pragma unroll
+                    for (int k = 0; k < 2 * Q; ++k) {
+                        u[k] = raw[k] & mask;
+                        uncertain |= (uint32_t)(i_cur - (int)u[k]) < (uint32_t)RAW;  // i_cur - RAW < u <= i_cur
+                    }
+                    if (!__any_sync(0xffffffffu, uncertain)) {
+                        int c[2 * Q], run = 0;
+#pragma unroll
+                        for (int q = 0; q < Q; ++q) {
+                            const uint32_t blo = __ballot_sync(0xffffffffu, u[2 * q] <= (uint32_t)i_cur);
+                            const uint32_t bhi = __ballot_sync(0xffffffffu, u[2 * q + 1] <= (uint32_t)i_cur);
+                            c[2 * q] = run + __popc(blo & lt_mask) + __popc(bhi & lt_mask);
+                            c[2 * q + 1] = c[2 * q] + (int)((blo >> lane) & 1u);
+                            run += __popc(blo) + __popc(bhi);
+                        }
+                        const int bL = blk * L;
+                        if (run < n_ph && (!PART || i_cur - run >= max(bL, 1))) {
+                            if (!PART) {
+                                uint32_t* __restrict__ Jtop = Jp + base + i_cur;
+#pragma unroll
+                                for (int k = 0; k < 2 * Q; ++k) st_cs_target(Jtop, c[k], u[k], i_cur);
+                            } else {
+                                uint32_t* stage = pair + 8 + (seq & 1) * SQB_PART_LP;
+                                const int t = i_cur - bL;
+#pragma unroll
+                                for (int k = 0; k < 2 * Q; ++k)
+                                    if (u[k] <= (uint32_t)i_cur) stage[part_idx(t - c[k])] = u[k];
+                            }
+                            i_cur -= run;
+                            pos = RAW;
+                            continue;
+                        }
+                    }
+                }
                 // no swaps here, hence no conflicts to bound: the window is the rest of the batch (capped at i/4, which keeps
                 // the acceptance fixed point short at the small-i end); wfactor only matters to the kernels that swap
                 int K = min(i_cur >> 2, RAW);
@@ -2384,8 +2450,9 @@ static int launch_jgen(sqb_nhood* h, uint32_t* J, const uint64_t* states, int64_
                        int region_cap) {
     sqb_ctx* c = h->ctx;
     SqbLaunchScope scope(c, SQB_K_MISC);  // J generation is accounted under "misc"
-    // one generator warp per permutation; small blocks spread the (latency-bound) warps evenly over the SMs.  jgen_threads =
-    // generator threads per block; PART adds as many partition threads.
+    // one generator warp per permutation; small blocks spread the warps evenly over the SMs.  From two generator warps per SM
+    // scheduler on, the SM's instruction throughput bounds the generation (DESIGN.md §3.1).  jgen_threads = generator threads
+    // per block; PART adds as many partition threads.
     const int jt = (int)h->jgen_threads;
     int64_t ctas = (int64_t)c->sm_count * 8 * (128 / jt);
     const size_t smem = PART ? (size_t)(jt / 32) * SQB_PART_PAIR_WORDS * sizeof(uint32_t) : 0;

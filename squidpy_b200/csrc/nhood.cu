@@ -14,11 +14,12 @@
 //                          shared memory, next window marked while the current one is resolved (sections 2f, 2h; 2b, 2c
 //                          are the single-kernel replays for few permutations or small arrays, 2j the region replay
 //                          for many permutations of large arrays)
-//   3. nhood_transpose     [P][n] -> [PB/32][n + 1][32] (groups of 32 permutations, permutation-minor inside a group) so that
-//                          one warp lane = one permutation and a CTA's labels of consecutive nodes are contiguous
-//   4. nhood_count         CSR neighbour-pair histogram: lane = permutation, warp walks the CSR once for 32
-//                          permutations; lane-private shared-memory histogram columns (bank = lane, no
-//                          conflicts), one flush per CTA; symmetric graphs are walked over j >= i only (3b).
+//   3. nhood_transpose     [P][n] -> [PB/64][n + 1][64] (groups of 64 permutations, permutation-minor inside a group) so that
+//                          one warp lane = two adjacent permutations and a CTA's labels of consecutive nodes are contiguous
+//   4. nhood_count         neighbour-pair histogram from row records: lane = two permutations, warp walks the records once
+//                          for 64 permutations; lane-private shared-memory histogram columns (bank = lane, no conflicts)
+//                          holding both permutations' counters as 16-bit halves of one word, one flush per CTA;
+//                          symmetric graphs are walked over j >= i only (3b).
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
@@ -1659,33 +1660,50 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
 }
 
 // ------------------------------------------------------------------------------------------------
-// 3. transpose [P][stride] -> [PB/32][n + 1][32]  (32 permutations x 256 nodes per CTA), optional row scatter through
-//    `order` (library-grouped position k -> original node id)
+// 3. transpose [P][stride] -> [PB/64][n + 1][64]  (one group of 64 permutations x 256 nodes per CTA), optional row scatter
+//    through `order` (library-grouped position k -> original node id)
 // ------------------------------------------------------------------------------------------------
+// Group-major label matrix labT[PB/64][n + 1][64], PB = P rounded up to 64: the label of node `node` under permutation `perm`.
+// A group holds the 64 permutations one warp of the count kernel covers (two per lane); row n of every group is the spare row.
+__host__ __device__ __forceinline__ int64_t sqb_labT_off(int64_t n, int64_t perm, int64_t node) {
+    return ((perm >> 6) * (n + 1) + node) * 64 + (perm & 63);
+}
+__host__ __device__ __forceinline__ int64_t sqb_labT_pb(int64_t np) { return ((np + 63) / 64) * 64; }
+
+// The tile is read in 4-byte words (a warp reads 128 contiguous bytes of one permutation's row) and every node's 64 labels
+// are written by one thread as whole 16-byte vectors, so each node row of the group is written by one CTA in full sectors.
 template <typename LT>
 __global__ void __launch_bounds__(256) nhood_transpose_kernel(const LT* __restrict__ lab, LT* __restrict__ labT, int64_t n,
-                                                              int64_t stride, int P, int PB,
-                                                              const uint32_t* __restrict__ order) {
-    __shared__ LT tile[32][256 + 16 / sizeof(LT)];
+                                                              int64_t stride, int P, const uint32_t* __restrict__ order) {
+    constexpr int ROWB = 256 * (int)sizeof(LT) + 16;  // bytes per tile row (padding: the column reads below do not conflict)
+    constexpr int WPR = 256 * (int)sizeof(LT) / 4;    // words per tile row
+    __shared__ __align__(16) uint8_t tile[64 * ROWB];
     const int tx = threadIdx.x;
-    const int64_t node = (int64_t)blockIdx.x * 256 + tx;
-    const int pg = blockIdx.y * 32;
-#pragma unroll 8
-    for (int pp = 0; pp < 32; ++pp) {
+    const int64_t n0 = (int64_t)blockIdx.x * 256;
+    const int pg = blockIdx.y * 64;
+    // stride is a multiple of 16 bytes, so a word lies entirely inside or entirely past the row
+    const uint32_t* __restrict__ src = reinterpret_cast<const uint32_t*>(lab + n0);
+#pragma unroll 4
+    for (int i = tx; i < 64 * WPR; i += 256) {
+        const int pp = i / WPR, w = i % WPR;
         const int perm = pg + pp;
-        tile[pp][tx] = (perm < P && node < n) ? lab[(int64_t)perm * stride + node] : (LT)0;
+        uint32_t v = 0u;
+        if (perm < P && n0 + (int64_t)w * (4 / (int)sizeof(LT)) < stride)
+            v = src[((int64_t)perm * stride * (int64_t)sizeof(LT)) / 4 + w];
+        *reinterpret_cast<uint32_t*>(tile + pp * ROWB + w * 4) = v;
     }
     __syncthreads();
+    const int64_t node = n0 + tx;
     if (node < n) {
         const int64_t row = order ? (int64_t)order[node] : node;
-        constexpr int NV = (int)(32 * sizeof(LT) / 16);
+        constexpr int NV = (int)(64 * sizeof(LT) / 16);
         union {
-            LT e[32];
+            LT e[64];
             uint4 v[NV];
         } pack;
 #pragma unroll
-        for (int pp = 0; pp < 32; ++pp) pack.e[pp] = tile[pp][tx];
-        uint4* dst = reinterpret_cast<uint4*>(labT + ((int64_t)(pg >> 5) * (n + 1) + row) * 32);  // group-major: [PB/32][n + 1][32]
+        for (int pp = 0; pp < 64; ++pp) pack.e[pp] = reinterpret_cast<const LT*>(tile + pp * ROWB)[tx];
+        uint4* dst = reinterpret_cast<uint4*>(labT + sqb_labT_off(n, pg, row));
 #pragma unroll
         for (int k = 0; k < NV; ++k) dst[k] = pack.v[k];
     }
@@ -1703,7 +1721,7 @@ __global__ void __launch_bounds__(256) nhood_transpose_kernel(const LT* __restri
 //     class_of(pi_p(r)) = the last c with cum[c] <= pi_p(r), found through a shared-memory bucket table + a fixed
 //     number of bisection steps instead of a random gather from a 1 MB array.  Shuffling the sorted vector has the same
 //     distribution as shuffling the original.  One lane evaluates 4 consecutive permutations of one position (4
-//     independent dependency chains) and stores 4 labels straight into the group-major matrix labT[PB/32][node][32] the
+//     independent dependency chains) and stores 4 labels straight into the group-major matrix labT[PB/64][node][64] the
 //     count kernel reads: fill + target generation + apply + transpose (most of the exact mode's time)
 //     collapse into one streaming kernel.  tests/philox_ref.py is the executable specification (numpy, bit-identical);
 //     results are validated statistically against the exact mode (SURVEY.md 8d).
@@ -1808,7 +1826,7 @@ __global__ void __launch_bounds__(256) nhood_philox_labels_kernel(LT* __restrict
             }
             cls[q] = lo;
         }
-        LT* dst = labT + ((int64_t)(p4 >> 5) * (n_nodes + 1) + node) * 32 + (p4 & 31);
+        LT* dst = labT + sqb_labT_off(n_nodes, p4, node);
         if (sizeof(LT) == 1) {
             *reinterpret_cast<uint32_t*>(dst) = cls[0] | (cls[1] << 8) | (cls[2] << 16) | (cls[3] << 24);
         } else {
@@ -1817,11 +1835,11 @@ __global__ void __launch_bounds__(256) nhood_philox_labels_kernel(LT* __restrict
     }
 }
 
-// single label vector (uint32 from the host) -> column 0 of a [n][32] permutation-minor matrix
+// single label vector (uint32 from the host) -> permutation 0 of a one-group label matrix [n + 1][64]
 template <typename LT>
 __global__ void nhood_single_to_T_kernel(const uint32_t* __restrict__ labels, LT* __restrict__ labT, int64_t n) {
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i < n) labT[i * 32] = (LT)labels[i];
+    if (i < n) labT[sqb_labT_off(n, 0, i)] = (LT)labels[i];
 }
 
 template <typename LT>
@@ -1897,7 +1915,7 @@ __global__ void nhood_upper_fill_kernel(const uint32_t* __restrict__ indptr, con
 
 // 3c. Row records for the count kernel: {i, j0, j1, j2} (16 bytes) = a row and up to three of its stored columns, unused
 //     slots = n; a row with more entries continues in further records.  One 16-byte load then serves three
-//     (pair x 32 permutations) units and the row label is fetched once per record.  Unused slots name node n: row n of every
+//     (pair x 64 permutations) units and the row labels are fetched once per record.  Unused slots name node n: row n of every
 //     group of the label matrix holds the label n_cls, whose histogram column is a spare that is never flushed -- the
 //     kernel needs no predicate for them.  Built from the entries with j >= i of a
 //     symmetric graph (self loops stay in: they are over-counted by one in the symmetrised flush and taken off again by
@@ -1956,9 +1974,9 @@ __global__ void __launch_bounds__(1024) nhood_count_kernel(const uint32_t* __res
         // ~7 instructions per (edge x 32 permutations), memory-level parallelism UN per warp.
         constexpr int UN = UNROWS;
         const int perm = blockIdx.y * 32 + lane;
-        const LT* __restrict__ col = labT + (int64_t)blockIdx.y * (n + 1) * 32 + lane;  // group-major label matrix [PB/32][n + 1][32]
+        const LT* __restrict__ col = labT + sqb_labT_off(n, perm, 0);  // group-major label matrix [PB/64][n + 1][64]
         // all element offsets are 32 x 32 -> 64 bit products (one IMAD.WIDE.U32 each): n < 2^31
-        const uint32_t PBu = 32u, Cu = (uint32_t)C;
+        const uint32_t PBu = 64u, Cu = (uint32_t)C;
         (void)perm;
         const uint32_t nb32 = (uint32_t)node_begin, ne32 = (uint32_t)node_end;
         uint32_t* __restrict__ myhist = hist + lane;
@@ -2007,15 +2025,15 @@ __global__ void __launch_bounds__(1024) nhood_count_kernel(const uint32_t* __res
         const int sub = lane / G, pl = lane % G;
         const int perm = blockIdx.y * G + pl;
         const bool valid = perm < P;
-        const LT* __restrict__ col = labT + (int64_t)(perm >> 5) * (n + 1) * 32 + (perm & 31);  // padded columns exist up to PB
+        const LT* __restrict__ col = labT + sqb_labT_off(n, perm, 0);  // padded columns exist up to PB
         for (int64_t i = node_begin + warp; i < node_end; i += nwarps) {
             const uint32_t beg = indptr[i], end = indptr[i + 1];
-            const uint32_t a = (uint32_t)col[i * 32];
+            const uint32_t a = (uint32_t)col[i * 64];
             const uint32_t rowbase = a * (uint32_t)C;
 #pragma unroll 4
             for (uint32_t e = beg + sub; e < end; e += EPW) {
                 const uint32_t j = indices[e];
-                const uint32_t b = (uint32_t)col[(int64_t)j * 32];
+                const uint32_t b = (uint32_t)col[(int64_t)j * 64];
                 if (valid) atomicAdd(&hist[(rowbase + b) * G + pl], 1u);
             }
         }
@@ -2034,47 +2052,60 @@ __global__ void __launch_bounds__(1024) nhood_count_kernel(const uint32_t* __res
 //     Structurally symmetric graphs (MIRROR = true): per unordered pair {i, j} the full count is +1 on (l_i, l_j) and +1 on
 //     (l_j, l_i): the kernel makes ONE increment, U[l_i][l_j], per stored entry with j >= i and adds the mirror when the
 //     histogram is flushed (counts += U + U^T; a self loop lands twice on the diagonal and is taken off once by
-//     nhood_count_selfloops_kernel).  lane = permutation, every lane owns its histogram column (bank == lane): the
-//     shared-memory reductions of a warp never conflict.
-//     What bounds it (tools/micro/smem_bench.cu): the SM's single load/store pipe, which takes about two cycles per warp
-//     instruction, global load or shared-memory reduction alike -- not the reduction itself and not DRAM.  So the
-//     kernel minimises LSU instructions per (entry x 32 permutations): one 16-byte record load per three entries, the row
-//     label once per record, one label load and one reduction per entry = 2.67 (CSR-row kernel of rounds 1-2: 2 reductions,
-//     1.3 label loads and an index load per entry + a branch, 21 instructions;
-//     flat (i, j) pairs: 3.5).  A warp takes UN records per pass, software-pipelined three deep: while the reductions of
-//     group k issue, the label loads of group k+1 and the record loads of group k+2 are in flight (one CTA of 32 warps per
-//     SM: without the pipeline most warps stall on label addresses waiting for the index load).
+//     nhood_count_selfloops_kernel).  Lane l of the CTA's group g owns permutations 64 g + 2 l and 64 g + 2 l + 1 and one
+//     histogram column (bank == lane: the shared-memory reductions of a warp never conflict); each counter word holds the
+//     even permutation's count in its low 16 bits and the odd one's in its high 16 bits.
+//     What bounds it: the SM's single load/store pipe, global load or shared-memory reduction alike -- not the reduction
+//     itself and not DRAM (1M spots x 1000 permutations: 1.77 cycles per LSU warp instruction, against 1.68 for a lane-private
+//     reduction alone in tools/micro/smem_bench.cu).  So the kernel minimises LSU instructions per (entry x 64
+//     permutations): one 16-byte record load per three entries, the row label pair once per record, one label-pair load and
+//     two reductions per entry = 11 per record = 1.83 per (entry x 32 permutations), where one permutation per lane took 8
+//     per record = 2.67 (CSR-row kernel: ~4.3, flat (i, j) pairs: 3.5).  Splitting a label pair is ALU work.  A warp takes UN
+//     records per pass, software-pipelined three deep: while the reductions of group k issue, the label loads of group k+1
+//     and the record loads of group k+2 are in flight (one CTA of 32 warps per SM: without the pipeline most warps stall on
+//     label addresses waiting for the index load).
+//     16-bit halves: a half can carry into its neighbour once one CTA adds 65 536 increments to one bin of one permutation,
+//     and a chunk of R records can add 3 R.  A chunk of at most SQB_RECS_NO_DRAIN records therefore runs in one round.  A
+//     larger one runs in rounds of SQB_RECS_ROUND records separated by a drain that moves every counter word with a half at
+//     or above 2^15 to `counts` and clears it: a round then starts below 2^15 in every half and adds at most 3 R < 2^15.
 // ------------------------------------------------------------------------------------------------
-// label load straight into a 32-bit register (ld.u8 / ld.u16 zero-extend: no cvt + mask after the load); the address is one
-// 32 x 32 + 64 bit multiply-add (node_bytes is kept opaque by the caller so that it is not strength-reduced into two shifts)
+constexpr int64_t SQB_RECS_NO_DRAIN = 65535 / 3;
+constexpr int64_t SQB_RECS_ROUND = 32768 / 3;
+
+// the label pair of permutations (2 l, 2 l + 1) of one node, zero-extended into a 32-bit register (u8 labels: one u16 load,
+// u16 labels: one u32 load); the address is one 32 x 32 + 64 bit multiply-add (node_bytes is kept opaque by the caller so that
+// it is not strength-reduced into two shifts)
 template <typename LT>
-__device__ __forceinline__ uint32_t sqb_ld_label_u32(unsigned long long base, uint32_t node, uint32_t node_bytes);
+__device__ __forceinline__ uint32_t sqb_ld_label_pair(unsigned long long base, uint32_t node, uint32_t node_bytes);
 template <>
-__device__ __forceinline__ uint32_t sqb_ld_label_u32<uint8_t>(unsigned long long base, uint32_t node, uint32_t node_bytes) {
-    uint32_t v;
-    asm volatile("{\n .reg .u64 a;\n mad.wide.u32 a, %1, %3, %2;\n ld.global.nc.u8 %0, [a];\n}" : "=r"(v) : "r"(node), "l"(base), "r"(node_bytes));
-    return v;
-}
-template <>
-__device__ __forceinline__ uint32_t sqb_ld_label_u32<uint16_t>(unsigned long long base, uint32_t node, uint32_t node_bytes) {
+__device__ __forceinline__ uint32_t sqb_ld_label_pair<uint8_t>(unsigned long long base, uint32_t node, uint32_t node_bytes) {
     uint32_t v;
     asm volatile("{\n .reg .u64 a;\n mad.wide.u32 a, %1, %3, %2;\n ld.global.nc.u16 %0, [a];\n}" : "=r"(v) : "r"(node), "l"(base), "r"(node_bytes));
     return v;
 }
-// one reduction on this lane's counter of bin (l_i, l_j): rowaddr = l_i * bytes per histogram row + the lane's column.  The
+template <>
+__device__ __forceinline__ uint32_t sqb_ld_label_pair<uint16_t>(unsigned long long base, uint32_t node, uint32_t node_bytes) {
+    uint32_t v;
+    asm volatile("{\n .reg .u64 a;\n mad.wide.u32 a, %1, %3, %2;\n ld.global.nc.u32 %0, [a];\n}" : "=r"(v) : "r"(node), "l"(base), "r"(node_bytes));
+    return v;
+}
+// one reduction on each of the lane's two counters of its bins: +1 on (l_i, l_j) of the even permutation, +2^16 on
+// (l_i', l_j') of the odd one; row_even / row_odd = the row label times bytes per histogram row + the lane's column.  The
 // histogram rows have C + 1 columns: unused record slots name the spare row of the label matrix, carry the label C and land
 // in the spare column, which is never flushed -- no predicate anywhere (ptxas wraps a predicated ATOMS into a four-instruction
-// convergence region).
-__device__ __forceinline__ void sqb_hist_inc(uint32_t rowaddr, uint32_t lb) {
-    asm volatile("{\n .reg .u32 a;\n mad.lo.u32 a, %1, 128, %0;\n red.shared.add.u32 [a], 1;\n}" ::"r"(rowaddr), "r"(lb));
+// convergence region).  A carry out of a spare-column half only reaches the other half of that spare word.
+__device__ __forceinline__ void sqb_hist_inc2(uint32_t row_even, uint32_t row_odd, uint32_t lb_even, uint32_t lb_odd) {
+    asm volatile("{\n .reg .u32 a, b;\n mad.lo.u32 a, %2, 128, %0;\n red.shared.add.u32 [a], 1;\n mad.lo.u32 b, %3, 128, %1;\n"
+                 " red.shared.add.u32 [b], 65536;\n}" ::"r"(row_even), "r"(row_odd), "r"(lb_even), "r"(lb_odd));
 }
 
 template <typename LT, int UN, bool MIRROR>
 __global__ void __launch_bounds__(1024) nhood_count_recs_kernel(const uint4* __restrict__ recs, int64_t n_recs,
                                                                 const LT* __restrict__ labT, int64_t n, int C,
-                                                                int64_t recs_per_cta, int P, uint32_t* __restrict__ counts) {
+                                                                int64_t recs_per_cta, int64_t recs_per_round, int P,
+                                                                uint32_t* __restrict__ counts) {
     extern __shared__ __align__(16) uint32_t hist[];
-    const int C1 = C + 1;  // one spare column per histogram row (see sqb_hist_inc)
+    const int C1 = C + 1;  // one spare column per histogram row (see sqb_hist_inc2)
     const int nb = C * C1 * 32;
     {
         uint4* hz = reinterpret_cast<uint4*>(hist);
@@ -2082,23 +2113,25 @@ __global__ void __launch_bounds__(1024) nhood_count_recs_kernel(const uint4* __r
     }
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    // lanes of padded permutations (blockIdx.y * 32 + lane >= P) count into columns nobody reads
-    unsigned long long colp = reinterpret_cast<unsigned long long>(labT + (int64_t)blockIdx.y * (n + 1) * 32 + lane);  // [PB/32][n + 1][32]
+    constexpr int LBITS = 8 * (int)sizeof(LT);
+    constexpr uint32_t LMASK = (1u << LBITS) - 1u;
+    // lanes of padded permutations (>= P) count into halves nobody reads
+    const int p_even = (int)blockIdx.y * 64 + 2 * lane;
+    unsigned long long colp = reinterpret_cast<unsigned long long>(labT + sqb_labT_off(n, p_even, 0));  // [PB/64][n + 1][64]
     asm volatile("" : "+l"(colp));  // opaque: every label address stays ONE 32x32+64 multiply-add
-    uint32_t NB = 32u * (uint32_t)sizeof(LT);  // bytes between the labels of consecutive nodes
+    uint32_t NB = 64u * (uint32_t)sizeof(LT);  // bytes between the labels of consecutive nodes
     asm volatile("" : "+r"(NB));
     const uint32_t hbase = (uint32_t)__cvta_generic_to_shared(hist) + (uint32_t)lane * 4u;  // byte address of this lane's column
     const uint32_t rowmul = (uint32_t)C1 * 128u;                                           // bytes per histogram row ((C + 1) bins x 32 lanes)
-    const int64_t r_begin = (int64_t)blockIdx.x * recs_per_cta;
-    int64_t r_end = r_begin + recs_per_cta;
-    if (r_end > n_recs) r_end = n_recs;
-    const int64_t r_full = r_begin + ((r_end - r_begin) / UN) * UN;  // whole groups of UN records
-    const int64_t step = (int64_t)nwarps * UN;
-    const int64_t r_first = r_begin + (int64_t)warp * UN;
-    const int n_it = r_first < r_full ? (int)((r_full - 1 - r_first) / step) + 1 : 0;  // groups of this warp
-    const uint4* __restrict__ pp = recs + r_first;                                     // the group being fetched
+    const int CC = C * C;
+    // record indices fit 32 bits (every record holds one or more of the < 2^32 stored entries): fewer live registers
+    const uint32_t r_begin = blockIdx.x * (uint32_t)recs_per_cta;
+    const uint32_t r_end = (uint32_t)((int64_t)r_begin + recs_per_cta < n_recs ? (int64_t)r_begin + recs_per_cta : n_recs);
+    const uint32_t rpr = (uint32_t)recs_per_round;
+    const uint32_t step = (uint32_t)nwarps * UN;
     uint4 rc[UN];
     uint32_t la[UN], lb[UN][3];
+    const uint4* __restrict__ pp = recs;  // the group being fetched
     auto ld_recs = [&]() {
 #pragma unroll
         for (int u = 0; u < UN; ++u)  // streamed once: keep the records out of L1, which holds the label sectors
@@ -2110,60 +2143,101 @@ __global__ void __launch_bounds__(1024) nhood_count_recs_kernel(const uint4* __r
     auto ld_labels = [&](uint32_t(&xa)[UN], uint32_t(&xb)[UN][3]) {
 #pragma unroll
         for (int u = 0; u < UN; ++u) {
-            xa[u] = sqb_ld_label_u32<LT>(colp, rc[u].x, NB);
-            xb[u][0] = sqb_ld_label_u32<LT>(colp, rc[u].y, NB);
-            xb[u][1] = sqb_ld_label_u32<LT>(colp, rc[u].z, NB);
-            xb[u][2] = sqb_ld_label_u32<LT>(colp, rc[u].w, NB);
+            xa[u] = sqb_ld_label_pair<LT>(colp, rc[u].x, NB);
+            xb[u][0] = sqb_ld_label_pair<LT>(colp, rc[u].y, NB);
+            xb[u][1] = sqb_ld_label_pair<LT>(colp, rc[u].z, NB);
+            xb[u][2] = sqb_ld_label_pair<LT>(colp, rc[u].w, NB);
         }
+    };
+    auto reduce1 = [&](uint32_t a, uint32_t b0, uint32_t b1, uint32_t b2) {
+        const uint32_t row_e = (a & LMASK) * rowmul + hbase, row_o = (a >> LBITS) * rowmul + hbase;
+        sqb_hist_inc2(row_e, row_o, b0 & LMASK, b0 >> LBITS);
+        sqb_hist_inc2(row_e, row_o, b1 & LMASK, b1 >> LBITS);
+        sqb_hist_inc2(row_e, row_o, b2 & LMASK, b2 >> LBITS);
     };
     auto reduce = [&](const uint32_t(&xa)[UN], const uint32_t(&xb)[UN][3]) {
 #pragma unroll
-        for (int u = 0; u < UN; ++u) {
-            const uint32_t rowaddr = xa[u] * rowmul + hbase;
-            sqb_hist_inc(rowaddr, xb[u][0]);
-            sqb_hist_inc(rowaddr, xb[u][1]);
-            sqb_hist_inc(rowaddr, xb[u][2]);
+        for (int u = 0; u < UN; ++u) reduce1(xa[u], xb[u][0], xb[u][1], xb[u][2]);
+    };
+    // counter word -> counts of both permutations in 32 bits (bin = a * C + b; MIRROR: the same amount on (b, a))
+    auto add_word = [&](uint32_t w, int a, int b, int l) {
+        const int p = (int)blockIdx.y * 64 + 2 * l;
+        const uint32_t v0 = w & 0xFFFFu, v1 = w >> 16;
+        if (v0 != 0 && p < P) {
+            atomicAdd(&counts[(int64_t)p * CC + a * C + b], v0);
+            if (MIRROR) atomicAdd(&counts[(int64_t)p * CC + b * C + a], v0);
+        }
+        if (v1 != 0 && p + 1 < P) {
+            atomicAdd(&counts[(int64_t)(p + 1) * CC + a * C + b], v1);
+            if (MIRROR) atomicAdd(&counts[(int64_t)(p + 1) * CC + b * C + a], v1);
         }
     };
-    if (n_it > 0) {
-        ld_recs();
-        ld_labels(la, lb);
-        if (n_it > 1) ld_recs();
-        // steady state: all three stages are live; unrolled by two so that the label registers of consecutive groups swap
-        // roles instead of being copied
+    for (uint32_t rb = r_begin, re; rb < r_end; rb = re) {
+        re = r_end - rb > rpr ? rb + rpr : r_end;
+        if (rb > r_begin) {  // drain between rounds (see the section comment)
+            __syncthreads();
+            for (int i = threadIdx.x; i < CC * 32; i += blockDim.x) {
+                const int bin = i >> 5, l = i & 31;
+                const int a = bin / C, b = bin - a * C;
+                const int wi = ((a * C1 + b) << 5) + l;
+                const uint32_t w = hist[wi];
+                if (w & 0x80008000u) {
+                    hist[wi] = 0u;
+                    add_word(w, a, b, l);
+                }
+            }
+            __syncthreads();
+        }
+        const uint32_t r_full = rb + ((re - rb) / UN) * UN;  // whole groups of UN records
+        const uint32_t r_first = rb + (uint32_t)warp * UN;
+        const int n_it = r_first < r_full ? (int)((r_full - 1 - r_first) / step) + 1 : 0;  // groups of this warp
+        pp = recs + r_first;
+        if (n_it > 0) {
+            ld_recs();
+            ld_labels(la, lb);
+            if (n_it > 1) ld_recs();
+            // steady state: all three stages are live; unrolled by two so that the label registers of consecutive groups swap
+            // roles instead of being copied
 #pragma unroll 2
-        for (int k = 0; k < n_it - 2; ++k) {
-            uint32_t na[UN], nb2[UN][3];
-            ld_labels(na, nb2);  // group k+1
-            ld_recs();           // group k+2
-            reduce(la, lb);      // group k
+            for (int k = 0; k < n_it - 2; ++k) {
+                uint32_t na[UN], nb2[UN][3];
+                ld_labels(na, nb2);  // group k+1
+                ld_recs();           // group k+2
+                reduce(la, lb);      // group k
 #pragma unroll
-            for (int u = 0; u < UN; ++u) la[u] = na[u], lb[u][0] = nb2[u][0], lb[u][1] = nb2[u][1], lb[u][2] = nb2[u][2];
-        }
-        if (n_it > 1) {
-            uint32_t na[UN], nb2[UN][3];
-            ld_labels(na, nb2);
+                for (int u = 0; u < UN; ++u) la[u] = na[u], lb[u][0] = nb2[u][0], lb[u][1] = nb2[u][1], lb[u][2] = nb2[u][2];
+            }
+            if (n_it > 1) {
+                uint32_t na[UN], nb2[UN][3];
+                ld_labels(na, nb2);
+                reduce(la, lb);
+#pragma unroll
+                for (int u = 0; u < UN; ++u) la[u] = na[u], lb[u][0] = nb2[u][0], lb[u][1] = nb2[u][1], lb[u][2] = nb2[u][2];
+            }
             reduce(la, lb);
-#pragma unroll
-            for (int u = 0; u < UN; ++u) la[u] = na[u], lb[u][0] = nb2[u][0], lb[u][1] = nb2[u][1], lb[u][2] = nb2[u][2];
         }
-        reduce(la, lb);
-    }
-    for (int64_t r = r_full + warp; r < r_end; r += nwarps) {  // fewer than UN records are left
-        const uint4 v = __ldg(recs + r);
-        const uint32_t rowaddr = sqb_ld_label_u32<LT>(colp, v.x, NB) * rowmul + hbase;
-        sqb_hist_inc(rowaddr, sqb_ld_label_u32<LT>(colp, v.y, NB));
-        sqb_hist_inc(rowaddr, sqb_ld_label_u32<LT>(colp, v.z, NB));
-        sqb_hist_inc(rowaddr, sqb_ld_label_u32<LT>(colp, v.w, NB));
+        for (int64_t r = (int64_t)r_full + warp; r < re; r += nwarps) {  // fewer than UN records are left
+            const uint4 v = __ldg(recs + r);
+            reduce1(sqb_ld_label_pair<LT>(colp, v.x, NB), sqb_ld_label_pair<LT>(colp, v.y, NB), sqb_ld_label_pair<LT>(colp, v.z, NB),
+                    sqb_ld_label_pair<LT>(colp, v.w, NB));
+        }
     }
     __syncthreads();
-    const int CC = C * C;
-    for (int i = threadIdx.x; i < CC * 32; i += blockDim.x) {
-        const int bin = i >> 5, l = i & 31;
+    // flush order: a warp takes 8 consecutive bins of 4 lane columns, so each of its global reductions lands on a few
+    // sectors (a run of 8 bins of each of 4 permutations), not on 32 permutations' lines CC * 4 bytes apart.  Its shared-memory
+    // reads then conflict 8-way (4 banks), which costs far less than the scattered global reductions did.
+    const int nbb = (CC + 7) >> 3;
+    for (int i = threadIdx.x; i < nbb * 256; i += blockDim.x) {
+        const int bin = ((i >> 5) % nbb) * 8 + (i & 7), l = ((i >> 5) / nbb) * 4 + ((i >> 3) & 3);
+        if (bin >= CC) continue;
         const int a = bin / C, b = bin - a * C;
-        const uint32_t v = MIRROR ? hist[((a * C1 + b) << 5) + l] + hist[((b * C1 + a) << 5) + l] : hist[((a * C1 + b) << 5) + l];  // U[a][b] + U[b][a]
-        const int p = blockIdx.y * 32 + l;
-        if (v != 0 && p < P) atomicAdd(&counts[(int64_t)p * CC + bin], v);
+        const uint32_t w = hist[((a * C1 + b) << 5) + l];
+        // U[a][b] + U[b][a], unpacked first so that the sum of two halves cannot carry into the other permutation
+        const uint32_t wm = MIRROR ? hist[((b * C1 + a) << 5) + l] : 0u;
+        const uint32_t v0 = (w & 0xFFFFu) + (wm & 0xFFFFu), v1 = (w >> 16) + (wm >> 16);
+        const int p = (int)blockIdx.y * 64 + 2 * l;
+        if (v0 != 0 && p < P) atomicAdd(&counts[(int64_t)p * CC + bin], v0);
+        if (v1 != 0 && p + 1 < P) atomicAdd(&counts[(int64_t)(p + 1) * CC + bin], v1);
     }
 }
 
@@ -2171,7 +2245,7 @@ __global__ void __launch_bounds__(1024) nhood_count_recs_kernel(const uint4* __r
 template <typename LT>
 __global__ void nhood_spare_row_kernel(LT* __restrict__ labT, int64_t n, int PB, int C) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p < PB) labT[((int64_t)(p >> 5) * (n + 1) + n) * 32 + (p & 31)] = (LT)C;
+    if (p < PB) labT[sqb_labT_off(n, p, n)] = (LT)C;
 }
 
 // a self loop (i, i) is ONE stored entry: +1 on (l_i, l_i); the symmetrised flush above gave it 2
@@ -2181,7 +2255,7 @@ __global__ void nhood_count_selfloops_kernel(const uint32_t* __restrict__ selfno
     const int p = blockIdx.y * blockDim.x + threadIdx.x;
     if (p >= P) return;
     for (uint32_t k = blockIdx.x; k < n_self; k += gridDim.x) {
-        const uint32_t a = (uint32_t)labT[((int64_t)(p >> 5) * (n + 1) + selfnodes[k]) * 32 + (p & 31)];
+        const uint32_t a = (uint32_t)labT[sqb_labT_off(n, p, selfnodes[k])];
         atomicAdd(&counts[(int64_t)p * C * C + a * C + a], 0xFFFFFFFFu);  // -1 (mod 2^32)
     }
 }
@@ -2230,13 +2304,13 @@ __global__ void nhood_count_global_kernel(const uint32_t* __restrict__ indptr, c
     const int64_t node_begin = (int64_t)blockIdx.x * nodes_per_cta;
     int64_t node_end = node_begin + nodes_per_cta;
     if (node_end > n) node_end = n;
-    const LT* __restrict__ col = labT + (int64_t)blockIdx.y * (n + 1) * 32 + lane;  // group-major label matrix [PB/32][n + 1][32]
+    const LT* __restrict__ col = labT + sqb_labT_off(n, perm, 0);  // group-major label matrix [PB/64][n + 1][64]
     const int64_t CC = (int64_t)C * C;
     for (int64_t i = node_begin + warp; i < node_end; i += nwarps) {
         const uint32_t beg = indptr[i], end = indptr[i + 1];
-        const uint32_t a = (uint32_t)col[i * 32];
+        const uint32_t a = (uint32_t)col[i * 64];
         for (uint32_t e = beg; e < end; ++e) {
-            const uint32_t b = (uint32_t)col[(int64_t)indices[e] * 32];
+            const uint32_t b = (uint32_t)col[(int64_t)indices[e] * 64];
             if (valid) atomicAdd(&counts[(int64_t)perm * CC + (int64_t)a * C + b], 1u);
         }
     }
@@ -2279,7 +2353,7 @@ struct sqb_nhood {
     std::vector<int64_t> h_seg_start, h_seg_len, h_bkt_off;
     bool philox_ready = false;
     std::vector<PhiloxSeg> h_pseg;
-    // label matrices [chunk][stride] and [PB/32][n + 1][32] live in ctx->scratch[0..1]
+    // label matrices [chunk][stride] and [PB/64][n + 1][64] live in ctx->scratch[0..1]
     DevBuf<uint32_t> d_counts;  // [P][C*C]
     DevBuf<uint32_t> d_tmp_u32;
     std::vector<uint32_t> h_order;
@@ -2339,7 +2413,7 @@ static int launch_count(sqb_nhood* h, const LT* labT, int PB, int P, uint32_t* d
                                               d_counts);                                                          \
     } break;
     if (G == 32 && h->n_recs > 0 && h->count_sym != 0 && (size_t)C * (C + 1) * 128 <= smem_limit) {  // record kernel (4b): mirrored flush for symmetric graphs
-        void (*k)(const uint4*, int64_t, const LT*, int64_t, int, int64_t, int, uint32_t*) = nullptr;
+        void (*k)(const uint4*, int64_t, const LT*, int64_t, int, int64_t, int64_t, int, uint32_t*) = nullptr;
 #define SQB_RECS_PICK(UNV) (h->sym ? nhood_count_recs_kernel<LT, UNV, true> : nhood_count_recs_kernel<LT, UNV, false>)
         // records per warp pass (1-4; more records pipeline deeper)
         k = SQB_RECS_PICK(4);
@@ -2347,12 +2421,16 @@ static int launch_count(sqb_nhood* h, const LT* labT, int PB, int P, uint32_t* d
         if (h->count_un == 2) k = SQB_RECS_PICK(2);
         if (h->count_un == 3) k = SQB_RECS_PICK(3);
 #undef SQB_RECS_PICK
-        // grid = pchunk x ngroups CTAs, one per SM at a time: aim at ~8 waves and, when a nearby pchunk makes the CTA count a
-        // multiple of the SM count, take it (a grid just past a whole number of waves pays a full extra round for a sliver of work)
-        int64_t pchunk = ((int64_t)8 * c->sm_count + ngroups / 2) / ngroups;
+        const int rgroups = (P + 63) / 64;  // a CTA covers one group of 64 permutations (two per lane)
+        // grid = pchunk x rgroups CTAs, one per SM at a time: aim at ~4 waves and, when a nearby pchunk makes the CTA count a
+        // multiple of the SM count, take it (a grid just past a whole number of waves pays a full extra round for a sliver of
+        // work).  Every CTA zeroes its histogram and flushes 64 x C^2 counters, so fewer waves flush less; but the CTAs resident
+        // at once then span more permutation groups, whose label matrices compete for L2 when neighbours are far apart in
+        // node order (300 K random kNN cells: 1.2 ms with one wave against 1.0 ms with four).
+        int64_t pchunk = ((int64_t)4 * c->sm_count + rgroups / 2) / rgroups;
         if (pchunk < 1) pchunk = 1;
         for (int64_t q = pchunk; q <= 2 * pchunk; ++q)
-            if ((q * ngroups) % c->sm_count == 0) {
+            if ((q * rgroups) % c->sm_count == 0) {
                 pchunk = q;
                 break;
             }
@@ -2362,11 +2440,17 @@ static int launch_count(sqb_nhood* h, const LT* labT, int PB, int P, uint32_t* d
         const int64_t recs_per_cta = ceil_div64(h->n_recs, pchunk);
         pchunk = ceil_div64(h->n_recs, recs_per_cta);
         if (pchunk < 1) pchunk = 1;
-        dim3 pgrid((unsigned)pchunk, (unsigned)ngroups);
+        // Overflow rule of the 16-bit counter halves (4b): a CTA's chunk of R records adds at most 3 R to one bin of one
+        // permutation.  Up to SQB_RECS_NO_DRAIN records that stays below 2^16 and the chunk runs in one round.  A larger chunk
+        // (few SMs per permutation group: many permutations, or many records per node) is not split over more CTAs -- each
+        // extra CTA zeroes and flushes a whole histogram -- but runs in rounds of SQB_RECS_ROUND records, between which the
+        // kernel drains the counter words that reached 2^15.
+        const int64_t recs_per_round = recs_per_cta <= SQB_RECS_NO_DRAIN ? recs_per_cta : SQB_RECS_ROUND;
+        dim3 pgrid((unsigned)pchunk, (unsigned)rgroups);
         const size_t rsmem = (size_t)C * (C + 1) * 128;  // one spare column per row
         nhood_spare_row_kernel<LT><<<(unsigned)((PB + 255) / 256), 256, 0, c->stream>>>(const_cast<LT*>(labT), h->n, PB, C);
         SQB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem));
-        k<<<pgrid, threads, rsmem, c->stream>>>(h->d_recs.p, h->n_recs, labT, h->n, C, recs_per_cta, P, d_counts);
+        k<<<pgrid, threads, rsmem, c->stream>>>(h->d_recs.p, h->n_recs, labT, h->n, C, recs_per_cta, recs_per_round, P, d_counts);
         SQB_POST_LAUNCH();
         if (h->sym && h->n_self > 0) {
             dim3 sgrid((unsigned)(h->n_self < 4096 ? h->n_self : 4096), (unsigned)((P + 127) / 128));
@@ -2670,13 +2754,14 @@ static int launch_shuffle(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t
 }
 
 static int64_t auto_chunk(sqb_nhood* h) {
-    if (h->perm_chunk > 0) return ((h->perm_chunk + 31) / 32) * 32;
+    // a multiple of 64: every chunk's label matrix [PB/64][n + 1][64] then fits the scratch sized for the chunk
+    if (h->perm_chunk > 0) return sqb_labT_pb(h->perm_chunk);
     // keep [chunk][stride] + [n][chunk] under ~8 GB
     int64_t per_perm = 2 * h->stride * h->lt_bytes + 4 * h->stride;  // label matrices + uint32 swap targets J (algos 7 and 9)
     int64_t ch = (int64_t)8e9 / (per_perm > 0 ? per_perm : 1);
-    if (ch < 32) ch = 32;
+    if (ch < 64) ch = 64;
     if (ch > 16384) ch = 16384;
-    return (ch / 32) * 32;
+    return (ch / 64) * 64;
 }
 
 template <typename LT>
@@ -2700,11 +2785,11 @@ static int run_chunk(sqb_nhood* h, int64_t p0, int64_t np, bool do_count) {
     }
     SQB_TRY(launch_shuffle<LT>(h, lab, h->d_states.p + p0 * 4, np, ps));
     if (!do_count) return SQB_OK;
-    const int PB = (int)(((np + 31) / 32) * 32);
+    const int PB = (int)sqb_labT_pb(np);
     {
         SqbLaunchScope scope(c, SQB_K_NHOOD_TRANSPOSE);
-        dim3 grid((unsigned)ceil_div64(h->n, 256), (unsigned)(PB / 32));
-        nhood_transpose_kernel<LT><<<grid, 256, 0, c->stream>>>(lab, labT, h->n, h->stride, (int)np, PB,
+        dim3 grid((unsigned)ceil_div64(h->n, 256), (unsigned)(PB / 64));
+        nhood_transpose_kernel<LT><<<grid, 256, 0, c->stream>>>(lab, labT, h->n, h->stride, (int)np,
                                                                 h->has_order ? h->d_order.p : nullptr);
         SQB_POST_LAUNCH();
     }
@@ -2712,7 +2797,7 @@ static int run_chunk(sqb_nhood* h, int64_t p0, int64_t np, bool do_count) {
     return SQB_OK;
 }
 
-// fast RNG mode: labels of permutations [p0, p0 + np) straight into labT[PB/32][n + 1][32] (one launch per library segment)
+// fast RNG mode: labels of permutations [p0, p0 + np) straight into labT[PB/64][n + 1][64] (one launch per library segment)
 template <typename LT>
 static int philox_labels(sqb_nhood* h, int64_t p0, int64_t np, LT* labT, int PB) {
     sqb_ctx* c = h->ctx;
@@ -2744,7 +2829,7 @@ static int philox_labels(sqb_nhood* h, int64_t p0, int64_t np, LT* labT, int PB)
 template <typename LT>
 static int run_chunk_philox(sqb_nhood* h, int64_t p0, int64_t np) {
     LT* labT = reinterpret_cast<LT*>(h->ctx->scratch[1].p);
-    const int PB = (int)(((np + 31) / 32) * 32);
+    const int PB = (int)sqb_labT_pb(np);
     SQB_TRY(philox_labels<LT>(h, p0, np, labT, PB));
     return launch_count<LT>(h, labT, PB, (int)np, h->d_counts.p + p0 * (int64_t)h->n_cls * h->n_cls);
 }
@@ -2875,7 +2960,7 @@ static int nhood_count_batched_path(sqb_nhood* h, const uint32_t* labels, uint32
     cnt.bind(c->stream);
     int rc = SQB_OK;
     if ((rc = h->d_tmp_u32.alloc(h->n)) != SQB_OK) return rc;
-    if ((rc = labT.alloc((size_t)(h->n + 1) * 32 * h->lt_bytes)) != SQB_OK) return rc;
+    if ((rc = labT.alloc((size_t)(h->n + 1) * 64 * h->lt_bytes)) != SQB_OK) return rc;  // one group of the label matrix
     if ((rc = cnt.alloc(CC)) != SQB_OK) {
         labT.release();
         return rc;
@@ -2886,7 +2971,7 @@ static int nhood_count_batched_path(sqb_nhood* h, const uint32_t* labels, uint32
     };
     cudaError_t e;
     e = cudaMemcpyAsync(h->d_tmp_u32.p, labels, h->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(labT.p, 0, (size_t)(h->n + 1) * 32 * h->lt_bytes, c->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(labT.p, 0, (size_t)(h->n + 1) * 64 * h->lt_bytes, c->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(cnt.p, 0, CC * sizeof(uint32_t), c->stream);
     if (e != cudaSuccess) {
         cleanup();
@@ -2901,8 +2986,8 @@ static int nhood_count_batched_path(sqb_nhood* h, const uint32_t* labels, uint32
         else
             nhood_single_to_T_kernel<uint16_t><<<g, 256, 0, c->stream>>>(h->d_tmp_u32.p, reinterpret_cast<uint16_t*>(labT.p), h->n);
     }
-    rc = (h->lt_bytes == 1) ? launch_count<uint8_t>(h, labT.p, 32, 1, cnt.p)
-                            : launch_count<uint16_t>(h, reinterpret_cast<uint16_t*>(labT.p), 32, 1, cnt.p);
+    rc = (h->lt_bytes == 1) ? launch_count<uint8_t>(h, labT.p, 64, 1, cnt.p)
+                            : launch_count<uint16_t>(h, reinterpret_cast<uint16_t*>(labT.p), 64, 1, cnt.p);
     if (rc == SQB_OK) {
         e = cudaMemcpyAsync(out, cnt.p, CC * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -3405,7 +3490,7 @@ int sqb_nhood_permute_upload(sqb_nhood* h, const uint64_t* states, int64_t n_per
     SQB_TRY(h->d_states.alloc((size_t)n_perms * 4));
     SQB_TRY(h->d_counts.alloc((size_t)n_perms * h->n_cls * h->n_cls));
     int64_t chunk = auto_chunk(h);
-    if (chunk > ((n_perms + 31) / 32) * 32) chunk = ((n_perms + 31) / 32) * 32;
+    if (chunk > sqb_labT_pb(n_perms)) chunk = sqb_labT_pb(n_perms);
     SQB_TRY(ensure_buffers(h, chunk));
     SQB_CUDA(cudaMemcpyAsync(h->d_states.p, packed.data(), packed.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
     SQB_CUDA(cudaStreamSynchronize(c->stream));
@@ -3426,7 +3511,7 @@ int sqb_nhood_permute_upload_philox(sqb_nhood* h, uint64_t seed, int64_t first_p
     SQB_TRY(philox_prepare(h));
     SQB_TRY(h->d_counts.alloc((size_t)n_perms * h->n_cls * h->n_cls));
     int64_t chunk = auto_chunk(h);
-    if (chunk > ((n_perms + 31) / 32) * 32) chunk = ((n_perms + 31) / 32) * 32;
+    if (chunk > sqb_labT_pb(n_perms)) chunk = sqb_labT_pb(n_perms);
     SQB_TRY(c->scratch[1].alloc((size_t)(h->n + 1) * chunk * h->lt_bytes));  // labT only: nothing permutation-major exists in this mode
     h->n_perms = n_perms;
     h->chunk = chunk;
@@ -3833,21 +3918,22 @@ int sqb_nhood_shuffled_labels(sqb_nhood* h, int64_t p0, int64_t p1, uint32_t* ou
               (long long)p0, (long long)p1);
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    if (h->rng_mode == 1) {  // fast mode: 32 permutations at a time through labT[n][32]
+    if (h->rng_mode == 1) {  // fast mode: 64 permutations at a time through one group of the label matrix, [n + 1][64]
         SQB_TRY(c->scratch[1].alloc((size_t)(h->n + 1) * h->chunk * h->lt_bytes));
-        std::vector<uint8_t> host((size_t)h->n * 32 * h->lt_bytes);  // group 0 rows [0, n); row n is the spare row
-        for (int64_t q0 = p0; q0 < p1; q0 += 32) {
-            const int64_t np = p1 - q0 < 32 ? p1 - q0 : 32;
+        std::vector<uint8_t> host((size_t)h->n * 64 * h->lt_bytes);  // group 0 rows [0, n); row n is the spare row
+        for (int64_t q0 = p0; q0 < p1; q0 += 64) {
+            const int64_t np = p1 - q0 < 64 ? p1 - q0 : 64;
             if (h->lt_bytes == 1)
-                SQB_TRY(philox_labels<uint8_t>(h, q0, np, c->scratch[1].p, 32));
+                SQB_TRY(philox_labels<uint8_t>(h, q0, np, c->scratch[1].p, 64));
             else
-                SQB_TRY(philox_labels<uint16_t>(h, q0, np, reinterpret_cast<uint16_t*>(c->scratch[1].p), 32));
+                SQB_TRY(philox_labels<uint16_t>(h, q0, np, reinterpret_cast<uint16_t*>(c->scratch[1].p), 64));
             SQB_CUDA(cudaMemcpyAsync(host.data(), c->scratch[1].p, host.size(), cudaMemcpyDeviceToHost, c->stream));
             SQB_CUDA(cudaStreamSynchronize(c->stream));
             for (int64_t p = 0; p < np; ++p) {
                 uint32_t* row = out + (size_t)(q0 - p0 + p) * h->n;
                 for (int64_t k = 0; k < h->n; ++k)
-                    row[k] = h->lt_bytes == 1 ? host[(size_t)k * 32 + p] : reinterpret_cast<uint16_t*>(host.data())[(size_t)k * 32 + p];
+                    row[k] = h->lt_bytes == 1 ? host[(size_t)sqb_labT_off(h->n, p, k)]
+                                              : reinterpret_cast<uint16_t*>(host.data())[(size_t)sqb_labT_off(h->n, p, k)];
             }
         }
         return SQB_OK;

@@ -22,6 +22,11 @@
  *   sqb_pair_counts_f64        <- KDTree.two_point_correlation(points, r)     src/squidpy/gr/_ripley.py:218-223
  *   sqb_ligrec_counts          <- _score_permutations(data, clustering, generators, ...)  src/squidpy/gr/_ligrec.py:616-676
  *   sqb_sepal                  <- _diffusion(conc, use_hex, n_iter, sat, sat_idx, unsat, unsat_idx, dt, thresh)  src/squidpy/gr/_sepal.py:186-233
+ *   sqb_dense_gather_device    <- X.toarray() / np.asarray(X) + DataFrame.fillna(0.0) + column selection  src/squidpy/gr/_ligrec.py:203-218,
+ *                                 vals[:, genes] of _diffusion_genes  src/squidpy/gr/_sepal.py:117-128,186-233
+ *   sqb_ligrec_observed        <- data.groupby("clusters").mean() / the expression-fraction mask of _analysis  src/squidpy/gr/_ligrec.py:679-700
+ *   sqb_ligrec_counts_dense    <- _score_permutations on a gathered device matrix  src/squidpy/gr/_ligrec.py:616-676
+ *   sqb_sepal_dense            <- _diffusion on a gathered device matrix  src/squidpy/gr/_sepal.py:186-233
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
  *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
@@ -36,7 +41,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 6
+#define SQB_ABI_VERSION 7
 
 typedef enum {
     SQB_OK = 0,
@@ -50,6 +55,7 @@ typedef enum {
 typedef struct sqb_ctx sqb_ctx;
 typedef struct sqb_nhood sqb_nhood;
 typedef struct sqb_autocorr sqb_autocorr;
+typedef struct sqb_dense sqb_dense;
 
 /* ---- library / context --------------------------------------------------------------------------- */
 int sqb_abi_version(void);
@@ -198,6 +204,45 @@ int sqb_interaction_matrix_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const vo
 int sqb_ligrec_counts(sqb_nhood* h, const double* data, int64_t n_genes, const double* inv_counts, const double* mean_obs,
                       const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs,
                       const uint8_t* valid, int64_t* out_counts);
+
+/* ---- expression matrix in GPU memory: ligrec and sepal -------------------------------------------------------------
+ * sqb_dense_gather_device reads a caller's device-resident X (observations x genes: n_rows x n_cols) in place and writes the
+ * selected rows x selected columns into a dense matrix owned by the returned handle (on the context's device).
+ *   format 0 dense: x is the matrix with element strides stride_row / stride_col (C order, F order or a strided view);
+ *   format 1 CSR / 2 CSC: x is the values array, indptr / indices DEVICE pointers with indptr_bits / index_bits 32 or 64, nnz
+ *          the number of stored entries.  indptr must run from 0 to nnz without decreasing (checked on the device before
+ *          anything follows it, one synchronisation); an index outside its range is rejected; two stored entries that fall
+ *          into the same gathered cell are rejected (SQB_ERR_INVALID): scipy's toarray() sums such duplicates on the host, so
+ *          sum them first.  Duplicates in rows or columns that are not gathered are never read.
+ *   x_dtype: 0 = f32, 1 = f64, 2 = f16, 3 = int32, 4 = int64.
+ *   rows (HOST, ascending, n_rows_out entries) or NULL for every row; cols (HOST, n_cols_out distinct input columns, in output
+ *          order).
+ *   layout 0: observations x genes row-major (what sqb_ligrec_observed / sqb_ligrec_counts_dense read); 1: genes x observations
+ *          row-major (what sqb_sepal_dense reads).
+ *   flags: 1 = write NaN as 0.0 (ligrec's fillna(0.0)); 2 = keep the input's value type (else every value is converted to
+ *          float64 exactly, like astype(float64)).
+ *   producer_stream: as in sqb_autocorr_load_csr_device.  Returns after the device has stopped reading the caller's buffers;
+ *   on an error no handle is returned and the context stays usable.  The extra device memory is the gathered block.      */
+int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void* indptr, int indptr_bits, const void* indices,
+                            int index_bits, int64_t nnz, int x_dtype, int64_t n_rows, int64_t n_cols, int64_t stride_row,
+                            int64_t stride_col, const int64_t* rows, int64_t n_rows_out, const int32_t* cols, int64_t n_cols_out,
+                            int layout, int flags, uintptr_t producer_stream, sqb_dense** out);
+/* The gathered values in their stored layout and type (n_rows_out x n_cols_out or its transpose) into HOST memory.          */
+int sqb_dense_download(sqb_dense* d, void* out);
+int sqb_dense_free(sqb_dense* d);
+/* Observed statistics of ligrec on a layout-0 float64 gathered matrix with NaN written as 0: codes[i] in [0, n_cls) is the
+ * cluster of observation i.  mean_out[k, g] = pandas' groupby mean (a Kahan sum over the cluster's observations in order,
+ * the compensation reset when it is NaN, divided by the count), npos_out[k, g] = number of values > 0, sizes_out[k] = number
+ * of observations of cluster k (all HOST, n_cls x n_genes / n_cls).                                                       */
+int sqb_ligrec_observed(sqb_dense* d, const int32_t* codes, int n_cls, double* mean_out, int64_t* npos_out, int64_t* sizes_out);
+/* sqb_ligrec_counts with the layout-0 float64 gathered matrix (observations = the handle's cells) in place of data.        */
+int sqb_ligrec_counts_dense(sqb_nhood* h, const sqb_dense* x, const double* inv_counts, const double* mean_obs,
+                            const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs,
+                            const uint8_t* valid, int64_t* out_counts);
+/* sqb_sepal with a layout-1 float64 gathered matrix (one row per gene) in place of vals, on the matrix's context.          */
+int sqb_sepal_dense(const sqb_dense* x, const int32_t* sat, int64_t n_sat, const int32_t* sat_idx, int max_neighs,
+                    const int32_t* unsat, const int32_t* unsat_idx, int64_t n_unsat, int n_iter, double dt, double thresh,
+                    double* out);
 
 /* ---- spatial_autocorr (Moran's I / Geary's C) -------------------------------------------------------
  * W = obsp[connectivity_key] (after optional float32 row normalisation on the host) as CSR; w_dtype 0 = f32,

@@ -231,6 +231,50 @@ def feature_map(n_cols: int, positions: Any, lo: int = 0, hi: int | None = None)
     return col_map, int(uniq.size), rank[inverse.reshape(-1)]
 
 
+@dataclass
+class DevMatrix:
+    """The ABI arguments of a device expression matrix for ``sqb_dense_gather_device`` (observations x genes).
+
+    ``format`` 0 dense (``x`` the array, ``strides`` in elements), 1 CSR, 2 CSC (``x`` the values); ``code`` the value dtype
+    code (``DTYPE_CODES``)."""
+
+    format: int
+    shape: tuple[int, int]
+    x: int
+    indptr: int
+    indptr_bits: int
+    indices: int
+    index_bits: int
+    nnz: int
+    dtype: np.dtype
+    code: int
+    strides: tuple[int, int]
+    stream: int
+    source: DevArray | DevSparse
+
+
+def matrix_args(d: DevArray | DevSparse, shape: tuple[int, int]) -> DevMatrix:
+    """Check that ``d`` is an expression matrix of ``shape`` in a supported layout and dtype, and describe it."""
+    shape = (int(shape[0]), int(shape[1]))
+    if tuple(d.shape) != shape:
+        raise ValueError(f"Expected the expression matrix to be of shape `{shape}`, found `{tuple(d.shape)}`.")
+    stream = common_stream(d)
+    if isinstance(d, DevSparse):
+        ip_bits, ix_bits = index_bits(d.indptr, "indptr"), index_bits(d.indices, "indices")
+        major = shape[0] if d.format == "csr" else shape[1]
+        if d.indptr.shape[0] != major + 1:
+            raise ValueError(f"Expected `indptr` of length `{major + 1}`, found `{d.indptr.shape[0]}`.")
+        nnz = int(d.indices.shape[0])
+        code = dtype_code(d.data)
+        if len(d.data.shape) != 1 or d.data.shape[0] < nnz or (nnz > 1 and d.data.strides[0] != 1):
+            raise ValueError(f"The matrix's values must be a contiguous 1-D array of `{nnz}` entries.")
+        return DevMatrix(1 if d.format == "csr" else 2, shape, d.data.ptr, d.indptr.ptr, ip_bits, d.indices.ptr, ix_bits, nnz, d.data.dtype,
+                         code, (0, 0), stream, d)
+    if len(d.shape) != 2:
+        raise ValueError(f"Expected a 2-D device array, found shape `{d.shape}`.")
+    return DevMatrix(0, shape, d.ptr, 0, 32, 0, 32, 0, d.dtype, dtype_code(d), (int(d.strides[0]), int(d.strides[1])), stream, d)
+
+
 def _host_array(a: Any) -> np.ndarray:
     torch = sys.modules.get("torch")
     if torch is not None and isinstance(a, torch.Tensor):

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
 # phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -96,6 +96,16 @@ _SIGNATURES: dict[str, tuple] = {
                                     C.c_void_p, C.c_void_p]),
     "sqb_sepal": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64,
                             C.c_int, C.c_double, C.c_double, C.c_void_p]),
+    "sqb_dense_gather_device": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_int,
+                                          C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int,
+                                          C.c_int, C.c_size_t, c_void_pp]),
+    "sqb_dense_download": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "sqb_dense_free": (C.c_int, [C.c_void_p]),
+    "sqb_ligrec_observed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sqb_ligrec_counts_dense": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                          C.c_void_p, C.c_void_p]),
+    "sqb_sepal_dense": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
+                                  C.c_double, C.c_double, C.c_void_p]),
     "sqb_knn_2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sqb_radius_2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "sqb_graph_build_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int,

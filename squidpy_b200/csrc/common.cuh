@@ -120,6 +120,16 @@ struct sqb_ctx {
     bool stage_used[kStage] = {};
 };
 
+// A dense matrix gathered from a caller's device X (sqb_dense_gather_device, dense.cu): n_obs x n_genes row-major (layout 0)
+// or n_genes x n_obs row-major (layout 1), float64 (dtype 1) or the input's own value type (DTYPE_CODES of _device.py).
+struct sqb_dense {
+    sqb_ctx* ctx = nullptr;
+    DevBuf<uint8_t> buf;
+    int64_t n_obs = 0, n_genes = 0;
+    int layout = 0, dtype = 1;
+    bool nan_zero = false;  // NaN entries were written as 0.0
+};
+
 // Host-to-device copy of caller-owned (pageable) memory on the ctx stream.  Large copies go through a ring of pinned
 // staging buffers filled by several host threads while the previous chunk is on the bus: a plain cudaMemcpyAsync from
 // pageable memory is bounded by the host's single-threaded page-locking copy.

@@ -3821,46 +3821,34 @@ __global__ void ligrec_compare_kernel(const double* __restrict__ G, int64_t np, 
     counts[t] += cnt;
 }
 
-extern "C" {
-
-int sqb_ligrec_counts(sqb_nhood* h, const double* data, int64_t n_genes, const double* inv_counts, const double* mean_obs,
-                      const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs,
-                      const uint8_t* valid, int64_t* out_counts) {
-    SQB_CHECK(h && data && inv_counts && mean_obs && interactions && inter_clusters && valid && out_counts, SQB_ERR_INVALID,
-              "sqb_ligrec_counts: null argument");
-    SQB_CHECK(h->uploaded && h->rng_mode == 0, SQB_ERR_STATE, "sqb_ligrec_counts: upload numpy generator states first (sqb_nhood_permute_upload)");
-    SQB_CHECK(!h->has_order, SQB_ERR_UNSUPPORTED, "sqb_ligrec_counts: library partitions are not part of the ligrec test");
-    SQB_CHECK(n_genes >= 1 && n_genes < 2147483647LL && n_inter >= 1 && n_cpairs >= 1, SQB_ERR_INVALID, "sqb_ligrec_counts: bad sizes");
+// sqb_ligrec_counts over an observations x genes float64 matrix already on the device (d_data: the host copy of
+// sqb_ligrec_counts, or a gathered sqb_dense).  where: the entry point named in error messages.
+static int ligrec_counts_impl(sqb_nhood* h, const double* d_data, int64_t n_genes, const double* inv_counts, const double* mean_obs,
+                              const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs,
+                              const uint8_t* valid, int64_t* out_counts, const char* where) {
     sqb_ctx* c = h->ctx;
-    SQB_CUDA(cudaSetDevice(c->device));
     const int C = h->n_cls;
     const size_t smem = (size_t)4 * C * 32 * sizeof(double);
-    SQB_CHECK(smem <= c->smem_optin, SQB_ERR_UNSUPPORTED, "sqb_ligrec_counts: %d clusters exceed the shared-memory accumulators", C);
-    for (int64_t i = 0; i < n_inter * 2; ++i)
-        SQB_CHECK(interactions[i] >= 0 && interactions[i] < n_genes, SQB_ERR_INVALID, "sqb_ligrec_counts: gene index %d out of range", interactions[i]);
-    for (int64_t i = 0; i < n_cpairs * 2; ++i)
-        SQB_CHECK(inter_clusters[i] >= 0 && inter_clusters[i] < C, SQB_ERR_INVALID, "sqb_ligrec_counts: cluster index %d out of range", inter_clusters[i]);
     const int64_t n = h->n, NT = n_inter * n_cpairs;
     // permutations per pass: the shuffled label rows (upload chunk) and the [perm][cluster][gene] means (<= 1 GB)
     int64_t chunk = h->chunk;
     const int64_t gcap = ((int64_t)1 << 30) / ((int64_t)C * n_genes * 8);
     if (chunk > gcap) chunk = gcap < 1 ? 1 : gcap;
-    DevBuf<double> d_data, d_inv, d_obs, d_G;
+    DevBuf<double> d_inv, d_obs, d_G;
     DevBuf<int32_t> d_inter, d_cp;
     DevBuf<uint8_t> d_valid;
     DevBuf<long long> d_cnt;
     auto cleanup = [&]() {
-        d_data.release(), d_inv.release(), d_obs.release(), d_G.release(), d_inter.release(), d_cp.release(), d_valid.release(), d_cnt.release();
+        d_inv.release(), d_obs.release(), d_G.release(), d_inter.release(), d_cp.release(), d_valid.release(), d_cnt.release();
     };
     int rc;
-    if ((rc = d_data.alloc((size_t)n * n_genes)) || (rc = d_inv.alloc(C)) || (rc = d_obs.alloc((size_t)C * n_genes)) ||
-        (rc = d_G.alloc((size_t)chunk * C * n_genes)) || (rc = d_inter.alloc(2 * n_inter)) || (rc = d_cp.alloc(2 * n_cpairs)) ||
-        (rc = d_valid.alloc(NT)) || (rc = d_cnt.alloc(NT)) || (rc = ensure_buffers(h, h->chunk))) {
+    if ((rc = d_inv.alloc(C)) || (rc = d_obs.alloc((size_t)C * n_genes)) || (rc = d_G.alloc((size_t)chunk * C * n_genes)) ||
+        (rc = d_inter.alloc(2 * n_inter)) || (rc = d_cp.alloc(2 * n_cpairs)) || (rc = d_valid.alloc(NT)) || (rc = d_cnt.alloc(NT)) ||
+        (rc = ensure_buffers(h, h->chunk))) {
         cleanup();
         return rc;
     }
     cudaError_t e = cudaMemsetAsync(d_cnt.p, 0, NT * sizeof(long long), c->stream);
-    if (e == cudaSuccess && sqb_h2d(c, d_data.p, data, (size_t)n * n_genes * sizeof(double)) != SQB_OK) e = cudaErrorUnknown;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_inv.p, inv_counts, C * sizeof(double), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_obs.p, mean_obs, (size_t)C * n_genes * sizeof(double), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_inter.p, interactions, 2 * n_inter * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
@@ -3882,10 +3870,10 @@ int sqb_ligrec_counts(sqb_nhood* h, const double* data, int64_t n_genes, const d
             SqbLaunchScope scope(c, SQB_K_MISC);
             dim3 grid((unsigned)ceil_div64(n_genes, 128), (unsigned)np);
             if (h->lt_bytes == 1)
-                ligrec_group_means_kernel<uint8_t><<<grid, 128, smem, c->stream>>>(c->scratch[0].p, h->stride, d_data.p, n, (int)n_genes, C, d_inv.p, d_G.p);
+                ligrec_group_means_kernel<uint8_t><<<grid, 128, smem, c->stream>>>(c->scratch[0].p, h->stride, d_data, n, (int)n_genes, C, d_inv.p, d_G.p);
             else
                 ligrec_group_means_kernel<uint16_t><<<grid, 128, smem, c->stream>>>(reinterpret_cast<const uint16_t*>(c->scratch[0].p), h->stride,
-                                                                                     d_data.p, n, (int)n_genes, C, d_inv.p, d_G.p);
+                                                                                     d_data, n, (int)n_genes, C, d_inv.p, d_G.p);
         }
         {
             SqbLaunchScope scope(c, SQB_K_MISC);
@@ -3899,10 +3887,62 @@ int sqb_ligrec_counts(sqb_nhood* h, const double* data, int64_t n_genes, const d
     else cudaStreamSynchronize(c->stream);
     cleanup();
     if (e != cudaSuccess) {
-        sqb_set_error("sqb_ligrec_counts: %s", cudaGetErrorString(e));
+        sqb_set_error("%s: %s", where, cudaGetErrorString(e));
         return SQB_ERR_CUDA;
     }
     return SQB_OK;
+}
+
+// the argument checks shared by both entry points
+static int ligrec_counts_check(sqb_nhood* h, int64_t n_genes, const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters,
+                               int64_t n_cpairs, const char* where) {
+    SQB_CHECK(h->uploaded && h->rng_mode == 0, SQB_ERR_STATE, "%s: upload numpy generator states first (sqb_nhood_permute_upload)", where);
+    SQB_CHECK(!h->has_order, SQB_ERR_UNSUPPORTED, "%s: library partitions are not part of the ligrec test", where);
+    SQB_CHECK(n_genes >= 1 && n_genes < 2147483647LL && n_inter >= 1 && n_cpairs >= 1, SQB_ERR_INVALID, "%s: bad sizes", where);
+    sqb_ctx* c = h->ctx;
+    SQB_CUDA(cudaSetDevice(c->device));
+    const int C = h->n_cls;
+    const size_t smem = (size_t)4 * C * 32 * sizeof(double);
+    SQB_CHECK(smem <= c->smem_optin, SQB_ERR_UNSUPPORTED, "%s: %d clusters exceed the shared-memory accumulators", where, C);
+    for (int64_t i = 0; i < n_inter * 2; ++i)
+        SQB_CHECK(interactions[i] >= 0 && interactions[i] < n_genes, SQB_ERR_INVALID, "%s: gene index %d out of range", where, interactions[i]);
+    for (int64_t i = 0; i < n_cpairs * 2; ++i)
+        SQB_CHECK(inter_clusters[i] >= 0 && inter_clusters[i] < C, SQB_ERR_INVALID, "%s: cluster index %d out of range", where, inter_clusters[i]);
+    return SQB_OK;
+}
+
+extern "C" {
+
+int sqb_ligrec_counts(sqb_nhood* h, const double* data, int64_t n_genes, const double* inv_counts, const double* mean_obs,
+                      const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs,
+                      const uint8_t* valid, int64_t* out_counts) {
+    static const char* where = "sqb_ligrec_counts";
+    SQB_CHECK(h && data && inv_counts && mean_obs && interactions && inter_clusters && valid && out_counts, SQB_ERR_INVALID,
+              "%s: null argument", where);
+    SQB_TRY(ligrec_counts_check(h, n_genes, interactions, n_inter, inter_clusters, n_cpairs, where));
+    sqb_ctx* c = h->ctx;
+    DevBuf<double> d_data;
+    SQB_TRY(d_data.alloc((size_t)h->n * n_genes));
+    int rc = sqb_h2d(c, d_data.p, data, (size_t)h->n * n_genes * sizeof(double));
+    if (rc == SQB_OK)
+        rc = ligrec_counts_impl(h, d_data.p, n_genes, inv_counts, mean_obs, interactions, n_inter, inter_clusters, n_cpairs, valid, out_counts, where);
+    else
+        cudaStreamSynchronize(c->stream);
+    d_data.release();
+    return rc;
+}
+
+int sqb_ligrec_counts_dense(sqb_nhood* h, const sqb_dense* x, const double* inv_counts, const double* mean_obs, const int32_t* interactions,
+                            int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs, const uint8_t* valid, int64_t* out_counts) {
+    static const char* where = "sqb_ligrec_counts_dense";
+    SQB_CHECK(h && x && inv_counts && mean_obs && interactions && inter_clusters && valid && out_counts, SQB_ERR_INVALID,
+              "%s: null argument", where);
+    SQB_CHECK(x->ctx == h->ctx, SQB_ERR_INVALID, "%s: the matrix and the handle belong to different contexts", where);
+    SQB_CHECK(x->layout == 0 && x->dtype == 1 && x->n_obs == h->n, SQB_ERR_INVALID,
+              "%s: expected a float64 observations x genes matrix of %lld observations", where, (long long)h->n);
+    SQB_TRY(ligrec_counts_check(h, x->n_genes, interactions, n_inter, inter_clusters, n_cpairs, where));
+    return ligrec_counts_impl(h, reinterpret_cast<const double*>(x->buf.p), x->n_genes, inv_counts, mean_obs, interactions, n_inter,
+                              inter_clusters, n_cpairs, valid, out_counts, where);
 }
 
 int sqb_nhood_permute(sqb_nhood* h, const uint64_t* states, int64_t n_perms, uint32_t* out_counts) {

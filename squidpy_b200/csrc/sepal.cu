@@ -116,12 +116,9 @@ __global__ void __launch_bounds__(SEPAL_T) sepal_kernel(const __grid_constant__ 
     }
 }
 
-extern "C" {
-
-int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, const int32_t* sat, int64_t n_sat, const int32_t* sat_idx,
-              int max_neighs, const int32_t* unsat, const int32_t* unsat_idx, int64_t n_unsat, int n_iter, double dt, double thresh,
-              double* out) {
-    SQB_CHECK(ctx && vals && sat && sat_idx && out && (n_unsat == 0 || (unsat && unsat_idx)), SQB_ERR_INVALID, "sqb_sepal: null argument");
+// the host-side argument checks shared by both entry points
+static int sepal_check(const int32_t* sat, int64_t n_sat, const int32_t* sat_idx, int max_neighs, const int32_t* unsat,
+                       const int32_t* unsat_idx, int64_t n_unsat, int64_t n_genes, int64_t n, int n_iter) {
     SQB_CHECK(max_neighs == 4 || max_neighs == 6, SQB_ERR_INVALID, "Expected `max_neighs` to be either `4` or `6`, found `%d`.", max_neighs);
     SQB_CHECK(n_genes >= 1 && n >= 1 && n < 2147483647LL && n_sat >= 1 && n_sat <= n && n_unsat >= 0 && n_iter >= 1, SQB_ERR_INVALID,
               "sqb_sepal: bad sizes");
@@ -129,13 +126,19 @@ int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, cons
     for (int64_t j = 0; j < n_sat * max_neighs; ++j) SQB_CHECK(sat_idx[j] >= 0 && sat_idx[j] < n, SQB_ERR_INVALID, "sqb_sepal: neighbour index out of range");
     for (int64_t j = 0; j < n_unsat; ++j)
         SQB_CHECK(unsat[j] >= 0 && unsat[j] < n && unsat_idx[j] >= 0 && unsat_idx[j] < n, SQB_ERR_INVALID, "sqb_sepal: node index out of range");
-    sqb_ctx* c = ctx;
-    SQB_CUDA(cudaSetDevice(c->device));
-    DevBuf<double> d_vals, d_out, d_scr;
+    return SQB_OK;
+}
+
+// sqb_sepal over genes x observations float64 values already on the device (d_vals: the host copy of sqb_sepal, or a gathered
+// sqb_dense); the arguments have been checked
+static int sepal_impl(sqb_ctx* c, const double* d_vals, int64_t n_genes, int64_t n, const int32_t* sat, int64_t n_sat, const int32_t* sat_idx,
+                      int max_neighs, const int32_t* unsat, const int32_t* unsat_idx, int64_t n_unsat, int n_iter, double dt, double thresh,
+                      double* out) {
+    DevBuf<double> d_out, d_scr;
     DevBuf<int32_t> d_sat, d_idx, d_unsat, d_uidx;
     DevBuf<int> d_cnt;
     auto cleanup = [&]() {
-        d_vals.release(), d_out.release(), d_scr.release(), d_sat.release(), d_idx.release(), d_unsat.release(), d_uidx.release(), d_cnt.release();
+        d_out.release(), d_scr.release(), d_sat.release(), d_idx.release(), d_unsat.release(), d_uidx.release(), d_cnt.release();
     };
     const size_t need = (size_t)2 * n * sizeof(double);
     const bool global = need + 1024 > c->smem_optin;
@@ -147,21 +150,20 @@ int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, cons
     int64_t ctas = (int64_t)per_sm * c->sm_count;
     if (ctas > n_genes) ctas = n_genes;
     int rc;
-    if ((rc = d_vals.alloc((size_t)n_genes * n)) || (rc = d_out.alloc(n_genes)) || (rc = d_sat.alloc(n_sat)) || (rc = d_idx.alloc((size_t)n_sat * max_neighs)) ||
+    if ((rc = d_out.alloc(n_genes)) || (rc = d_sat.alloc(n_sat)) || (rc = d_idx.alloc((size_t)n_sat * max_neighs)) ||
         (rc = d_unsat.alloc(n_unsat > 0 ? n_unsat : 1)) || (rc = d_uidx.alloc(n_unsat > 0 ? n_unsat : 1)) || (rc = d_cnt.alloc(1)) ||
         (global && (rc = d_scr.alloc((size_t)ctas * 2 * n)))) {
         cleanup();
         return rc;
     }
     cudaError_t e = cudaMemsetAsync(d_cnt.p, 0, sizeof(int), c->stream);
-    if (e == cudaSuccess && sqb_h2d(c, d_vals.p, vals, (size_t)n_genes * n * sizeof(double)) != SQB_OK) e = cudaErrorUnknown;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_sat.p, sat, n_sat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_idx.p, sat_idx, (size_t)n_sat * max_neighs * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess && n_unsat > 0) e = cudaMemcpyAsync(d_unsat.p, unsat, n_unsat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess && n_unsat > 0) e = cudaMemcpyAsync(d_uidx.p, unsat_idx, n_unsat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) {
         SepalParams p;
-        p.vals = d_vals.p, p.n_genes = n_genes, p.n = n, p.sat = d_sat.p, p.sat_idx = d_idx.p, p.n_sat = (int)n_sat, p.K = max_neighs;
+        p.vals = d_vals, p.n_genes = n_genes, p.n = n, p.sat = d_sat.p, p.sat_idx = d_idx.p, p.n_sat = (int)n_sat, p.K = max_neighs;
         p.unsat = d_unsat.p, p.unsat_idx = d_uidx.p, p.n_unsat = (int)n_unsat, p.use_hex = max_neighs == 6, p.n_iter = n_iter, p.dt = dt, p.thresh = thresh;
         p.out = d_out.p, p.g_scratch = global ? d_scr.p : nullptr, p.counter = d_cnt.p;
         SqbLaunchScope scope(c, SQB_K_MISC);
@@ -177,6 +179,37 @@ int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, cons
         return SQB_ERR_CUDA;
     }
     return SQB_OK;
+}
+
+extern "C" {
+
+int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, const int32_t* sat, int64_t n_sat, const int32_t* sat_idx,
+              int max_neighs, const int32_t* unsat, const int32_t* unsat_idx, int64_t n_unsat, int n_iter, double dt, double thresh,
+              double* out) {
+    SQB_CHECK(ctx && vals && sat && sat_idx && out && (n_unsat == 0 || (unsat && unsat_idx)), SQB_ERR_INVALID, "sqb_sepal: null argument");
+    SQB_TRY(sepal_check(sat, n_sat, sat_idx, max_neighs, unsat, unsat_idx, n_unsat, n_genes, n, n_iter));
+    sqb_ctx* c = ctx;
+    SQB_CUDA(cudaSetDevice(c->device));
+    DevBuf<double> d_vals;
+    SQB_TRY(d_vals.alloc((size_t)n_genes * n));
+    int rc = sqb_h2d(c, d_vals.p, vals, (size_t)n_genes * n * sizeof(double));
+    if (rc == SQB_OK)
+        rc = sepal_impl(c, d_vals.p, n_genes, n, sat, n_sat, sat_idx, max_neighs, unsat, unsat_idx, n_unsat, n_iter, dt, thresh, out);
+    else
+        cudaStreamSynchronize(c->stream);
+    d_vals.release();
+    return rc;
+}
+
+int sqb_sepal_dense(const sqb_dense* x, const int32_t* sat, int64_t n_sat, const int32_t* sat_idx, int max_neighs, const int32_t* unsat,
+                    const int32_t* unsat_idx, int64_t n_unsat, int n_iter, double dt, double thresh, double* out) {
+    SQB_CHECK(x && sat && sat_idx && out && (n_unsat == 0 || (unsat && unsat_idx)), SQB_ERR_INVALID, "sqb_sepal_dense: null argument");
+    SQB_CHECK(x->layout == 1 && x->dtype == 1, SQB_ERR_INVALID, "sqb_sepal_dense: expected a float64 genes x observations matrix");
+    SQB_TRY(sepal_check(sat, n_sat, sat_idx, max_neighs, unsat, unsat_idx, n_unsat, x->n_genes, x->n_obs, n_iter));
+    sqb_ctx* c = x->ctx;
+    SQB_CUDA(cudaSetDevice(c->device));
+    return sepal_impl(c, reinterpret_cast<const double*>(x->buf.p), x->n_genes, x->n_obs, sat, n_sat, sat_idx, max_neighs, unsat, unsat_idx,
+                      n_unsat, n_iter, dt, thresh, out);
 }
 
 }  // extern "C"

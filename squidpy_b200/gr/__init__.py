@@ -2,7 +2,7 @@
 
 from ._build import (GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, knn_2d, radius_2d, spatial_neighbors_grid,
                      spatial_neighbors_knn, spatial_neighbors_radius)
-from ._ligrec import ligrec, ligrec_analysis
+from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
 from ._nhood import NhoodEnrichmentResult, NhoodPlan, interaction_matrix, nhood_enrichment
 from ._ppatterns import AutocorrPlan, co_occurrence, cooc_counts, spatial_autocorr
 from ._ripley import pair_counts, ripley
@@ -22,6 +22,7 @@ __all__ = [
     "sepal",
     "sepal_scores",
     "ligrec_analysis",
+    "ligrec_analysis_device",
     "nhood_enrichment",
     "interaction_matrix",
     "spatial_autocorr",

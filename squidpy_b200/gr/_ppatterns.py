@@ -36,7 +36,7 @@ from .._validators import (
     assert_spatial_basis,
     extract_adata_if_sdata,
 )
-from ._utils import _save_data, as_csr, category_codes, logg
+from ._utils import _save_data, as_csr, category_codes, logg, var_positions
 
 __all__ = ["spatial_autocorr", "co_occurrence", "AutocorrPlan", "cooc_counts"]
 
@@ -256,15 +256,6 @@ def spatial_autocorr(
             subset = adata[:, genes]
             return (subset.X if layer is None else subset.layers[layer]), genes
         return adata.raw[:, genes].X, genes
-
-    def var_positions(var_names, genes):  # adata[:, genes] as column positions (names, or integer positions)
-        sel = np.asarray(genes)
-        if sel.dtype.kind in "iu":
-            return sel.astype(np.int64)
-        ix = pd.Index(var_names).get_indexer(sel)
-        if (ix < 0).any():
-            raise KeyError(f"Values {[str(s) for s, i in zip(sel, ix) if i < 0]} are not valid var names or indices.")
-        return ix.astype(np.int64)
 
     def extract_obs(cols):
         if cols is None:

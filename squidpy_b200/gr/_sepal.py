@@ -14,10 +14,11 @@ import pandas as pd
 from scipy.sparse import csr_matrix, issparse
 
 from .._constants import Key
-from .._device import on_host
+from .._device import DevMatrix, device_matrix, on_host
 from .._lib import Context, check, default_context, load
 from .._validators import assert_connectivity_key, assert_spatial_basis, extract_adata_if_sdata
-from ._utils import _save_data, logg
+from ._gather import GENE_MAJOR, Gathered, device_context
+from ._utils import _save_data, logg, var_positions
 
 __all__ = ["sepal", "sepal_scores"]
 
@@ -48,8 +49,14 @@ def _compute_idxs(g: csr_matrix, spatial: np.ndarray, sat_thresh: int):
 
 
 def sepal_scores(vals: Any, sat, sat_idx, unsat, unsat_idx, *, max_neighs: int, n_iter: int = 30000, dt: float = 0.001,
-                 thresh: float = 1e-8, ctx: Context | None = None) -> np.ndarray:
-    """``_diffusion_genes`` (``_sepal.py:186-233``): ``vals`` observations x genes (dense or scipy sparse) -> float64 score per gene."""
+                 thresh: float = 1e-8, ctx: Context | None = None, batch_genes: int | None = None) -> np.ndarray:
+    """``_diffusion_genes`` (``_sepal.py:186-233``): ``vals`` observations x genes (dense or scipy sparse, or a matrix in GPU
+    memory: see ``sepal``) -> float64 score per gene.  The genes are scored in batches of ``batch_genes`` (default: as many as
+    fill 1 GB of dense float64)."""
+    if device_matrix(vals) is not None:
+        m, on = device_context(vals, None if ctx is None else ctx.device)
+        return _scores_device(m, ctx or on, np.arange(m.shape[1]), sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=n_iter, dt=dt,
+                              thresh=thresh, batch_genes=batch_genes)
     lib = load()
     ctx = ctx or default_context()
     n, n_genes = vals.shape
@@ -58,7 +65,7 @@ def sepal_scores(vals: Any, sat, sat_idx, unsat, unsat_idx, *, max_neighs: int, 
     sat_idx = np.ascontiguousarray(sat_idx, dtype=np.int32)
     unsat = np.ascontiguousarray(unsat, dtype=np.int32)
     unsat_idx = np.ascontiguousarray(unsat_idx, dtype=np.int32)
-    step = max(1, min(n_genes, (1 << 30) // (8 * max(n, 1))))  # <= 1 GB of dense float64 per device call
+    step = _batch(n, n_genes, batch_genes)
     sparse = issparse(vals)
     if sparse:
         vals = vals.tocsc()
@@ -69,6 +76,35 @@ def sepal_scores(vals: Any, sat, sat_idx, unsat, unsat_idx, *, max_neighs: int, 
             dense = np.ascontiguousarray((blk.toarray() if sparse else np.asarray(blk)).T, dtype=np.float64)  # genes x observations
             check(lib.sqb_sepal(ctx.handle, dense.ctypes.data, g1 - g0, n, sat.ctypes.data, sat.size, sat_idx.ctypes.data, int(max_neighs),
                                 unsat.ctypes.data, unsat_idx.ctypes.data, unsat.size, int(n_iter), float(dt), float(thresh), out[g0:g1].ctypes.data))
+    return out
+
+
+def _batch(n: int, n_genes: int, batch_genes: int | None) -> int:
+    if batch_genes is not None:
+        if int(batch_genes) < 1:
+            raise ValueError(f"Expected `batch_genes` to be positive, found `{batch_genes}`.")
+        return min(n_genes, int(batch_genes))
+    return max(1, min(n_genes, (1 << 30) // (8 * max(n, 1))))  # <= 1 GB of dense float64 per device call
+
+
+def _scores_device(m: DevMatrix, ctx: Context, positions: np.ndarray, sat, sat_idx, unsat, unsat_idx, *, max_neighs: int, n_iter: int,
+                   dt: float, thresh: float, batch_genes: int | None) -> np.ndarray:
+    """``sepal_scores`` of the columns ``positions`` of a device matrix: every batch is gathered on the device (genes x
+    observations, float64, NaN kept as the host path keeps it) and scored there."""
+    lib = load()
+    n, n_genes = m.shape[0], len(positions)
+    out = np.empty(n_genes, dtype=np.float64)
+    sat = np.ascontiguousarray(sat, dtype=np.int32)
+    sat_idx = np.ascontiguousarray(sat_idx, dtype=np.int32)
+    unsat = np.ascontiguousarray(unsat, dtype=np.int32)
+    unsat_idx = np.ascontiguousarray(unsat_idx, dtype=np.int32)
+    step = _batch(n, n_genes, batch_genes)
+    with ctx.lock:
+        for g0 in range(0, n_genes, step):
+            g1 = min(g0 + step, n_genes)
+            with Gathered(ctx, m, None, positions[g0:g1], GENE_MAJOR, nan_zero=False) as x:
+                check(lib.sqb_sepal_dense(x.handle, sat.ctypes.data, sat.size, sat_idx.ctypes.data, int(max_neighs), unsat.ctypes.data,
+                                          unsat_idx.ctypes.data, unsat.size, int(n_iter), float(dt), float(thresh), out[g0:g1].ctypes.data))
     return out
 
 
@@ -106,12 +142,26 @@ def sepal(adata: Any, max_neighs: int, genes: str | Sequence[str] | None = None,
     src = adata.raw if use_raw else adata
     if use_raw:
         genes = list(set(src.var_names) & set(genes))
-    sub = src[:, genes]
-    vals = sub.X if (layer is None or use_raw) else sub.layers[layer]
-    start = time.perf_counter()
-    logg.info("Calculating sepal score for `%d` genes on the GPU", len(genes))
-    score = sepal_scores(vals, sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter), dt=dt, thresh=thresh,
-                         ctx=default_context(device))
+    whole = src.X if (layer is None or use_raw) else src.layers[layer]
+    if device_matrix(whole) is not None:  # the genes are gathered by position on the array's device; X is not read on the host
+        m, ctx = device_context(whole, device)
+        if m.shape[0] != adata.shape[0]:
+            raise ValueError(f"Expected the expression matrix to have `{adata.shape[0]}` rows, found `{m.shape[0]}`.")
+        positions = var_positions(src.var_names, genes)  # names or integer positions, as src[:, genes] takes them
+        if ((positions < -m.shape[1]) | (positions >= m.shape[1])).any():
+            raise IndexError(f"Gene positions must lie in [-{m.shape[1]}, {m.shape[1]}).")
+        positions = positions % m.shape[1]  # negative positions count from the end, as in X[:, genes]
+        start = time.perf_counter()
+        logg.info("Calculating sepal score for `%d` genes on the GPU", len(genes))
+        score = _scores_device(m, ctx, positions, sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter),
+                               dt=dt, thresh=thresh, batch_genes=None)
+    else:
+        sub = src[:, genes]
+        vals = sub.X if (layer is None or use_raw) else sub.layers[layer]
+        start = time.perf_counter()
+        logg.info("Calculating sepal score for `%d` genes on the GPU", len(genes))
+        score = sepal_scores(vals, sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter), dt=dt, thresh=thresh,
+                             ctx=default_context(device))
     key_added = "sepal_score"
     sepal_score = pd.DataFrame(score, index=genes, columns=[key_added])
     if sepal_score[key_added].isna().any():

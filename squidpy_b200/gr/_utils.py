@@ -29,6 +29,19 @@ def category_codes(series, *, dtype) -> tuple[np.ndarray, int]:
     return codes.astype(dtype), len(series.cat.categories)
 
 
+def var_positions(var_names, genes) -> np.ndarray:
+    """``adata[:, genes]`` as int64 column positions: ``genes`` holds var names, or integer positions."""
+    import pandas as pd
+
+    sel = np.asarray(genes)
+    if sel.dtype.kind in "iu":
+        return sel.astype(np.int64)
+    ix = pd.Index(var_names).get_indexer(sel)
+    if (ix < 0).any():
+        raise KeyError(f"Values {[str(s) for s, i in zip(sel, ix) if i < 0]} are not valid var names or indices.")
+    return ix.astype(np.int64)
+
+
 def as_csr(mat):
     import scipy.sparse as sp
 

@@ -9,9 +9,15 @@
 // One CTA owns one gene at a time (genes are independent; up to 30 000 dependent iterations each): the concentration and the
 // increment vector live in shared memory (2 x 8 bytes per spot; global scratch beyond ~14 000 spots), the neighbour tables are
 // re-read through L1 every iteration, two block barriers + one fixed-order block reduction of (sum x, sum x log x) per
-// iteration (ent = log S - sum(x log x) / S is the same entropy with one pass instead of two).  float64 throughout; the
-// reference compiles with numba fastmath (re-associated sums, approximate log), so the stopping iteration can differ by one
-// or two steps on genes whose entropy change crosses the threshold very slowly — the tests allow for exactly that.
+// iteration (ent = log S - sum(x log x) / S is the same entropy with one pass instead of two).  float64 throughout.
+// The reference's entropy clamps p = x / S to at least eps before the log; this one does not.  For one entry with p < eps the
+// two terms differ by p (log eps - log p) <= eps / e ~ 8.2e-17 (the maximum, at p = eps / e), so after the division by n_sat the
+// entropies differ by at most 8.2e-17 times the clamped fraction of the saturated spots: the clamp can move a stop only where
+// |ent change| lies within ~1.6e-16 of thresh, a decision float64 rounding alone already leaves open.
+// tests/test_gpu_sepal_exact.py pins the stopping iteration exactly, on both sides of the shared-memory rule, against a
+// float64 / long-double restatement of the reference on every gene whose decisions are well conditioned.  The reference
+// itself compiles with numba fastmath (re-associated sums, approximate log), so against its own output a stop can differ by
+// one or two steps on genes whose entropy change crosses the threshold very slowly.
 #include <math.h>
 
 #include "common.cuh"

@@ -848,28 +848,33 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
 }
 
 // ================================================================================================
+// Every buffer of a handle is allocated, used and freed in ctx->stream order, from the device pool: a handle is created and
+// destroyed per API call, and GB-sized cudaMalloc / cudaFree pairs would synchronise the device every time.  The buffers'
+// initialisers read ctx, which is declared first.
 struct sqb_autocorr {
-    sqb_ctx* ctx = nullptr;
+    explicit sqb_autocorr(sqb_ctx* c) : ctx(c) {}
+    sqb_ctx* ctx;
     int64_t n = 0, nnz = 0;
     double s0 = 0.0;
     int w_fmt = 2;  // 0 packed 8 lanes, 1 packed 16 lanes, 2 CSR, 3 compact (7 columns + one common weight in 32 bytes)
-    DevBuf<int32_t> d_wp, d_wi;
-    DevBuf<double> d_wd, d_csum;
-    DevBuf<uint2> d_rows;
+    DevBuf<int32_t> d_wp{ctx->stream}, d_wi{ctx->stream};
+    DevBuf<double> d_wd{ctx->stream}, d_csum{ctx->stream};
+    DevBuf<uint2> d_rows{ctx->stream};
     // loaded X
     int kind = 0;     // 0 none, 1 dense feat x obs, 2 dense obs x feat (zero copy tiles), 3 sparse (padded CSR by feature)
     int x_dtype = 0;  // 0 f32, 1 f64
     int64_t n_feat = 0, x_nnz = 0;
-    DevBuf<uint8_t> d_x;  // dense matrix or padded sparse values
-    DevBuf<int64_t> d_xp;  // padded segment starts (n_feat + 1)
-    DevBuf<int32_t> d_xi, d_len, d_order;
-    DevBuf<uint8_t> d_tile;
-    DevBuf<double> d_sums, d_partial, d_pnum, d_pden, d_out, d_aux, d_out_perms;
-    DevBuf<int64_t> d_perm;
-    DevBuf<int32_t> d_perm32;
-    DevBuf<unsigned int> d_seen;
-    DevBuf<uint2> d_bitmap;  // global-memory bitmap scratch (large n)
-    DevBuf<int> d_flags;     // [0] error flags, [1] feature queue counter
+    DevBuf<uint8_t> d_x{ctx->stream};   // dense matrix or padded sparse values
+    DevBuf<int64_t> d_xp{ctx->stream};  // padded segment starts (n_feat + 1)
+    DevBuf<int32_t> d_xi{ctx->stream}, d_len{ctx->stream}, d_order{ctx->stream};
+    DevBuf<uint8_t> d_tile{ctx->stream};
+    DevBuf<double> d_sums{ctx->stream}, d_partial{ctx->stream}, d_pnum{ctx->stream}, d_pden{ctx->stream}, d_out{ctx->stream}, d_aux{ctx->stream},
+        d_out_perms{ctx->stream};
+    DevBuf<int64_t> d_perm{ctx->stream};
+    DevBuf<int32_t> d_perm32{ctx->stream};
+    DevBuf<unsigned int> d_seen{ctx->stream};
+    DevBuf<uint2> d_bitmap{ctx->stream};  // global-memory bitmap scratch (large n)
+    DevBuf<int> d_flags{ctx->stream};     // [0] error flags, [1] feature queue counter
     bool aux_valid = false;
     int tiles_per_launch = 8;  // dense path: 256 features per launch
     bool ran = false;
@@ -1095,37 +1100,21 @@ static int ac_build_segments(sqb_autocorr* h, const int64_t* d_beg, const int64_
     }
     // features by decreasing length: the queue hands out the long ones first (LPT), the tail of the grid stays short
     {
-        DevBuf<unsigned int> keys_out;
-        DevBuf<int32_t> iota;
-        DevBuf<uint8_t> tmp;
-        keys_out.bind(c->stream);
-        iota.bind(c->stream);
-        tmp.bind(c->stream);
-        int rc;
-        if ((rc = keys_out.alloc(n_feat)) || (rc = iota.alloc(n_feat))) {
-            keys_out.release();
-            iota.release();
-            return rc;
-        }
+        DevBuf<unsigned int> keys_out(c->stream);
+        DevBuf<int32_t> iota(c->stream);
+        DevBuf<uint8_t> tmp(c->stream);
+        SQB_TRY(keys_out.alloc(n_feat));
+        SQB_TRY(iota.alloc(n_feat));
         std::vector<int32_t> hi((size_t)n_feat);
         for (int64_t g = 0; g < n_feat; ++g) hi[g] = (int32_t)g;
-        cudaError_t e = cudaMemcpyAsync(iota.p, hi.data(), n_feat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
+        SQB_CUDA(cudaMemcpyAsync(iota.p, hi.data(), n_feat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
         size_t tmp_bytes = 0;
-        if (e == cudaSuccess)
-            e = cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp_bytes, d_cnt, keys_out.p, iota.p, h->d_order.p, (int)n_feat, 0, 32,
-                                                          c->stream);
-        if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
-        if (e == cudaSuccess)
-            e = cub::DeviceRadixSort::SortPairsDescending(tmp.p, tmp_bytes, d_cnt, keys_out.p, iota.p, h->d_order.p, (int)n_feat, 0, 32,
-                                                          c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);  // hi must outlive the copy
-        keys_out.release();
-        iota.release();
-        tmp.release();
-        if (e != cudaSuccess) {
-            sqb_set_error("autocorr load: %s", cudaGetErrorString(e));
-            return SQB_ERR_CUDA;
-        }
+        SQB_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp_bytes, d_cnt, keys_out.p, iota.p, h->d_order.p, (int)n_feat, 0, 32,
+                                                           c->stream));
+        SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
+        SQB_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp.p, tmp_bytes, d_cnt, keys_out.p, iota.p, h->d_order.p, (int)n_feat, 0, 32,
+                                                           c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));  // hi must outlive the copy
         c->launches += 2;
     }
     // the padded starts now belong to the handle
@@ -1144,51 +1133,31 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
     const int64_t n = h->n;
     const int64_t rows = layout == 0 ? n_feat : n;
     const int64_t nz1 = nnz > 0 ? nnz : 1;
-    DevBuf<int64_t> r_ptr, t_ptr, pad;
-    DevBuf<int32_t> r_idx, t_idx;
-    DevBuf<uint8_t> r_val, t_val;
-    DevBuf<unsigned int> cnt;
-    DevBuf<unsigned long long> cursor;
-    r_ptr.bind(c->stream), t_ptr.bind(c->stream), pad.bind(c->stream), r_idx.bind(c->stream), t_idx.bind(c->stream);
-    r_val.bind(c->stream), t_val.bind(c->stream), cnt.bind(c->stream), cursor.bind(c->stream);
-    auto cleanup = [&]() {
-        r_ptr.release(), t_ptr.release(), pad.release(), r_idx.release(), t_idx.release(), r_val.release(), t_val.release();
-        cnt.release(), cursor.release();
-    };
-    int rc;
-    if ((rc = r_ptr.alloc(rows + 1)) || (rc = r_idx.alloc(nz1)) || (rc = r_val.alloc((size_t)nz1 * sizeof(XT))) ||
-        (rc = cnt.alloc(n_feat + 1)) || (rc = pad.alloc(n_feat + 1)) || (rc = h->d_flags.alloc(2))) {
-        cleanup();
-        return rc;
-    }
-    auto fail = [&](cudaError_t e) {
-        cleanup();
-        sqb_set_error("autocorr load: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    };
-    cudaError_t e = cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(r_ptr.p, h_xp, (rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) return fail(e);
-    if (nnz > 0) {
-        if (sub_start)
-            rc = sqb_h2d_gather(c, r_idx.p, h_xi, sizeof(int32_t), sub_start, sub_cnt, h_xp, rows) ||
-                 sqb_h2d_gather(c, r_val.p, h_xv, sizeof(XT), sub_start, sub_cnt, h_xp, rows);
-        else
-            rc = sqb_h2d(c, r_idx.p, h_xi, nnz * sizeof(int32_t)) || sqb_h2d(c, r_val.p, h_xv, (size_t)nnz * sizeof(XT));
-        if (rc) {
-            cleanup();
-            return SQB_ERR_CUDA;
-        }
+    DevBuf<int64_t> r_ptr(c->stream), t_ptr(c->stream), pad(c->stream);
+    DevBuf<int32_t> r_idx(c->stream), t_idx(c->stream);
+    DevBuf<uint8_t> r_val(c->stream), t_val(c->stream);
+    DevBuf<unsigned int> cnt(c->stream);
+    DevBuf<unsigned long long> cursor(c->stream);
+    SQB_TRY(r_ptr.alloc(rows + 1));
+    SQB_TRY(r_idx.alloc(nz1));
+    SQB_TRY(r_val.alloc((size_t)nz1 * sizeof(XT)));
+    SQB_TRY(cnt.alloc(n_feat + 1));
+    SQB_TRY(pad.alloc(n_feat + 1));
+    SQB_TRY(h->d_flags.alloc(2));
+    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream));
+    SQB_CUDA(cudaMemcpyAsync(r_ptr.p, h_xp, (rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+    if (nnz > 0) {  // a failed upload is reported as SQB_ERR_CUDA, whatever the copy returned
+        const bool failed = sub_start ? sqb_h2d_gather(c, r_idx.p, h_xi, sizeof(int32_t), sub_start, sub_cnt, h_xp, rows) ||
+                                            sqb_h2d_gather(c, r_val.p, h_xv, sizeof(XT), sub_start, sub_cnt, h_xp, rows)
+                                      : sqb_h2d(c, r_idx.p, h_xi, nnz * sizeof(int32_t)) || sqb_h2d(c, r_val.p, h_xv, (size_t)nnz * sizeof(XT));
+        if (failed) return SQB_ERR_CUDA;
     }
     {
         SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
         ac_check_indptr_kernel<int64_t><<<c->sm_count * 4, 256, 0, c->stream>>>(r_ptr.p, rows, nnz, h->d_flags.p);
     }
     // the kernels below follow indptr: a bad one must stop the load before they read or write outside [0, nnz)
-    if ((rc = ac_check_flags(h, "sqb_autocorr_load_csr"))) {
-        cleanup();
-        return rc;
-    }
+    SQB_TRY(ac_check_flags(h, "sqb_autocorr_load_csr"));
     const int64_t* seg_ptr;
     const int32_t* seg_idx;
     const XT* seg_val;
@@ -1199,13 +1168,11 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
         seg_idx = r_idx.p;
         seg_val = reinterpret_cast<const XT*>(r_val.p);
     } else {
-        if ((rc = t_ptr.alloc(n_feat + 1)) || (rc = t_idx.alloc(nz1)) || (rc = t_val.alloc((size_t)nz1 * sizeof(XT))) ||
-            (rc = cursor.alloc(n_feat + 1))) {
-            cleanup();
-            return rc;
-        }
-        e = cudaMemsetAsync(cnt.p, 0, (n_feat + 1) * sizeof(unsigned int), c->stream);
-        if (e != cudaSuccess) return fail(e);
+        SQB_TRY(t_ptr.alloc(n_feat + 1));
+        SQB_TRY(t_idx.alloc(nz1));
+        SQB_TRY(t_val.alloc((size_t)nz1 * sizeof(XT)));
+        SQB_TRY(cursor.alloc(n_feat + 1));
+        SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_feat + 1) * sizeof(unsigned int), c->stream));
         {
             SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
             const size_t hist_bytes = (size_t)n_feat * sizeof(unsigned int);
@@ -1231,12 +1198,10 @@ static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t
         seg_idx = t_idx.p;
         seg_val = reinterpret_cast<const XT*>(t_val.p);
     }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(e);
-    rc = ac_build_segments<int32_t, XT, XT>(h, seg_ptr, seg_ptr + 1, cnt.p, pad.p, seg_idx, seg_val, nnz, n_feat);
+    SQB_POST_LAUNCH();
+    int rc = ac_build_segments<int32_t, XT, XT>(h, seg_ptr, seg_ptr + 1, cnt.p, pad.p, seg_idx, seg_val, nnz, n_feat);
     if (rc == SQB_OK) rc = ac_check_flags(h, "sqb_autocorr_load_csr");  // synchronises: the temporaries may go
     else cudaStreamSynchronize(c->stream);
-    cleanup();
     h->x_nnz = nnz;
     return rc;
 }
@@ -1270,13 +1235,11 @@ static int ac_load_csr_device_typed(sqb_autocorr* h, const IP* xp, const II* xi,
     sqb_ctx* c = h->ctx;
     const int64_t n = h->n;
     const int64_t rows = layout == 0 ? n_cols : n;
-    DevBuf<int32_t> map, t_idx;
-    DevBuf<XT> t_val;
-    DevBuf<int64_t> beg, end, t_ptr, pad;
-    DevBuf<unsigned int> cnt;
-    DevBuf<unsigned long long> cursor;
-    map.bind(c->stream), t_idx.bind(c->stream), t_val.bind(c->stream), beg.bind(c->stream), end.bind(c->stream);
-    t_ptr.bind(c->stream), pad.bind(c->stream), cnt.bind(c->stream), cursor.bind(c->stream);
+    DevBuf<int32_t> map(c->stream), t_idx(c->stream);
+    DevBuf<XT> t_val(c->stream);
+    DevBuf<int64_t> beg(c->stream), end(c->stream), t_ptr(c->stream), pad(c->stream);
+    DevBuf<unsigned int> cnt(c->stream);
+    DevBuf<unsigned long long> cursor(c->stream);
     int64_t sel = 0;
     auto body = [&]() -> int {
         SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream));
@@ -1341,8 +1304,6 @@ static int ac_load_csr_device_typed(sqb_autocorr* h, const IP* xp, const II* xi,
     int rc = body();
     if (rc == SQB_OK) rc = ac_check_flags(h, where);  // synchronises: the caller's buffers are no longer read
     else cudaStreamSynchronize(c->stream);
-    map.release(), t_idx.release(), t_val.release(), beg.release(), end.release(), t_ptr.release(), pad.release(), cnt.release();
-    cursor.release();
     h->x_nnz = sel;
     return rc;
 }
@@ -1411,34 +1372,25 @@ int sqb_autocorr_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const int32_t* w_i
                 }
     }
     SQB_CUDA(cudaSetDevice(ctx->device));
-    sqb_autocorr* h = new sqb_autocorr();
-    h->ctx = ctx;
-    {  // stream-ordered allocation from the device pool: a handle is created and destroyed per API call, and GB-sized
-       // cudaMalloc / cudaFree pairs would synchronise the device every time
-        cudaStream_t st = ctx->stream;
-        h->d_wp.bind(st), h->d_wi.bind(st), h->d_wd.bind(st), h->d_csum.bind(st), h->d_rows.bind(st), h->d_x.bind(st), h->d_xp.bind(st);
-        h->d_xi.bind(st), h->d_len.bind(st), h->d_order.bind(st), h->d_tile.bind(st), h->d_sums.bind(st), h->d_partial.bind(st);
-        h->d_pnum.bind(st), h->d_pden.bind(st), h->d_out.bind(st), h->d_aux.bind(st), h->d_out_perms.bind(st), h->d_perm.bind(st);
-        h->d_perm32.bind(st), h->d_seen.bind(st), h->d_bitmap.bind(st), h->d_flags.bind(st);
-    }
+    std::unique_ptr<sqb_autocorr> h(new sqb_autocorr(ctx));
     h->n = n;
     h->nnz = nnz;
     h->s0 = s0;
     // packed rows hold float32 weights: only for float32 W (lossless); float64 W walks the CSR
     h->w_fmt = uniform7 ? 3 : (w_dtype == 0 && maxdeg <= 8) ? 0 : (w_dtype == 0 && maxdeg <= 16) ? 1 : 2;
     const int lpr = h->w_fmt == 3 ? 4 : h->w_fmt == 0 ? 8 : 16;  // uint2 units per row
-    int rc;
-    if ((rc = h->d_wp.alloc(n + 1)) || (rc = h->d_wi.alloc(nnz > 0 ? nnz : 1)) || (rc = h->d_wd.alloc(nnz > 0 ? nnz : 1)) ||
-        (rc = h->d_csum.alloc(n)) || (rc = h->d_flags.alloc(2)) || (h->w_fmt != 2 && (rc = h->d_rows.alloc((size_t)n * lpr)))) {
-        sqb_autocorr_destroy(h);
-        return rc;
-    }
-    cudaError_t e = cudaMemcpyAsync(h->d_wp.p, w_indptr, (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && nnz > 0) e = cudaMemcpyAsync(h->d_wi.p, w_indices, nnz * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && nnz > 0) e = cudaMemcpyAsync(h->d_wd.p, wd.data(), nnz * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->d_csum.p, csum.data(), n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), ctx->stream);
-    if (e == cudaSuccess && h->w_fmt != 2) {
+    SQB_TRY(h->d_wp.alloc(n + 1));
+    SQB_TRY(h->d_wi.alloc(nnz > 0 ? nnz : 1));
+    SQB_TRY(h->d_wd.alloc(nnz > 0 ? nnz : 1));
+    SQB_TRY(h->d_csum.alloc(n));
+    SQB_TRY(h->d_flags.alloc(2));
+    if (h->w_fmt != 2) SQB_TRY(h->d_rows.alloc((size_t)n * lpr));
+    SQB_CUDA(cudaMemcpyAsync(h->d_wp.p, w_indptr, (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    if (nnz > 0) SQB_CUDA(cudaMemcpyAsync(h->d_wi.p, w_indices, nnz * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    if (nnz > 0) SQB_CUDA(cudaMemcpyAsync(h->d_wd.p, wd.data(), nnz * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    SQB_CUDA(cudaMemcpyAsync(h->d_csum.p, csum.data(), n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), ctx->stream));
+    if (h->w_fmt != 2) {
         ctx->launches += 1;
         if (h->w_fmt == 3)
             ac_pack_rows32_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n,
@@ -1447,44 +1399,16 @@ int sqb_autocorr_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const int32_t* w_i
             ac_pack_rows_kernel<8><<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, h->d_rows.p);
         else
             ac_pack_rows_kernel<16><<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, h->d_rows.p);
-        e = cudaGetLastError();
+        SQB_POST_LAUNCH();
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // wd / csum are host temporaries
-    if (e != cudaSuccess) {
-        sqb_autocorr_destroy(h);
-        sqb_set_error("sqb_autocorr_create: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
-    *out = h;
+    SQB_CUDA(cudaStreamSynchronize(ctx->stream));  // wd / csum are host temporaries
+    *out = h.release();
     return SQB_OK;
 }
 
 int sqb_autocorr_destroy(sqb_autocorr* h) {
     if (!h) return SQB_OK;
     cudaSetDevice(h->ctx->device);
-    h->d_wp.release();
-    h->d_wi.release();
-    h->d_wd.release();
-    h->d_csum.release();
-    h->d_rows.release();
-    h->d_x.release();
-    h->d_xp.release();
-    h->d_xi.release();
-    h->d_len.release();
-    h->d_order.release();
-    h->d_tile.release();
-    h->d_sums.release();
-    h->d_partial.release();
-    h->d_pnum.release();
-    h->d_pden.release();
-    h->d_out.release();
-    h->d_aux.release();
-    h->d_out_perms.release();
-    h->d_perm.release();
-    h->d_perm32.release();
-    h->d_seen.release();
-    h->d_bitmap.release();
-    h->d_flags.release();
     delete h;
     return SQB_OK;
 }
@@ -1648,25 +1572,20 @@ int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, 
     // zero-copy tiles read up to 31 elements past the last feature of a row: pad the allocation (as sqb_autocorr_load_dense)
     SQB_TRY(h->d_x.alloc((size_t)n_out * h->n * xsize(xt) + 64 * 8));
     SQB_TRY(h->d_out.alloc((size_t)n_out));
-    DevBuf<int32_t> map;
-    map.bind(c->stream);
+    DevBuf<int32_t> map(c->stream);
     SQB_TRY(map.alloc(n_out));
-    int rc = SQB_OK;
-    cudaError_t e = cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) {
-        sqb_set_error("%s: %s", where, cudaGetErrorString(e));
-        rc = SQB_ERR_CUDA;
-    } else {
+    auto gather = [&]() -> int {
+        SQB_CUDA(cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
         switch (x_dtype) {
-            case 0: rc = ac_gather_dense<float, float>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
-            case 1: rc = ac_gather_dense<double, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
-            case 2: rc = ac_gather_dense<__half, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
-            case 3: rc = ac_gather_dense<int32_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
-            default: rc = ac_gather_dense<int64_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout); break;
+            case 0: return ac_gather_dense<float, float>(h, x, n_out, s_obs, s_feat, map.p, layout);
+            case 1: return ac_gather_dense<double, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
+            case 2: return ac_gather_dense<__half, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
+            case 3: return ac_gather_dense<int32_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
+            default: return ac_gather_dense<int64_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
         }
-    }
-    map.release();
-    e = cudaStreamSynchronize(c->stream);  // the caller's buffer is no longer read
+    };
+    const int rc = gather();
+    const cudaError_t e = cudaStreamSynchronize(c->stream);  // the caller's buffer is no longer read
     SQB_TRY(rc);
     SQB_CUDA(e);
     h->kind = layout == 0 ? 1 : 2;

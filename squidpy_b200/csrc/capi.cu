@@ -218,10 +218,7 @@ int sqb_ctx_destroy(sqb_ctx* c) {
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    c->scratch[0].release();
-    c->scratch[1].release();
-    c->scratch[2].release();
-    c->scratch[3].release();
+    for (auto& s : c->scratch) s.release();
     for (int b = 0; b < sqb_ctx::kStage; ++b) {
         if (c->stage_ev[b]) cudaEventDestroy(c->stage_ev[b]);
         if (c->stage[b]) cudaFreeHost(c->stage[b]);

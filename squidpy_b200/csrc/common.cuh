@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -56,20 +57,33 @@ enum {
 
 struct sqb_ctx;
 
-// RAII-less device buffer helper (explicit free).  Unbound buffers use synchronous cudaMalloc / cudaFree; a buffer bound
-// to a stream uses the stream-ordered allocator (cudaMallocAsync / cudaFreeAsync on the device's default memory pool,
-// whose release threshold sqb_ctx_create raises so freed blocks are reused): creating and destroying a handle per API
-// call then costs microseconds instead of ~1 ms of device synchronisation per buffer.
+// A device buffer that owns its allocation: the destructor frees it, so a buffer is freed when the local or the handle
+// holding it goes away, on every return path.  release() frees it earlier on purpose.  Buffers move but do not copy.
+// A default-constructed buffer uses synchronous cudaMalloc / cudaFree.  A buffer constructed with a stream uses the
+// stream-ordered allocator (cudaMallocAsync / cudaFreeAsync on that stream, from the device's default memory pool, whose
+// release threshold sqb_ctx_create raises so freed blocks are reused): creating and destroying a handle per API call then
+// costs microseconds instead of ~1 ms of device synchronisation per buffer.  Its free is enqueued on the stream, so a
+// stream-bound buffer must be destroyed before its stream is.
 template <typename T>
 struct DevBuf {
     T* p = nullptr;
     size_t n = 0;
     cudaStream_t stream = nullptr;
     bool async = false;
-    void bind(cudaStream_t s) {
-        stream = s;
-        async = true;
+    DevBuf() = default;
+    explicit DevBuf(cudaStream_t s) : stream(s), async(true) {}
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n), stream(o.stream), async(o.async) { o.p = nullptr, o.n = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) {
+            release();
+            p = o.p, n = o.n, stream = o.stream, async = o.async;
+            o.p = nullptr, o.n = 0;
+        }
+        return *this;
     }
+    ~DevBuf() { release(); }
     int alloc(size_t count) {
         if (count <= n && p) return SQB_OK;
         release();
@@ -123,8 +137,9 @@ struct sqb_ctx {
 // A dense matrix gathered from a caller's device X (sqb_dense_gather_device, dense.cu): n_obs x n_genes row-major (layout 0)
 // or n_genes x n_obs row-major (layout 1), float64 (dtype 1) or the input's own value type (DTYPE_CODES of _device.py).
 struct sqb_dense {
-    sqb_ctx* ctx = nullptr;
-    DevBuf<uint8_t> buf;
+    explicit sqb_dense(sqb_ctx* c) : ctx(c) {}
+    sqb_ctx* ctx;
+    DevBuf<uint8_t> buf{ctx->stream};  // in ctx->stream order (ctx is declared first: this initialiser reads it)
     int64_t n_obs = 0, n_genes = 0;
     int layout = 0, dtype = 1;
     bool nan_zero = false;  // NaN entries were written as 0.0

@@ -203,14 +203,12 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
     SQB_CUDA(cudaSetDevice(c->device));
     SQB_TRY(sqb_wait_producer(c, producer_stream));
     const bool keep = flags & 2, nan0 = flags & 1;
-    sqb_dense* d = new sqb_dense();
-    d->ctx = c, d->n_obs = n_rows_out, d->n_genes = n_cols_out, d->layout = layout, d->dtype = keep ? x_dtype : 1, d->nan_zero = nan0;
-    d->buf.bind(c->stream);
+    std::unique_ptr<sqb_dense> d(new sqb_dense(c));
+    d->n_obs = n_rows_out, d->n_genes = n_cols_out, d->layout = layout, d->dtype = keep ? x_dtype : 1, d->nan_zero = nan0;
     const int64_t cells = n_rows_out * n_cols_out;
-    DevBuf<int32_t> d_rmap, d_cmap;
-    DevBuf<int64_t> d_rlist;
-    DevBuf<unsigned> d_bits, d_err;
-    d_rmap.bind(c->stream), d_cmap.bind(c->stream), d_rlist.bind(c->stream), d_bits.bind(c->stream), d_err.bind(c->stream);
+    DevBuf<int32_t> d_rmap(c->stream), d_cmap(c->stream);
+    DevBuf<int64_t> d_rlist(c->stream);
+    DevBuf<unsigned> d_bits(c->stream), d_err(c->stream);
     unsigned flag = 0;
     auto body = [&]() -> int {
         SQB_TRY(d->buf.alloc((size_t)cells * kDtypeSize[d->dtype]));
@@ -265,11 +263,11 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
         const int32_t* mnr = csr ? d_cmap.p : d_rmap.p;
         int rc;
         if (indptr_bits == 32)
-            rc = index_bits == 32 ? dg_sparse_launch<int32_t, int32_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d, nan0, keep, d_bits.p, d_err.p)
-                                  : dg_sparse_launch<int32_t, int64_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d, nan0, keep, d_bits.p, d_err.p);
+            rc = index_bits == 32 ? dg_sparse_launch<int32_t, int32_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p)
+                                  : dg_sparse_launch<int32_t, int64_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p);
         else
-            rc = index_bits == 32 ? dg_sparse_launch<int64_t, int32_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d, nan0, keep, d_bits.p, d_err.p)
-                                  : dg_sparse_launch<int64_t, int64_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d, nan0, keep, d_bits.p, d_err.p);
+            rc = index_bits == 32 ? dg_sparse_launch<int64_t, int32_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p)
+                                  : dg_sparse_launch<int64_t, int64_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p);
         SQB_TRY(rc);
         SQB_CUDA(cudaMemcpyAsync(&flag, d_err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
         SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffers are no longer read
@@ -281,15 +279,11 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
         return SQB_OK;
     };
     const int rc = body();
-    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);
-    d_rmap.release(), d_cmap.release(), d_rlist.release(), d_bits.release(), d_err.release();
     if (rc != SQB_OK) {
-        d->buf.release();
-        cudaStreamSynchronize(c->stream);
-        delete d;
+        cudaStreamSynchronize(c->stream);  // the caller's buffers are no longer read
         return rc;
     }
-    *out = d;
+    *out = d.release();
     return SQB_OK;
 }
 
@@ -305,7 +299,6 @@ int sqb_dense_download(sqb_dense* d, void* out) {
 int sqb_dense_free(sqb_dense* d) {
     if (!d) return SQB_OK;
     cudaSetDevice(d->ctx->device);
-    d->buf.release();
     delete d;
     return SQB_OK;
 }
@@ -332,10 +325,9 @@ int sqb_ligrec_observed(sqb_dense* d, const int32_t* codes, int n_cls, double* m
     wpb = wpb > 4 ? 4 : wpb;
     const size_t smem = per_warp * wpb;
     SQB_CUDA(cudaSetDevice(c->device));
-    DevBuf<int32_t> d_codes;
-    DevBuf<double> d_sizes, d_mean;
-    DevBuf<long long> d_npos;
-    d_codes.bind(c->stream), d_sizes.bind(c->stream), d_mean.bind(c->stream), d_npos.bind(c->stream);
+    DevBuf<int32_t> d_codes(c->stream);
+    DevBuf<double> d_sizes(c->stream), d_mean(c->stream);
+    DevBuf<long long> d_npos(c->stream);
     auto body = [&]() -> int {
         SQB_TRY(d_codes.alloc(n));
         SQB_TRY(d_sizes.alloc(n_cls));
@@ -357,7 +349,6 @@ int sqb_ligrec_observed(sqb_dense* d, const int32_t* codes, int n_cls, double* m
     };
     const int rc = body();
     if (rc != SQB_OK) cudaStreamSynchronize(c->stream);
-    d_codes.release(), d_sizes.release(), d_mean.release(), d_npos.release();
     return rc;
 }
 

@@ -208,36 +208,27 @@ GridGeom grid_geometry(double x0, double y0, double x1, double y1, int64_t n, do
 int grid_bucket(sqb_ctx* c, int64_t n, PointGrid* g) {
     const GridGeom gm = g->gm;
     const int64_t n_cells = (int64_t)gm.gx * gm.gy;
-    DevBuf<uint32_t> cell_a, cell_b;
-    DevBuf<int32_t> idx_a;
-    DevBuf<uint8_t> tmp;
-    cell_a.bind(c->stream), cell_b.bind(c->stream), idx_a.bind(c->stream), tmp.bind(c->stream);
-    auto cleanup = [&]() { cell_a.release(), cell_b.release(), idx_a.release(), tmp.release(); };
-    int rc;
-    if ((rc = g->d_pts.alloc(n)) || (rc = g->d_idx_sorted.alloc(n)) || (rc = g->d_cell_start.alloc(n_cells + 1)) || (rc = cell_a.alloc(n)) ||
-        (rc = cell_b.alloc(n)) || (rc = idx_a.alloc(n))) {
-        cleanup();
-        return rc;
-    }
+    DevBuf<uint32_t> cell_a(c->stream), cell_b(c->stream);
+    DevBuf<int32_t> idx_a(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(g->d_pts.alloc(n));
+    SQB_TRY(g->d_idx_sorted.alloc(n));
+    SQB_TRY(g->d_cell_start.alloc(n_cells + 1));
+    SQB_TRY(cell_a.alloc(n));
+    SQB_TRY(cell_b.alloc(n));
+    SQB_TRY(idx_a.alloc(n));
     c->launches += 1;
     graph_cell_id_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, c->stream>>>(g->d_xy.p, n, gm, cell_a.p, idx_a.p);
-    cudaError_t e = cudaGetLastError();
+    SQB_POST_LAUNCH();
     int bits = 1;
     while (bits < 32 && ((uint64_t)(n_cells - 1) >> bits) != 0) ++bits;
     size_t tmp_bytes = 0;
-    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cell_a.p, cell_b.p, idx_a.p, g->d_idx_sorted.p, (int)n, 0, bits, c->stream);
-    if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
-    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, cell_a.p, cell_b.p, idx_a.p, g->d_idx_sorted.p, (int)n, 0, bits, c->stream);
-    if (e == cudaSuccess) {
-        c->launches += 2;
-        graph_gather_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, c->stream>>>(g->d_xy.p, cell_b.p, g->d_idx_sorted.p, n, n_cells, g->d_pts.p, g->d_cell_start.p);
-        e = cudaGetLastError();
-    }
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("spatial grid: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cell_a.p, cell_b.p, idx_a.p, g->d_idx_sorted.p, (int)n, 0, bits, c->stream));
+    SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
+    SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, cell_a.p, cell_b.p, idx_a.p, g->d_idx_sorted.p, (int)n, 0, bits, c->stream));
+    c->launches += 2;
+    graph_gather_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, c->stream>>>(g->d_xy.p, cell_b.p, g->d_idx_sorted.p, n, n_cells, g->d_pts.p, g->d_cell_start.p);
+    SQB_POST_LAUNCH();
     return SQB_OK;
 }
 
@@ -251,15 +242,11 @@ static int build_grid(sqb_ctx* c, const double* xy, int64_t n, double cell_hint,
     }
     g->gm = grid_geometry(x0, y0, x1, y1, n, cell_hint, pts_per_cell);
     SQB_TRY(g->d_xy.alloc(2 * n));
-    cudaError_t e = cudaMemcpyAsync(g->d_xy.p, xy, 2 * n * sizeof(double), cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) {
-        sqb_set_error("spatial grid: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cudaMemcpyAsync(g->d_xy.p, xy, 2 * n * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     return grid_bucket(c, n, g);
 }
 
-cudaError_t knn_launch(sqb_ctx* c, const PointGrid& g, int64_t n, int k, int32_t* idx, double* dist) {
+int knn_launch(sqb_ctx* c, const PointGrid& g, int64_t n, int k, int32_t* idx, double* dist) {
     SqbLaunchScope scope(c, SQB_K_MISC);
     const unsigned grid = (unsigned)ceil_div64(n, 128);
     if (k <= 8)
@@ -270,29 +257,30 @@ cudaError_t knn_launch(sqb_ctx* c, const PointGrid& g, int64_t n, int k, int32_t
         graph_knn_kernel<32><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, idx, dist);
     else
         graph_knn_kernel<64><<<grid, 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, k, idx, dist);
-    return cudaGetLastError();
+    SQB_POST_LAUNCH();
+    return SQB_OK;
 }
 
-cudaError_t median_enqueue(sqb_ctx* c, const double* dist, int64_t m, DevBuf<double>& sorted, DevBuf<uint8_t>& tmp, double* med) {
+int median_enqueue(sqb_ctx* c, const double* dist, int64_t m, DevBuf<double>& sorted, DevBuf<uint8_t>& tmp, double* med) {
     // np.median of all m distances: radix sort, the middle element (odd count) or the mean of the two middle ones
-    cudaError_t e = cudaSuccess;
     size_t tmp_bytes = 0;
-    if (sorted.alloc((size_t)m) != SQB_OK) e = cudaErrorMemoryAllocation;
-    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, dist, sorted.p, (int)m, 0, 64, c->stream);
-    if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
-    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, dist, sorted.p, (int)m, 0, 64, c->stream);
+    SQB_TRY(sorted.alloc((size_t)m));
+    SQB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, dist, sorted.p, (int)m, 0, 64, c->stream));
+    SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
+    SQB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, dist, sorted.p, (int)m, 0, 64, c->stream));
     c->launches += 1;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&med[0], sorted.p + (m - 1) / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&med[1], sorted.p + m / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    return e;
+    SQB_CUDA(cudaMemcpyAsync(&med[0], sorted.p + (m - 1) / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(&med[1], sorted.p + m / 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    return SQB_OK;
 }
 
-cudaError_t radius_launch(sqb_ctx* c, const PointGrid& g, int64_t n, double radius, int64_t* counts, const int64_t* indptr, int32_t* idx,
-                          double* dist) {
+int radius_launch(sqb_ctx* c, const PointGrid& g, int64_t n, double radius, int64_t* counts, const int64_t* indptr, int32_t* idx,
+                  double* dist) {
     SqbLaunchScope scope(c, SQB_K_MISC);
     graph_radius_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, c->stream>>>(g.d_pts.p, g.d_idx_sorted.p, g.d_cell_start.p, n, g.gm, radius,
                                                                              radius_reach(radius, g.gm), counts, indptr, idx, dist);
-    return cudaGetLastError();
+    SQB_POST_LAUNCH();
+    return SQB_OK;
 }
 
 extern "C" {
@@ -307,33 +295,19 @@ int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_id
     SQB_CHECK((int64_t)n * k < 2147483647LL, SQB_ERR_UNSUPPORTED, "sqb_knn_2d: n * k does not fit int32");
     sqb_ctx* c = ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    PointGrid g;
-    g.bind(c->stream);
-    int rc = build_grid(c, xy, n, 0.0, knn_pts_per_cell(k), &g);
-    if (rc != SQB_OK) {
-        g.release();
-        return rc;
-    }
-    DevBuf<int32_t> d_idx;
-    DevBuf<double> d_dist, d_sorted;
-    DevBuf<uint8_t> tmp;
-    d_idx.bind(c->stream), d_dist.bind(c->stream), d_sorted.bind(c->stream), tmp.bind(c->stream);
-    auto cleanup = [&]() { g.release(), d_idx.release(), d_dist.release(), d_sorted.release(), tmp.release(); };
-    if ((rc = d_idx.alloc((size_t)n * k)) || (rc = d_dist.alloc((size_t)n * k))) {
-        cleanup();
-        return rc;
-    }
-    cudaError_t e = knn_launch(c, g, n, k, d_idx.p, d_dist.p);
+    PointGrid g(c->stream);
+    SQB_TRY(build_grid(c, xy, n, 0.0, knn_pts_per_cell(k), &g));
+    DevBuf<int32_t> d_idx(c->stream);
+    DevBuf<double> d_dist(c->stream), d_sorted(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(d_idx.alloc((size_t)n * k));
+    SQB_TRY(d_dist.alloc((size_t)n * k));
+    SQB_TRY(knn_launch(c, g, n, k, d_idx.p, d_dist.p));
     double med[2] = {0.0, 0.0};
-    if (e == cudaSuccess && median_out) e = median_enqueue(c, d_dist.p, n * k, d_sorted, tmp, med);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_idx, d_idx.p, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, d_dist.p, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_knn_2d: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    if (median_out) SQB_TRY(median_enqueue(c, d_dist.p, n * k, d_sorted, tmp, med));
+    SQB_CUDA(cudaMemcpyAsync(out_idx, d_idx.p, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(out_dist, d_dist.p, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     if (median_out) *median_out = (med[0] + med[1]) / 2.0;  // numpy: mean of the two middle values (the same value twice if odd)
     return SQB_OK;
 }
@@ -345,56 +319,32 @@ int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int6
     SQB_CHECK(radius >= 0.0 && isfinite(radius), SQB_ERR_INVALID, "sqb_radius_2d: radius must be finite and non-negative");
     sqb_ctx* c = ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    PointGrid g;
-    g.bind(c->stream);
-    int rc = build_grid(c, xy, n, radius > 0.0 ? radius : 0.0, 2.5, &g);
-    if (rc != SQB_OK) {
-        g.release();
-        return rc;
-    }
-    DevBuf<int64_t> d_cnt, d_ptr;
-    DevBuf<int32_t> d_idx;
-    DevBuf<double> d_dist;
-    DevBuf<uint8_t> tmp;
-    d_cnt.bind(c->stream), d_ptr.bind(c->stream), d_idx.bind(c->stream), d_dist.bind(c->stream), tmp.bind(c->stream);
-    auto cleanup = [&]() { g.release(), d_cnt.release(), d_ptr.release(), d_idx.release(), d_dist.release(), tmp.release(); };
-    if ((rc = d_cnt.alloc(n + 1)) || (rc = d_ptr.alloc(n + 1))) {
-        cleanup();
-        return rc;
-    }
-    cudaError_t e = cudaMemsetAsync(d_cnt.p, 0, (n + 1) * sizeof(int64_t), c->stream);
-    if (e == cudaSuccess) e = radius_launch(c, g, n, radius, d_cnt.p, nullptr, nullptr, nullptr);
+    PointGrid g(c->stream);
+    SQB_TRY(build_grid(c, xy, n, radius > 0.0 ? radius : 0.0, 2.5, &g));
+    DevBuf<int64_t> d_cnt(c->stream), d_ptr(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(d_cnt.alloc(n + 1));
+    SQB_TRY(d_ptr.alloc(n + 1));
+    SQB_CUDA(cudaMemsetAsync(d_cnt.p, 0, (n + 1) * sizeof(int64_t), c->stream));
+    SQB_TRY(radius_launch(c, g, n, radius, d_cnt.p, nullptr, nullptr, nullptr));
     size_t tmp_bytes = 0;
-    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_cnt.p, d_ptr.p, (int)(n + 1), c->stream);
-    if (e == cudaSuccess && tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1) != SQB_OK) e = cudaErrorMemoryAllocation;
-    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, d_cnt.p, d_ptr.p, (int)(n + 1), c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_indptr, d_ptr.p, (n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) {
-        cleanup();
-        sqb_set_error("sqb_radius_2d: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_cnt.p, d_ptr.p, (int)(n + 1), c->stream));
+    SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
+    SQB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, d_cnt.p, d_ptr.p, (int)(n + 1), c->stream));
+    SQB_CUDA(cudaMemcpyAsync(out_indptr, d_ptr.p, (n + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     const int64_t nnz = out_indptr[n];
     *nnz_out = nnz;
-    if (!out_idx || !out_dist || capacity < nnz) {  // first call of the two-call protocol: the caller allocates nnz entries
-        cleanup();
-        return SQB_OK;
-    }
+    if (!out_idx || !out_dist || capacity < nnz) return SQB_OK;  // first call of the two-call protocol: the caller allocates nnz entries
     if (nnz > 0) {
-        if ((rc = d_idx.alloc((size_t)nnz)) || (rc = d_dist.alloc((size_t)nnz))) {
-            cleanup();
-            return rc;
-        }
-        e = radius_launch(c, g, n, radius, nullptr, d_ptr.p, d_idx.p, d_dist.p);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_idx, d_idx.p, (size_t)nnz * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, d_dist.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    }
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_radius_2d: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
+        DevBuf<int32_t> d_idx(c->stream);
+        DevBuf<double> d_dist(c->stream);
+        SQB_TRY(d_idx.alloc((size_t)nnz));
+        SQB_TRY(d_dist.alloc((size_t)nnz));
+        SQB_TRY(radius_launch(c, g, n, radius, nullptr, d_ptr.p, d_idx.p, d_dist.p));
+        SQB_CUDA(cudaMemcpyAsync(out_idx, d_idx.p, (size_t)nnz * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(out_dist, d_dist.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
     }
     return SQB_OK;
 }

@@ -34,13 +34,12 @@ enum { DST_DIST = 0, DST_ADJ = 1, DST_VAL = 2 };  // distances value: the distan
 namespace {
 
 struct Csr {
+    explicit Csr(cudaStream_t s) : ptr(s), idx(s), vf(s), vd(s) {}
     DevBuf<int32_t> ptr, idx;
     DevBuf<float> vf;   // float32 values
     DevBuf<double> vd;  // float64 values (distances of kNN / radius graphs)
     int64_t nnz = 0;
     bool f64 = false;
-    void bind(cudaStream_t s) { ptr.bind(s), idx.bind(s), vf.bind(s), vd.bind(s); }
-    void release() { ptr.release(), idx.release(), vf.release(), vd.release(); }
 };
 
 struct Params {
@@ -389,7 +388,8 @@ __global__ void gd_block_fill_kernel(const int32_t* __restrict__ ptr, const int3
 
 // ---- host steps --------------------------------------------------------------------------------------------------------
 struct sqb_graph {
-    sqb_ctx* c = nullptr;
+    explicit sqb_graph(sqb_ctx* ctx) : c(ctx), adj(ctx->stream), dst(ctx->stream) {}
+    sqb_ctx* c;
     int64_t n = 0;
     Csr adj, dst;
 };
@@ -399,160 +399,134 @@ namespace {
 // count pass -> per-row pointers of both matrices -> fill pass
 int assemble(sqb_ctx* c, const int64_t* bptr, const int32_t* bidx, const double* bval, int64_t n, const AsmParams& p, bool dst_f64, Csr* adj,
              Csr* dst) {
-    DevBuf<int32_t> ca, cd;
-    DevBuf<uint8_t> tmp;
-    ca.bind(c->stream), cd.bind(c->stream), tmp.bind(c->stream);
-    auto body = [&]() -> int {
-        SQB_TRY(ca.alloc(n + 1));
-        SQB_TRY(cd.alloc(n + 1));
-        SQB_TRY(adj->ptr.alloc(n + 1));
-        SQB_TRY(dst->ptr.alloc(n + 1));
-        SQB_CUDA(cudaMemsetAsync(ca.p + n, 0, sizeof(int32_t), c->stream));
-        SQB_CUDA(cudaMemsetAsync(cd.p + n, 0, sizeof(int32_t), c->stream));
-        GD_LAUNCH(gd_assemble_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(bptr, bidx, bval, n, p, ca.p, cd.p, nullptr, nullptr, nullptr, nullptr,
-                                                                               nullptr, nullptr, nullptr));
-        SQB_TRY(exclusive_scan(c, tmp, ca.p, adj->ptr.p, n + 1));
-        SQB_TRY(exclusive_scan(c, tmp, cd.p, dst->ptr.p, n + 1));
-        int32_t na = 0, nd = 0;
-        SQB_TRY(read_back(c, &na, adj->ptr.p + n, sizeof(int32_t)));
-        SQB_TRY(read_back(c, &nd, dst->ptr.p + n, sizeof(int32_t)));
-        adj->nnz = na, dst->nnz = nd, adj->f64 = false, dst->f64 = dst_f64;
-        SQB_TRY(adj->idx.alloc(na));
-        SQB_TRY(adj->vf.alloc(na));
-        SQB_TRY(dst->idx.alloc(nd));
-        SQB_TRY(dst_f64 ? dst->vd.alloc(nd) : dst->vf.alloc(nd));
-        GD_LAUNCH(gd_assemble_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(bptr, bidx, bval, n, p, nullptr, nullptr, adj->ptr.p, adj->idx.p, adj->vf.p,
-                                                                               dst->ptr.p, dst->idx.p, dst_f64 ? nullptr : dst->vf.p,
-                                                                               dst_f64 ? dst->vd.p : nullptr));
-        return SQB_OK;
-    };
-    const int rc = body();
-    ca.release(), cd.release(), tmp.release();
-    return rc;
+    DevBuf<int32_t> ca(c->stream), cd(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(ca.alloc(n + 1));
+    SQB_TRY(cd.alloc(n + 1));
+    SQB_TRY(adj->ptr.alloc(n + 1));
+    SQB_TRY(dst->ptr.alloc(n + 1));
+    SQB_CUDA(cudaMemsetAsync(ca.p + n, 0, sizeof(int32_t), c->stream));
+    SQB_CUDA(cudaMemsetAsync(cd.p + n, 0, sizeof(int32_t), c->stream));
+    GD_LAUNCH(gd_assemble_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(bptr, bidx, bval, n, p, ca.p, cd.p, nullptr, nullptr, nullptr, nullptr,
+                                                                           nullptr, nullptr, nullptr));
+    SQB_TRY(exclusive_scan(c, tmp, ca.p, adj->ptr.p, n + 1));
+    SQB_TRY(exclusive_scan(c, tmp, cd.p, dst->ptr.p, n + 1));
+    int32_t na = 0, nd = 0;
+    SQB_TRY(read_back(c, &na, adj->ptr.p + n, sizeof(int32_t)));
+    SQB_TRY(read_back(c, &nd, dst->ptr.p + n, sizeof(int32_t)));
+    adj->nnz = na, dst->nnz = nd, adj->f64 = false, dst->f64 = dst_f64;
+    SQB_TRY(adj->idx.alloc(na));
+    SQB_TRY(adj->vf.alloc(na));
+    SQB_TRY(dst->idx.alloc(nd));
+    SQB_TRY(dst_f64 ? dst->vd.alloc(nd) : dst->vf.alloc(nd));
+    GD_LAUNCH(gd_assemble_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(bptr, bidx, bval, n, p, nullptr, nullptr, adj->ptr.p, adj->idx.p, adj->vf.p,
+                                                                           dst->ptr.p, dst->idx.p, dst_f64 ? nullptr : dst->vf.p,
+                                                                           dst_f64 ? dst->vd.p : nullptr));
+    return SQB_OK;
 }
 
 // Xn Xn^T of the row-normalised connectivities (sklearn's cosine_similarity(adj, dense_output=False))
 int cosine(sqb_ctx* c, int64_t n, Csr* adj) {
     const int64_t m = adj->nnz;
-    DevBuf<float> xn, bval, prod, pout;
-    DevBuf<uint64_t> keys, bkeys, lkeys, lkeys_s;
-    DevBuf<int32_t> bptr, cnt;
-    DevBuf<int64_t> lcnt, lptr;
-    DevBuf<uint8_t> tmp;
-    Csr out;
-    for (auto* b : {&xn, &bval, &prod, &pout}) b->bind(c->stream);
-    for (auto* b : {&keys, &bkeys, &lkeys, &lkeys_s}) b->bind(c->stream);
-    bptr.bind(c->stream), cnt.bind(c->stream), lcnt.bind(c->stream), lptr.bind(c->stream), tmp.bind(c->stream), out.bind(c->stream);
-    auto body = [&]() -> int {
-        const unsigned gb = blocks_for(c, n);
-        SQB_TRY(xn.alloc(m));
-        GD_LAUNCH(gd_rownorm_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, n, adj->vf.p, xn.p));
-        // B = Xn^T as CSR with ascending columns (scipy converts the CSC transpose to sorted CSR)
-        SQB_TRY(keys.alloc(m));
-        SQB_TRY(bkeys.alloc(m));
-        SQB_TRY(bval.alloc(m));
-        SQB_TRY(bptr.alloc(n + 1));
-        GD_LAUNCH(gd_keys_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, 1, keys.p));
-        if (m > 0) SQB_TRY(sort_pairs(c, tmp, keys.p, bkeys.p, xn.p, bval.p, m, key_bits(n)));
-        SQB_CUDA(cudaMemsetAsync(bptr.p, 0, (n + 1) * sizeof(int32_t), c->stream));
-        if (m > 0) GD_LAUNCH(gd_ptr_from_keys_kernel<int32_t><<<blocks_for(c, m), 256, 0, c->stream>>>(bkeys.p, m, n, bptr.p));
-        // the products of every row in walk order, then stably sorted by (row, column)
-        SQB_TRY(lcnt.alloc(n + 1));
-        SQB_TRY(lptr.alloc(n + 1));
-        SQB_CUDA(cudaMemsetAsync(lcnt.p + n, 0, sizeof(int64_t), c->stream));
-        GD_LAUNCH(gd_prod_count_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, bptr.p, lcnt.p));
-        SQB_TRY(exclusive_scan(c, tmp, lcnt.p, lptr.p, n + 1));
-        int64_t L = 0;
-        SQB_TRY(read_back(c, &L, lptr.p + n, sizeof(int64_t)));
-        SQB_CHECK(L < INT_MAX, SQB_ERR_UNSUPPORTED, "cosine transform: %lld products exceed 2^31 - 1", (long long)L);
-        SQB_TRY(lkeys.alloc(L));
-        SQB_TRY(lkeys_s.alloc(L));
-        SQB_TRY(prod.alloc(L));
-        SQB_TRY(pout.alloc(L));
-        GD_LAUNCH(gd_prod_fill_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, xn.p, n, bptr.p, bkeys.p, bval.p, lptr.p, lkeys.p, prod.p));
-        if (L > 0) SQB_TRY(sort_pairs(c, tmp, lkeys.p, lkeys_s.p, prod.p, pout.p, L, key_bits(n)));
-        // column sums in order; zero sums dropped (csr_matmat)
-        SQB_TRY(cnt.alloc(n + 1));
-        SQB_TRY(out.ptr.alloc(n + 1));
-        SQB_CUDA(cudaMemsetAsync(cnt.p + n, 0, sizeof(int32_t), c->stream));
-        GD_LAUNCH(gd_prod_reduce_kernel<<<gb, 256, 0, c->stream>>>(lptr.p, lkeys_s.p, pout.p, n, cnt.p, nullptr, nullptr, nullptr));
-        SQB_TRY(exclusive_scan(c, tmp, cnt.p, out.ptr.p, n + 1));
-        int32_t nnz = 0;
-        SQB_TRY(read_back(c, &nnz, out.ptr.p + n, sizeof(int32_t)));
-        SQB_TRY(out.idx.alloc(nnz));
-        SQB_TRY(out.vf.alloc(nnz));
-        GD_LAUNCH(gd_prod_reduce_kernel<<<gb, 256, 0, c->stream>>>(lptr.p, lkeys_s.p, pout.p, n, nullptr, out.ptr.p, out.idx.p, out.vf.p));
-        out.nnz = nnz;
-        std::swap(*adj, out);
-        return SQB_OK;
-    };
-    const int rc = body();
-    for (auto* b : {&xn, &bval, &prod, &pout}) b->release();
-    for (auto* b : {&keys, &bkeys, &lkeys, &lkeys_s}) b->release();
-    bptr.release(), cnt.release(), lcnt.release(), lptr.release(), tmp.release(), out.release();
-    return rc;
+    DevBuf<float> xn(c->stream), bval(c->stream), prod(c->stream), pout(c->stream);
+    DevBuf<uint64_t> keys(c->stream), bkeys(c->stream), lkeys(c->stream), lkeys_s(c->stream);
+    DevBuf<int32_t> bptr(c->stream), cnt(c->stream);
+    DevBuf<int64_t> lcnt(c->stream), lptr(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    Csr out(c->stream);
+    const unsigned gb = blocks_for(c, n);
+    SQB_TRY(xn.alloc(m));
+    GD_LAUNCH(gd_rownorm_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, n, adj->vf.p, xn.p));
+    // B = Xn^T as CSR with ascending columns (scipy converts the CSC transpose to sorted CSR)
+    SQB_TRY(keys.alloc(m));
+    SQB_TRY(bkeys.alloc(m));
+    SQB_TRY(bval.alloc(m));
+    SQB_TRY(bptr.alloc(n + 1));
+    GD_LAUNCH(gd_keys_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, 1, keys.p));
+    if (m > 0) SQB_TRY(sort_pairs(c, tmp, keys.p, bkeys.p, xn.p, bval.p, m, key_bits(n)));
+    SQB_CUDA(cudaMemsetAsync(bptr.p, 0, (n + 1) * sizeof(int32_t), c->stream));
+    if (m > 0) GD_LAUNCH(gd_ptr_from_keys_kernel<int32_t><<<blocks_for(c, m), 256, 0, c->stream>>>(bkeys.p, m, n, bptr.p));
+    // the products of every row in walk order, then stably sorted by (row, column)
+    SQB_TRY(lcnt.alloc(n + 1));
+    SQB_TRY(lptr.alloc(n + 1));
+    SQB_CUDA(cudaMemsetAsync(lcnt.p + n, 0, sizeof(int64_t), c->stream));
+    GD_LAUNCH(gd_prod_count_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, bptr.p, lcnt.p));
+    SQB_TRY(exclusive_scan(c, tmp, lcnt.p, lptr.p, n + 1));
+    int64_t L = 0;
+    SQB_TRY(read_back(c, &L, lptr.p + n, sizeof(int64_t)));
+    SQB_CHECK(L < INT_MAX, SQB_ERR_UNSUPPORTED, "cosine transform: %lld products exceed 2^31 - 1", (long long)L);
+    SQB_TRY(lkeys.alloc(L));
+    SQB_TRY(lkeys_s.alloc(L));
+    SQB_TRY(prod.alloc(L));
+    SQB_TRY(pout.alloc(L));
+    GD_LAUNCH(gd_prod_fill_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, xn.p, n, bptr.p, bkeys.p, bval.p, lptr.p, lkeys.p, prod.p));
+    if (L > 0) SQB_TRY(sort_pairs(c, tmp, lkeys.p, lkeys_s.p, prod.p, pout.p, L, key_bits(n)));
+    // column sums in order; zero sums dropped (csr_matmat)
+    SQB_TRY(cnt.alloc(n + 1));
+    SQB_TRY(out.ptr.alloc(n + 1));
+    SQB_CUDA(cudaMemsetAsync(cnt.p + n, 0, sizeof(int32_t), c->stream));
+    GD_LAUNCH(gd_prod_reduce_kernel<<<gb, 256, 0, c->stream>>>(lptr.p, lkeys_s.p, pout.p, n, cnt.p, nullptr, nullptr, nullptr));
+    SQB_TRY(exclusive_scan(c, tmp, cnt.p, out.ptr.p, n + 1));
+    int32_t nnz = 0;
+    SQB_TRY(read_back(c, &nnz, out.ptr.p + n, sizeof(int32_t)));
+    SQB_TRY(out.idx.alloc(nnz));
+    SQB_TRY(out.vf.alloc(nnz));
+    GD_LAUNCH(gd_prod_reduce_kernel<<<gb, 256, 0, c->stream>>>(lptr.p, lkeys_s.p, pout.p, n, nullptr, out.ptr.p, out.idx.p, out.vf.p));
+    out.nnz = nnz;
+    std::swap(*adj, out);
+    return SQB_OK;
 }
 
 // Entries (i, j) of graph distance 1 .. n_rings from i in the cut graph `cut`, as a base table (int64 pointers, ring numbers)
 int rings(sqb_ctx* c, int64_t n, const Csr& cut, int n_rings, DevBuf<int64_t>& tptr, DevBuf<int32_t>& tidx, DevBuf<double>& tval) {
-    DevBuf<uint64_t> keys, ekeys, skeys;
-    DevBuf<float> lvl, elvl, slvl;
-    DevBuf<int64_t> ecnt, eptr;
-    DevBuf<int32_t> flag, pos;
-    DevBuf<uint8_t> tmp;
-    for (auto* b : {&keys, &ekeys, &skeys}) b->bind(c->stream);
-    for (auto* b : {&lvl, &elvl, &slvl}) b->bind(c->stream);
-    ecnt.bind(c->stream), eptr.bind(c->stream), flag.bind(c->stream), pos.bind(c->stream), tmp.bind(c->stream);
-    auto body = [&]() -> int {
-        int64_t m = cut.nnz;
-        SQB_TRY(keys.alloc(m));
-        SQB_TRY(lvl.alloc(m));
-        GD_LAUNCH(gd_ring_init_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(cut.ptr.p, cut.idx.p, n, keys.p, lvl.p));
-        for (int level = 1; level < n_rings && m > 0; ++level) {
-            SQB_TRY(ecnt.alloc(m + 1));
-            SQB_TRY(eptr.alloc(m + 1));
-            SQB_CUDA(cudaMemsetAsync(ecnt.p + m, 0, sizeof(int64_t), c->stream));
-            GD_LAUNCH(gd_ring_count_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, lvl.p, m, (float)level, cut.ptr.p, ecnt.p));
-            SQB_TRY(exclusive_scan(c, tmp, ecnt.p, eptr.p, m + 1));
-            int64_t e = 0;
-            SQB_TRY(read_back(c, &e, eptr.p + m, sizeof(int64_t)));
-            if (e == 0) break;
-            const int64_t t = m + e;
-            SQB_CHECK(t < INT_MAX, SQB_ERR_UNSUPPORTED, "n_rings=%d: %lld candidate entries exceed 2^31 - 1", n_rings, (long long)t);
-            SQB_TRY(ekeys.alloc(t));
-            SQB_TRY(elvl.alloc(t));
-            SQB_TRY(skeys.alloc(t));
-            SQB_TRY(slvl.alloc(t));
-            SQB_TRY(flag.alloc(t + 1));
-            SQB_TRY(pos.alloc(t + 1));
-            GD_LAUNCH(gd_ring_expand_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, lvl.p, m, (float)level, cut.ptr.p, cut.idx.p, eptr.p,
-                                                                                      ekeys.p, elvl.p));
-            SQB_TRY(sort_pairs(c, tmp, ekeys.p, skeys.p, elvl.p, slvl.p, t, key_bits(n)));
-            SQB_CUDA(cudaMemsetAsync(flag.p + t, 0, sizeof(int32_t), c->stream));
-            GD_LAUNCH(gd_ring_first_kernel<<<blocks_for(c, t), 256, 0, c->stream>>>(skeys.p, t, flag.p));
-            SQB_TRY(exclusive_scan(c, tmp, flag.p, pos.p, t + 1));
-            int32_t mm = 0;
-            SQB_TRY(read_back(c, &mm, pos.p + t, sizeof(int32_t)));
-            SQB_TRY(keys.alloc(mm));
-            SQB_TRY(lvl.alloc(mm));
-            GD_LAUNCH(gd_ring_compact_kernel<<<blocks_for(c, t), 256, 0, c->stream>>>(skeys.p, slvl.p, flag.p, pos.p, t, keys.p, lvl.p));
-            m = mm;
-        }
-        SQB_TRY(tptr.alloc(n + 1));
-        SQB_TRY(tidx.alloc(m));
-        SQB_TRY(tval.alloc(m));
-        SQB_CUDA(cudaMemsetAsync(tptr.p, 0, (n + 1) * sizeof(int64_t), c->stream));
-        if (m > 0) {
-            GD_LAUNCH(gd_ptr_from_keys_kernel<int64_t><<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, m, n, tptr.p));
-            GD_LAUNCH(gd_split_keys_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, lvl.p, m, tidx.p, tval.p));
-        }
-        return SQB_OK;
-    };
-    const int rc = body();
-    for (auto* b : {&keys, &ekeys, &skeys}) b->release();
-    for (auto* b : {&lvl, &elvl, &slvl}) b->release();
-    ecnt.release(), eptr.release(), flag.release(), pos.release(), tmp.release();
-    return rc;
+    DevBuf<uint64_t> keys(c->stream), ekeys(c->stream), skeys(c->stream);
+    DevBuf<float> lvl(c->stream), elvl(c->stream), slvl(c->stream);
+    DevBuf<int64_t> ecnt(c->stream), eptr(c->stream);
+    DevBuf<int32_t> flag(c->stream), pos(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    int64_t m = cut.nnz;
+    SQB_TRY(keys.alloc(m));
+    SQB_TRY(lvl.alloc(m));
+    GD_LAUNCH(gd_ring_init_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(cut.ptr.p, cut.idx.p, n, keys.p, lvl.p));
+    for (int level = 1; level < n_rings && m > 0; ++level) {
+        SQB_TRY(ecnt.alloc(m + 1));
+        SQB_TRY(eptr.alloc(m + 1));
+        SQB_CUDA(cudaMemsetAsync(ecnt.p + m, 0, sizeof(int64_t), c->stream));
+        GD_LAUNCH(gd_ring_count_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, lvl.p, m, (float)level, cut.ptr.p, ecnt.p));
+        SQB_TRY(exclusive_scan(c, tmp, ecnt.p, eptr.p, m + 1));
+        int64_t e = 0;
+        SQB_TRY(read_back(c, &e, eptr.p + m, sizeof(int64_t)));
+        if (e == 0) break;
+        const int64_t t = m + e;
+        SQB_CHECK(t < INT_MAX, SQB_ERR_UNSUPPORTED, "n_rings=%d: %lld candidate entries exceed 2^31 - 1", n_rings, (long long)t);
+        SQB_TRY(ekeys.alloc(t));
+        SQB_TRY(elvl.alloc(t));
+        SQB_TRY(skeys.alloc(t));
+        SQB_TRY(slvl.alloc(t));
+        SQB_TRY(flag.alloc(t + 1));
+        SQB_TRY(pos.alloc(t + 1));
+        GD_LAUNCH(gd_ring_expand_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, lvl.p, m, (float)level, cut.ptr.p, cut.idx.p, eptr.p,
+                                                                                  ekeys.p, elvl.p));
+        SQB_TRY(sort_pairs(c, tmp, ekeys.p, skeys.p, elvl.p, slvl.p, t, key_bits(n)));
+        SQB_CUDA(cudaMemsetAsync(flag.p + t, 0, sizeof(int32_t), c->stream));
+        GD_LAUNCH(gd_ring_first_kernel<<<blocks_for(c, t), 256, 0, c->stream>>>(skeys.p, t, flag.p));
+        SQB_TRY(exclusive_scan(c, tmp, flag.p, pos.p, t + 1));
+        int32_t mm = 0;
+        SQB_TRY(read_back(c, &mm, pos.p + t, sizeof(int32_t)));
+        SQB_TRY(keys.alloc(mm));
+        SQB_TRY(lvl.alloc(mm));
+        GD_LAUNCH(gd_ring_compact_kernel<<<blocks_for(c, t), 256, 0, c->stream>>>(skeys.p, slvl.p, flag.p, pos.p, t, keys.p, lvl.p));
+        m = mm;
+    }
+    SQB_TRY(tptr.alloc(n + 1));
+    SQB_TRY(tidx.alloc(m));
+    SQB_TRY(tval.alloc(m));
+    SQB_CUDA(cudaMemsetAsync(tptr.p, 0, (n + 1) * sizeof(int64_t), c->stream));
+    if (m > 0) {
+        GD_LAUNCH(gd_ptr_from_keys_kernel<int64_t><<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, m, n, tptr.p));
+        GD_LAUNCH(gd_split_keys_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(keys.p, lvl.p, m, tidx.p, tval.p));
+    }
+    return SQB_OK;
 }
 
 struct PctEnv {
@@ -570,8 +544,9 @@ int pct_get(void* env, int64_t i, double* v) {
     return read_back(e->c, v, e->sorted + (i - e->zeros), sizeof(double));
 }
 
-// One graph (or one library's block) from the rows `rows` (device, or null: all n) of the caller's coordinates.
-int build_block(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64_t n, const Params& P, Csr* adj, Csr* dst) {
+// One graph (or one library's block), before its transform, from the rows `rows` (device, or null: all n) of the caller's
+// coordinates.  Its temporaries are freed when it returns.
+int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64_t n, const Params& P, Csr* adj, Csr* dst) {
     const bool knn = P.kind != GD_RADIUS;
     if (knn) {  // the checks and messages of sqb_knn_2d / sqb_radius_2d, in their order
         SQB_CHECK(n >= 2 && n < 2147483647LL, SQB_ERR_INVALID, "sqb_knn_2d: n=%lld out of range", (long long)n);
@@ -582,158 +557,147 @@ int build_block(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64_t n, co
     } else {
         SQB_CHECK(n >= 1 && n < 2147483647LL, SQB_ERR_INVALID, "sqb_radius_2d: n=%lld out of range", (long long)n);
     }
-    PointGrid g;
-    g.bind(c->stream);
-    DevBuf<double> box, dist, sorted, bval;
-    DevBuf<long long> bad;
-    DevBuf<int32_t> idx;
-    DevBuf<int64_t> bptr, cnt;
-    DevBuf<uint8_t> tmp;
-    Csr cut, cut_dst;
-    DevBuf<int64_t> tptr;
-    DevBuf<int32_t> tidx, colcnt;
-    DevBuf<double> tval;
-    for (auto* b : {&box, &dist, &sorted, &bval, &tval}) b->bind(c->stream);
-    bad.bind(c->stream), idx.bind(c->stream), bptr.bind(c->stream), cnt.bind(c->stream), tmp.bind(c->stream), cut.bind(c->stream);
-    cut_dst.bind(c->stream), tptr.bind(c->stream), tidx.bind(c->stream), colcnt.bind(c->stream);
-    auto body = [&]() -> int {
-        // coordinates: gathered into float64 (n, 2), bounding box and the first non-finite observation in one reduction
-        SQB_TRY(g.d_xy.alloc(2 * n));
-        const unsigned gb = blocks_for(c, n);
-        if (xy.dtype == 0)
-            GD_LAUNCH(gd_gather_kernel<float><<<gb, 256, 0, c->stream>>>((const float*)xy.p, xy.s0, xy.s1, rows, n, g.d_xy.p));
-        else
-            GD_LAUNCH(gd_gather_kernel<double><<<gb, 256, 0, c->stream>>>((const double*)xy.p, xy.s0, xy.s1, rows, n, g.d_xy.p));
-        SQB_TRY(box.alloc(4 * (size_t)gb));
-        SQB_TRY(bad.alloc(gb));
-        GD_LAUNCH(gd_bbox_kernel<<<gb, 256, 0, c->stream>>>(g.d_xy.p, n, box.p, bad.p));
-        std::vector<double> hbox(4 * (size_t)gb);
-        std::vector<long long> hbad(gb);
-        SQB_CUDA(cudaMemcpyAsync(hbox.data(), box.p, hbox.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-        SQB_TRY(read_back(c, hbad.data(), bad.p, hbad.size() * sizeof(long long)));
-        double x0 = INFINITY, y0 = INFINITY, x1 = -INFINITY, y1 = -INFINITY;
-        long long first_bad = LLONG_MAX;
-        for (unsigned b = 0; b < gb; ++b) {
-            x0 = fmin(x0, hbox[4 * b]), y0 = fmin(y0, hbox[4 * b + 1]), x1 = fmax(x1, hbox[4 * b + 2]), y1 = fmax(y1, hbox[4 * b + 3]);
-            first_bad = hbad[b] < first_bad ? hbad[b] : first_bad;
+    PointGrid g(c->stream);
+    DevBuf<double> box(c->stream), dist(c->stream), sorted(c->stream), bval(c->stream);
+    DevBuf<long long> bad(c->stream);
+    DevBuf<int32_t> idx(c->stream);
+    DevBuf<int64_t> bptr(c->stream), cnt(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    // coordinates: gathered into float64 (n, 2), bounding box and the first non-finite observation in one reduction
+    SQB_TRY(g.d_xy.alloc(2 * n));
+    const unsigned gb = blocks_for(c, n);
+    if (xy.dtype == 0)
+        GD_LAUNCH(gd_gather_kernel<float><<<gb, 256, 0, c->stream>>>((const float*)xy.p, xy.s0, xy.s1, rows, n, g.d_xy.p));
+    else
+        GD_LAUNCH(gd_gather_kernel<double><<<gb, 256, 0, c->stream>>>((const double*)xy.p, xy.s0, xy.s1, rows, n, g.d_xy.p));
+    SQB_TRY(box.alloc(4 * (size_t)gb));
+    SQB_TRY(bad.alloc(gb));
+    GD_LAUNCH(gd_bbox_kernel<<<gb, 256, 0, c->stream>>>(g.d_xy.p, n, box.p, bad.p));
+    std::vector<double> hbox(4 * (size_t)gb);
+    std::vector<long long> hbad(gb);
+    SQB_CUDA(cudaMemcpyAsync(hbox.data(), box.p, hbox.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_TRY(read_back(c, hbad.data(), bad.p, hbad.size() * sizeof(long long)));
+    double x0 = INFINITY, y0 = INFINITY, x1 = -INFINITY, y1 = -INFINITY;
+    long long first_bad = LLONG_MAX;
+    for (unsigned b = 0; b < gb; ++b) {
+        x0 = fmin(x0, hbox[4 * b]), y0 = fmin(y0, hbox[4 * b + 1]), x1 = fmax(x1, hbox[4 * b + 2]), y1 = fmax(y1, hbox[4 * b + 3]);
+        first_bad = hbad[b] < first_bad ? hbad[b] : first_bad;
+    }
+    SQB_CHECK(first_bad == LLONG_MAX, SQB_ERR_INVALID, "coordinates of observation %lld are not finite", first_bad);
+    g.gm = knn ? grid_geometry(x0, y0, x1, y1, n, 0.0, knn_pts_per_cell(P.k))
+               : grid_geometry(x0, y0, x1, y1, n, P.radius > 0.0 ? P.radius : 0.0, 2.5);
+    SQB_TRY(grid_bucket(c, n, &g));
+    // the neighbour table as rows of ascending columns: bptr / idx / dist
+    int64_t m;
+    SQB_TRY(bptr.alloc(n + 1));
+    if (knn) {
+        m = n * P.k;
+        SQB_TRY(idx.alloc(m));
+        SQB_TRY(dist.alloc(m));
+        SQB_TRY(knn_launch(c, g, n, P.k, idx.p, dist.p));
+        GD_LAUNCH(gd_knn_ptr_kernel<<<gb, 256, 0, c->stream>>>(bptr.p, n, P.k));
+    } else {
+        SQB_TRY(cnt.alloc(n + 1));
+        SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n + 1) * sizeof(int64_t), c->stream));
+        SQB_TRY(radius_launch(c, g, n, P.radius, cnt.p, nullptr, nullptr, nullptr));
+        SQB_TRY(exclusive_scan(c, tmp, cnt.p, bptr.p, n + 1));
+        SQB_TRY(read_back(c, &m, bptr.p + n, sizeof(int64_t)));
+        SQB_TRY(idx.alloc(m));
+        SQB_TRY(dist.alloc(m));
+        if (m > 0) SQB_TRY(radius_launch(c, g, n, P.radius, nullptr, bptr.p, idx.p, dist.p));
+    }
+    SQB_CHECK(m + n < INT_MAX, SQB_ERR_UNSUPPORTED, "the graph has %lld entries; int32 indices hold at most 2^31 - 1", (long long)(m + n));
+    AsmParams ap{};
+    ap.thr = INFINITY;
+    if (P.kind == GD_GRID) {
+        double med[2] = {0.0, 0.0};
+        SQB_TRY(median_enqueue(c, dist.p, m, sorted, tmp, med));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        ap.cut_on = 1, ap.cut = (med[0] + med[1]) / 2.0 * 1.3;
+        if (P.n_rings == 1) {
+            ap.diag = P.set_diag, ap.diag_adj = 1.0f, ap.dst_mode = DST_ADJ;
+            return assemble(c, bptr.p, idx.p, dist.p, n, ap, false, adj, dst);
         }
-        SQB_CHECK(first_bad == LLONG_MAX, SQB_ERR_INVALID, "coordinates of observation %lld are not finite", first_bad);
-        g.gm = knn ? grid_geometry(x0, y0, x1, y1, n, 0.0, knn_pts_per_cell(P.k))
-                   : grid_geometry(x0, y0, x1, y1, n, P.radius > 0.0 ? P.radius : 0.0, 2.5);
-        SQB_TRY(grid_bucket(c, n, &g));
-        // the neighbour table as rows of ascending columns: bptr / idx / dist
-        int64_t m;
-        SQB_TRY(bptr.alloc(n + 1));
-        if (knn) {
-            m = n * P.k;
-            SQB_TRY(idx.alloc(m));
-            SQB_TRY(dist.alloc(m));
-            SQB_CUDA(knn_launch(c, g, n, P.k, idx.p, dist.p));
-            GD_LAUNCH(gd_knn_ptr_kernel<<<gb, 256, 0, c->stream>>>(bptr.p, n, P.k));
-        } else {
-            SQB_TRY(cnt.alloc(n + 1));
-            SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n + 1) * sizeof(int64_t), c->stream));
-            SQB_CUDA(radius_launch(c, g, n, P.radius, cnt.p, nullptr, nullptr, nullptr));
-            SQB_TRY(exclusive_scan(c, tmp, cnt.p, bptr.p, n + 1));
-            SQB_TRY(read_back(c, &m, bptr.p + n, sizeof(int64_t)));
-            SQB_TRY(idx.alloc(m));
-            SQB_TRY(dist.alloc(m));
-            if (m > 0) SQB_CUDA(radius_launch(c, g, n, P.radius, nullptr, bptr.p, idx.p, dist.p));
-        }
-        SQB_CHECK(m + n < INT_MAX, SQB_ERR_UNSUPPORTED, "the graph has %lld entries; int32 indices hold at most 2^31 - 1", (long long)(m + n));
-        AsmParams ap{};
-        ap.thr = INFINITY;
-        if (P.kind == GD_GRID) {
-            double med[2] = {0.0, 0.0};
-            SQB_CUDA(median_enqueue(c, dist.p, m, sorted, tmp, med));
-            SQB_CUDA(cudaStreamSynchronize(c->stream));
-            ap.cut_on = 1, ap.cut = (med[0] + med[1]) / 2.0 * 1.3;
-            if (P.n_rings > 1) {  // neighbors.py:372-386 on the cut graph; the diagonal follows below
+        // neighbors.py:372-386 on the cut graph; the diagonal follows below.  Each graph is freed once the next is built.
+        DevBuf<int64_t> tptr(c->stream);
+        DevBuf<int32_t> tidx(c->stream);
+        DevBuf<double> tval(c->stream);
+        {
+            Csr cut(c->stream);
+            {
+                Csr cut_dst(c->stream);
                 ap.dst_mode = DST_ADJ;
                 SQB_TRY(assemble(c, bptr.p, idx.p, dist.p, n, ap, false, &cut, &cut_dst));
-                cut_dst.release();
-                SQB_TRY(rings(c, n, cut, P.n_rings, tptr, tidx, tval));
-                cut.release();
-                AsmParams rp{};
-                rp.thr = INFINITY, rp.diag = P.set_diag, rp.diag_adj = 1.0f, rp.dst_mode = DST_VAL;
-                SQB_TRY(assemble(c, tptr.p, tidx.p, tval.p, n, rp, false, adj, dst));
-            } else {
-                ap.diag = P.set_diag, ap.diag_adj = 1.0f, ap.dst_mode = DST_ADJ;
-                SQB_TRY(assemble(c, bptr.p, idx.p, dist.p, n, ap, false, adj, dst));
             }
-        } else {
-            ap.diag = P.set_diag || P.interval || !isnan(P.percentile);  // _Builder._diagonals
-            ap.diag_adj = P.set_diag ? 1.0f : 0.0f;
-            ap.interval = P.interval, ap.lo = P.lo, ap.hi = P.hi, ap.dst_mode = DST_DIST;
-            if (!isnan(P.percentile)) {
-                SQB_TRY(bval.alloc(m));
-                SQB_TRY(sorted.alloc(m));
-                if (m > 0) {
-                    GD_LAUNCH(gd_masked_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(dist.p, m, P.interval, P.lo, P.hi, bval.p));
-                    size_t bytes = 0;
-                    SQB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
-                    SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
-                    SQB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
-                    c->launches += 1;
-                }
-                PctEnv env{c, sorted.p, n};
-                SQB_TRY(percentile_linear(P.percentile, m + n, &ap.thr, pct_get, &env));
-            }
-            SQB_TRY(assemble(c, bptr.p, idx.p, dist.p, n, ap, true, adj, dst));
+            SQB_TRY(rings(c, n, cut, P.n_rings, tptr, tidx, tval));
         }
-        g.release(), idx.release(), dist.release(), bptr.release(), sorted.release(), bval.release(), tptr.release(), tidx.release(), tval.release();
-        if (P.transform == GD_SPECTRAL && adj->nnz > 0) {
-            SQB_TRY(colcnt.alloc(n));
-            SQB_CUDA(cudaMemsetAsync(colcnt.p, 0, n * sizeof(int32_t), c->stream));
-            GD_LAUNCH(gd_colcount_kernel<<<blocks_for(c, adj->nnz), 256, 0, c->stream>>>(adj->idx.p, adj->nnz, colcnt.p));
-            GD_LAUNCH(gd_spectral_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, colcnt.p, adj->vf.p));
-        } else if (P.transform == GD_COSINE) {
-            SQB_TRY(cosine(c, n, adj));
+        AsmParams rp{};
+        rp.thr = INFINITY, rp.diag = P.set_diag, rp.diag_adj = 1.0f, rp.dst_mode = DST_VAL;
+        return assemble(c, tptr.p, tidx.p, tval.p, n, rp, false, adj, dst);
+    }
+    ap.diag = P.set_diag || P.interval || !isnan(P.percentile);  // _Builder._diagonals
+    ap.diag_adj = P.set_diag ? 1.0f : 0.0f;
+    ap.interval = P.interval, ap.lo = P.lo, ap.hi = P.hi, ap.dst_mode = DST_DIST;
+    if (!isnan(P.percentile)) {
+        SQB_TRY(bval.alloc(m));
+        SQB_TRY(sorted.alloc(m));
+        if (m > 0) {
+            GD_LAUNCH(gd_masked_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(dist.p, m, P.interval, P.lo, P.hi, bval.p));
+            size_t bytes = 0;
+            SQB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
+            SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
+            SQB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
+            c->launches += 1;
         }
-        return SQB_OK;
-    };
-    const int rc = body();
-    g.release();
-    for (auto* b : {&box, &dist, &sorted, &bval, &tval}) b->release();
-    bad.release(), idx.release(), bptr.release(), cnt.release(), tmp.release(), cut.release(), cut_dst.release(), tptr.release(), tidx.release();
-    colcnt.release();
-    return rc;
+        PctEnv env{c, sorted.p, n};
+        SQB_TRY(percentile_linear(P.percentile, m + n, &ap.thr, pct_get, &env));
+    }
+    return assemble(c, bptr.p, idx.p, dist.p, n, ap, true, adj, dst);
+}
+
+// One graph (or one library's block) with its transform
+int build_block(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64_t n, const Params& P, Csr* adj, Csr* dst) {
+    SQB_TRY(build_untransformed(c, xy, rows, n, P, adj, dst));
+    if (P.transform == GD_SPECTRAL && adj->nnz > 0) {
+        DevBuf<int32_t> colcnt(c->stream);
+        SQB_TRY(colcnt.alloc(n));
+        SQB_CUDA(cudaMemsetAsync(colcnt.p, 0, n * sizeof(int32_t), c->stream));
+        GD_LAUNCH(gd_colcount_kernel<<<blocks_for(c, adj->nnz), 256, 0, c->stream>>>(adj->idx.p, adj->nnz, colcnt.p));
+        GD_LAUNCH(gd_spectral_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, colcnt.p, adj->vf.p));
+    } else if (P.transform == GD_COSINE) {
+        SQB_TRY(cosine(c, n, adj));
+    }
+    return SQB_OK;
 }
 
 // the library blocks as one matrix of n_out rows
 int combine(sqb_ctx* c, int64_t n_out, const std::vector<Csr>& blocks, const std::vector<DevBuf<int32_t>>& grow, const std::vector<int64_t>& nb,
             Csr* out) {
-    DevBuf<int32_t> cnt;
-    DevBuf<uint8_t> tmp;
-    cnt.bind(c->stream), tmp.bind(c->stream);
-    auto body = [&]() -> int {
-        SQB_TRY(cnt.alloc(n_out + 1));
-        SQB_TRY(out->ptr.alloc(n_out + 1));
-        SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_out + 1) * sizeof(int32_t), c->stream));
-        int64_t total = 0;
-        for (size_t b = 0; b < blocks.size(); ++b) {
-            total += blocks[b].nnz;
-            GD_LAUNCH(gd_block_count_kernel<<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(blocks[b].ptr.p, grow[b].p, nb[b], cnt.p));
-        }
-        SQB_CHECK(total < INT_MAX, SQB_ERR_UNSUPPORTED, "the graph has %lld entries; int32 indices hold at most 2^31 - 1", (long long)total);
-        SQB_TRY(exclusive_scan(c, tmp, cnt.p, out->ptr.p, n_out + 1));
-        out->nnz = total, out->f64 = !blocks.empty() && blocks[0].f64;
-        SQB_TRY(out->idx.alloc(total));
-        SQB_TRY(out->f64 ? out->vd.alloc(total) : out->vf.alloc(total));
-        for (size_t b = 0; b < blocks.size(); ++b) {
-            const Csr& k = blocks[b];
-            if (out->f64)
-                GD_LAUNCH(gd_block_fill_kernel<double><<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(k.ptr.p, k.idx.p, k.vd.p, grow[b].p, nb[b], out->ptr.p,
-                                                                                                   out->idx.p, out->vd.p));
-            else
-                GD_LAUNCH(gd_block_fill_kernel<float><<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(k.ptr.p, k.idx.p, k.vf.p, grow[b].p, nb[b], out->ptr.p,
-                                                                                                  out->idx.p, out->vf.p));
-        }
-        return SQB_OK;
-    };
-    const int rc = body();
-    cnt.release(), tmp.release();
-    return rc;
+    DevBuf<int32_t> cnt(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(cnt.alloc(n_out + 1));
+    SQB_TRY(out->ptr.alloc(n_out + 1));
+    SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_out + 1) * sizeof(int32_t), c->stream));
+    int64_t total = 0;
+    for (size_t b = 0; b < blocks.size(); ++b) {
+        total += blocks[b].nnz;
+        GD_LAUNCH(gd_block_count_kernel<<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(blocks[b].ptr.p, grow[b].p, nb[b], cnt.p));
+    }
+    SQB_CHECK(total < INT_MAX, SQB_ERR_UNSUPPORTED, "the graph has %lld entries; int32 indices hold at most 2^31 - 1", (long long)total);
+    SQB_TRY(exclusive_scan(c, tmp, cnt.p, out->ptr.p, n_out + 1));
+    out->nnz = total, out->f64 = !blocks.empty() && blocks[0].f64;
+    SQB_TRY(out->idx.alloc(total));
+    SQB_TRY(out->f64 ? out->vd.alloc(total) : out->vf.alloc(total));
+    for (size_t b = 0; b < blocks.size(); ++b) {
+        const Csr& k = blocks[b];
+        if (out->f64)
+            GD_LAUNCH(gd_block_fill_kernel<double><<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(k.ptr.p, k.idx.p, k.vd.p, grow[b].p, nb[b], out->ptr.p,
+                                                                                               out->idx.p, out->vd.p));
+        else
+            GD_LAUNCH(gd_block_fill_kernel<float><<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(k.ptr.p, k.idx.p, k.vf.p, grow[b].p, nb[b], out->ptr.p,
+                                                                                              out->idx.p, out->vf.p));
+    }
+    return SQB_OK;
 }
 
 }  // namespace
@@ -779,21 +743,17 @@ int sqb_graph_build_device(sqb_ctx* c, const void* xy, int xy_dtype, int64_t n, 
     SQB_CUDA(cudaSetDevice(c->device));
     SQB_TRY(sqb_wait_producer(c, producer_stream));
     const Coords co{xy, xy_dtype, stride_row, stride_col};
-    sqb_graph* g = new sqb_graph();
-    g->c = c;
-    g->adj.bind(c->stream), g->dst.bind(c->stream);
-    std::vector<Csr> ba, bd;
-    std::vector<DevBuf<int32_t>> rows, grow;
-    std::vector<int64_t> nb;
-    auto body = [&]() -> int {
-        if (n_libs == 0) {
-            g->n = n;
-            return build_block(c, co, nullptr, n, P, &g->adj, &g->dst);
-        }
+    std::unique_ptr<sqb_graph> g(new sqb_graph(c));
+    if (n_libs == 0) {
+        g->n = n;
+        SQB_TRY(build_block(c, co, nullptr, n, P, &g->adj, &g->dst));
+    } else {
         g->n = lib_ptr[n_libs];
-        ba.resize(n_libs), bd.resize(n_libs), rows.resize(n_libs), grow.resize(n_libs), nb.resize(n_libs);
+        std::vector<Csr> ba, bd;
+        std::vector<DevBuf<int32_t>> rows, grow;
+        std::vector<int64_t> nb(n_libs);
         for (int b = 0; b < n_libs; ++b) {
-            ba[b].bind(c->stream), bd[b].bind(c->stream), rows[b].bind(c->stream), grow[b].bind(c->stream);
+            ba.emplace_back(c->stream), bd.emplace_back(c->stream), rows.emplace_back(c->stream), grow.emplace_back(c->stream);
             nb[b] = lib_ptr[b + 1] - lib_ptr[b];
             std::vector<int32_t> gr(nb[b] > 0 ? nb[b] : 1);
             for (int64_t r = 0; r < nb[b]; ++r) gr[r] = rank[lib_rows[lib_ptr[b] + r]];
@@ -805,23 +765,11 @@ int sqb_graph_build_device(sqb_ctx* c, const void* xy, int xy_dtype, int64_t n, 
             SQB_TRY(build_block(c, co, rows[b].p, nb[b], P, &ba[b], &bd[b]));
         }
         SQB_TRY(combine(c, g->n, ba, grow, nb, &g->adj));
-        return combine(c, g->n, bd, grow, nb, &g->dst);
-    };
-    int rc = body();
-    for (auto& b : ba) b.release();
-    for (auto& b : bd) b.release();
-    for (auto& b : rows) b.release();
-    for (auto& b : grow) b.release();
-    if (rc == SQB_OK) {
-        const cudaError_t e = cudaStreamSynchronize(c->stream);  // surfaces an asynchronous fault of the build here
-        if (e != cudaSuccess) sqb_set_error("%s: %s", where, cudaGetErrorString(e)), rc = SQB_ERR_CUDA;
+        SQB_TRY(combine(c, g->n, bd, grow, nb, &g->dst));
     }
-    if (rc != SQB_OK) {
-        g->adj.release(), g->dst.release();
-        delete g;
-        return rc;
-    }
-    *out = g, *n_out = g->n, *adj_nnz = g->adj.nnz, *dst_nnz = g->dst.nnz, *dst_f64 = g->dst.f64 ? 1 : 0;
+    SQB_CUDA(cudaStreamSynchronize(c->stream));  // surfaces an asynchronous fault of the build here
+    *n_out = g->n, *adj_nnz = g->adj.nnz, *dst_nnz = g->dst.nnz, *dst_f64 = g->dst.f64 ? 1 : 0;
+    *out = g.release();
     return SQB_OK;
 }
 
@@ -851,7 +799,6 @@ int sqb_graph_export(sqb_graph* g, int32_t* adj_indptr, int32_t* adj_indices, fl
 int sqb_graph_free(sqb_graph* g) {
     if (!g) return SQB_OK;
     SQB_CUDA(cudaSetDevice(g->c->device));
-    g->adj.release(), g->dst.release();
     delete g;
     return SQB_OK;
 }

@@ -129,34 +129,21 @@ extern "C" int sqb_interaction_matrix(sqb_ctx* c, int64_t n, int64_t nnz, const 
     SQB_CUDA(cudaSetDevice(c->device));
     const int CC = n_cls * n_cls;
     const size_t vsize = weighted ? (data_dtype == 0 ? 4 : 8) : 0;
-    DevBuf<uint32_t> d_ptr, d_idx;
-    DevBuf<uint8_t> d_val;
-    DevBuf<int32_t> d_codes;
-    DevBuf<unsigned long long> d_out;  // 8 bytes per bin: double or uint64
-    d_ptr.bind(c->stream);
-    d_idx.bind(c->stream);
-    d_val.bind(c->stream);
-    d_codes.bind(c->stream);
-    d_out.bind(c->stream);
-    auto cleanup = [&]() {
-        d_ptr.release();
-        d_idx.release();
-        d_val.release();
-        d_codes.release();
-        d_out.release();
-    };
-    int rc;
-    if ((rc = d_ptr.alloc(n + 1)) || (rc = d_idx.alloc(nnz > 0 ? nnz : 1)) || (rc = d_val.alloc(weighted && nnz > 0 ? nnz * vsize : 1)) ||
-        (rc = d_codes.alloc(n)) || (rc = d_out.alloc(CC))) {
-        cleanup();
-        return rc;
-    }
-    cudaError_t e = cudaMemcpyAsync(d_ptr.p, indptr, (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess && nnz > 0 && sqb_h2d(c, d_idx.p, indices, nnz * sizeof(uint32_t)) != SQB_OK) e = cudaErrorUnknown;
-    if (e == cudaSuccess && weighted && nnz > 0 && sqb_h2d(c, d_val.p, data, nnz * vsize) != SQB_OK) e = cudaErrorUnknown;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_codes.p, codes, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_out.p, 0, (size_t)CC * 8, c->stream);
-    if (e == cudaSuccess) {
+    DevBuf<uint32_t> d_ptr(c->stream), d_idx(c->stream);
+    DevBuf<uint8_t> d_val(c->stream);
+    DevBuf<int32_t> d_codes(c->stream);
+    DevBuf<unsigned long long> d_out(c->stream);  // 8 bytes per bin: double or uint64
+    SQB_TRY(d_ptr.alloc(n + 1));
+    SQB_TRY(d_idx.alloc(nnz > 0 ? nnz : 1));
+    SQB_TRY(d_val.alloc(weighted && nnz > 0 ? nnz * vsize : 1));
+    SQB_TRY(d_codes.alloc(n));
+    SQB_TRY(d_out.alloc(CC));
+    SQB_CUDA(cudaMemcpyAsync(d_ptr.p, indptr, (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    if (nnz > 0) SQB_TRY(sqb_h2d(c, d_idx.p, indices, nnz * sizeof(uint32_t)));
+    if (weighted && nnz > 0) SQB_TRY(sqb_h2d(c, d_val.p, data, nnz * vsize));
+    SQB_CUDA(cudaMemcpyAsync(d_codes.p, codes, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemsetAsync(d_out.p, 0, (size_t)CC * 8, c->stream));
+    {
         const InterLaunch L(c, n, n_cls);
         SqbLaunchScope scope(c, SQB_K_MISC);
         double* ow = reinterpret_cast<double*>(d_out.p);
@@ -166,16 +153,10 @@ extern "C" int sqb_interaction_matrix(sqb_ctx* c, int64_t n, int64_t nnz, const 
             interaction_kernel<uint32_t, uint32_t, float, true><<<L.blocks, 256, L.smem, c->stream>>>(d_ptr.p, d_idx.p, reinterpret_cast<const float*>(d_val.p), d_codes.p, n, n_cls, L.use_smem, ow, d_out.p, nullptr);
         else
             interaction_kernel<uint32_t, uint32_t, double, true><<<L.blocks, 256, L.smem, c->stream>>>(d_ptr.p, d_idx.p, reinterpret_cast<const double*>(d_val.p), d_codes.p, n, n_cls, L.use_smem, ow, d_out.p, nullptr);
-        e = cudaGetLastError();
+        SQB_POST_LAUNCH();
     }
-    if (e == cudaSuccess)
-        e = cudaMemcpyAsync(weighted ? (void*)out_weighted : (void*)out_counts, d_out.p, (size_t)CC * 8, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_interaction_matrix: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cudaMemcpyAsync(weighted ? (void*)out_weighted : (void*)out_counts, d_out.p, (size_t)CC * 8, cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 
@@ -235,10 +216,9 @@ extern "C" int sqb_interaction_matrix_device(sqb_ctx* c, int64_t n, int64_t nnz,
     SQB_CUDA(cudaSetDevice(c->device));
     SQB_TRY(sqb_wait_producer(c, producer_stream));
     const int CC = n_cls * n_cls;
-    DevBuf<int32_t> d_codes;
-    DevBuf<unsigned long long> d_out;  // 8 bytes per bin: double or uint64
-    DevBuf<unsigned> d_err;
-    d_codes.bind(c->stream), d_out.bind(c->stream), d_err.bind(c->stream);
+    DevBuf<int32_t> d_codes(c->stream);
+    DevBuf<unsigned long long> d_out(c->stream);  // 8 bytes per bin: double or uint64
+    DevBuf<unsigned> d_err(c->stream);
     unsigned flag = 0;
     auto body = [&]() -> int {
         SQB_TRY(d_codes.alloc(n));
@@ -263,7 +243,6 @@ extern "C" int sqb_interaction_matrix_device(sqb_ctx* c, int64_t n, int64_t nnz,
         return SQB_OK;
     };
     const int rc = body();
-    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);
-    d_codes.release(), d_out.release(), d_err.release();
+    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);  // the caller's buffers are no longer read
     return rc;
 }

@@ -2319,15 +2319,18 @@ __global__ void nhood_count_global_kernel(const uint32_t* __restrict__ indptr, c
 // ================================================================================================
 // host side
 // ================================================================================================
+// Every buffer of a handle is allocated, used and freed in ctx->stream order; the buffers' initialisers read ctx, which is
+// declared first.
 struct sqb_nhood {
-    sqb_ctx* ctx = nullptr;
+    explicit sqb_nhood(sqb_ctx* c) : ctx(c) {}
+    sqb_ctx* ctx;
     int64_t n = 0, nnz = 0, stride = 0;
     int n_cls = 0;
     int lt_bytes = 1;  // 1: uint8 labels (n_cls <= 256), 2: uint16
-    DevBuf<uint32_t> d_indptr, d_indices;
-    DevBuf<uint32_t> d_uptr, d_uidx;  // entries with j >= i of a symmetric graph (see 3b): only while the pair list is built
-    DevBuf<uint4> d_recs;              // row records (3c) of those entries (symmetric graph) or of all entries: what the count kernel walks
-    DevBuf<uint32_t> d_selfnodes;      // nodes with a stored self loop (usually none)
+    DevBuf<uint32_t> d_indptr{ctx->stream}, d_indices{ctx->stream};
+    DevBuf<uint32_t> d_uptr{ctx->stream}, d_uidx{ctx->stream};  // entries with j >= i of a symmetric graph (see 3b): only while the pair list is built
+    DevBuf<uint4> d_recs{ctx->stream};          // row records (3c) of those entries (symmetric graph) or of all entries: what the count kernel walks
+    DevBuf<uint32_t> d_selfnodes{ctx->stream};  // nodes with a stored self loop (usually none)
     int64_t n_recs = 0;
     uint32_t n_self = 0;
     bool sym = false;
@@ -2335,27 +2338,27 @@ struct sqb_nhood {
     int jgen_threads = 128;  // generator threads per block of the swap-target generation kernel (32 / 64 / 128: 1 / 2 / 4
                              // permutations per block; the partitioned variant adds one partition warp per generator warp)
     int count_un = 4;    // records (of three entries) a warp takes per pass in the count kernel (1 / 2 / 3 / 4)
-    DevBuf<uint8_t> d_base;   // stride * lt_bytes, library-grouped order
-    DevBuf<uint32_t> d_order;  // grouped position -> node id (only with libraries)
+    DevBuf<uint8_t> d_base{ctx->stream};    // stride * lt_bytes, library-grouped order
+    DevBuf<uint32_t> d_order{ctx->stream};  // grouped position -> node id (only with libraries)
     bool has_order = false;
-    DevBuf<int64_t> d_seg_start, d_seg_len;
+    DevBuf<int64_t> d_seg_start{ctx->stream}, d_seg_len{ctx->stream};
     int nseg = 0;
     bool base_set = false;
-    DevBuf<uint64_t> d_states;  // P x 4
+    DevBuf<uint64_t> d_states{ctx->stream};  // P x 4
     int64_t n_perms = 0;
     bool uploaded = false, ran = false;
     int64_t chunk = 0;      // permutations resident at once, fixed by the upload that sized the scratch buffers
     int rng_mode = 0;       // 0: exact numpy PCG64 replay, 1: keyed-bijection ("philox") fast mode
     uint64_t philox_seed = 0;
     int64_t perm_first = 0;  // global index of permutation 0 of this handle (multi-GPU shards keep their global indices)
-    DevBuf<uint32_t> d_cum;  // [nseg][n_cls + 1] class offsets of every segment's sorted labels (fast mode)
-    DevBuf<uint32_t> d_bkt;  // per segment: class at the first value of every bucket (fast mode class lookup)
+    DevBuf<uint32_t> d_cum{ctx->stream};  // [nseg][n_cls + 1] class offsets of every segment's sorted labels (fast mode)
+    DevBuf<uint32_t> d_bkt{ctx->stream};  // per segment: class at the first value of every bucket (fast mode class lookup)
     std::vector<int64_t> h_seg_start, h_seg_len, h_bkt_off;
     bool philox_ready = false;
     std::vector<PhiloxSeg> h_pseg;
     // label matrices [chunk][stride] and [PB/64][n + 1][64] live in ctx->scratch[0..1]
-    DevBuf<uint32_t> d_counts;  // [P][C*C]
-    DevBuf<uint32_t> d_tmp_u32;
+    DevBuf<uint32_t> d_counts{ctx->stream};  // [P][C*C]
+    DevBuf<uint32_t> d_tmp_u32{ctx->stream};
     std::vector<uint32_t> h_order;
     // options
     int shuffle_algo = -1;  // -1 auto (see launch_shuffle and part_replay_shape); 1 CTA per permutation; 2 warp per
@@ -2865,11 +2868,10 @@ static int philox_prepare(sqb_nhood* h) {
     const int64_t C1h = (int64_t)h->n_cls + 1;
     std::vector<uint32_t> hcnt((size_t)h->nseg * C1h, 0u);
     {
-        DevBuf<uint32_t> d_hist;
-        d_hist.bind(c->stream);
+        DevBuf<uint32_t> d_hist(c->stream);
         SQB_TRY(d_hist.alloc(hcnt.size()));
-        cudaError_t e = cudaMemsetAsync(d_hist.p, 0, hcnt.size() * sizeof(uint32_t), c->stream);
-        for (int sgm = 0; sgm < h->nseg && e == cudaSuccess; ++sgm) {
+        SQB_CUDA(cudaMemsetAsync(d_hist.p, 0, hcnt.size() * sizeof(uint32_t), c->stream));
+        for (int sgm = 0; sgm < h->nseg; ++sgm) {
             const int64_t m = seg_len[sgm];
             if (m <= 0) continue;
             const unsigned g = (unsigned)(m < 256 * 296 ? ceil_div64(m, 256) : 296);
@@ -2879,15 +2881,10 @@ static int philox_prepare(sqb_nhood* h) {
             else
                 nhood_class_hist_kernel<uint16_t><<<g, 256, sm, c->stream>>>(reinterpret_cast<const uint16_t*>(h->d_base.p), seg_start[sgm], m,
                                                                               h->n_cls, d_hist.p + (size_t)sgm * C1h + 1);
-            e = cudaGetLastError();
+            SQB_POST_LAUNCH();
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(hcnt.data(), d_hist.p, hcnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        d_hist.release();
-        if (e != cudaSuccess) {
-            sqb_set_error("fast RNG mode: class histogram failed: %s", cudaGetErrorString(e));
-            return SQB_ERR_CUDA;
-        }
+        SQB_CUDA(cudaMemcpyAsync(hcnt.data(), d_hist.p, hcnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
     }
     {  // fast RNG mode: per segment the class offsets of its labels sorted by class, the Feistel radices and a bucket table
        // (class at the first value of every bucket of 2^shift values) that shortens the class search to `steps` bisections
@@ -2954,30 +2951,14 @@ static int nhood_count_batched_path(sqb_nhood* h, const uint32_t* labels, uint32
         SQB_CHECK(labels[i] < (uint32_t)h->n_cls, SQB_ERR_INVALID, "sqb_nhood_count: labels[%lld]=%u >= n_cls=%d",
                   (long long)i, labels[i], h->n_cls);
     const int64_t CC = (int64_t)h->n_cls * h->n_cls;
-    DevBuf<uint8_t> labT;
-    DevBuf<uint32_t> cnt;
-    labT.bind(c->stream);
-    cnt.bind(c->stream);
-    int rc = SQB_OK;
-    if ((rc = h->d_tmp_u32.alloc(h->n)) != SQB_OK) return rc;
-    if ((rc = labT.alloc((size_t)(h->n + 1) * 64 * h->lt_bytes)) != SQB_OK) return rc;  // one group of the label matrix
-    if ((rc = cnt.alloc(CC)) != SQB_OK) {
-        labT.release();
-        return rc;
-    }
-    auto cleanup = [&]() {
-        labT.release();
-        cnt.release();
-    };
-    cudaError_t e;
-    e = cudaMemcpyAsync(h->d_tmp_u32.p, labels, h->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(labT.p, 0, (size_t)(h->n + 1) * 64 * h->lt_bytes, c->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(cnt.p, 0, CC * sizeof(uint32_t), c->stream);
-    if (e != cudaSuccess) {
-        cleanup();
-        sqb_set_error("sqb_nhood_count: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    DevBuf<uint8_t> labT(c->stream);
+    DevBuf<uint32_t> cnt(c->stream);
+    SQB_TRY(h->d_tmp_u32.alloc(h->n));
+    SQB_TRY(labT.alloc((size_t)(h->n + 1) * 64 * h->lt_bytes));  // one group of the label matrix
+    SQB_TRY(cnt.alloc(CC));
+    SQB_CUDA(cudaMemcpyAsync(h->d_tmp_u32.p, labels, h->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemsetAsync(labT.p, 0, (size_t)(h->n + 1) * 64 * h->lt_bytes, c->stream));
+    SQB_CUDA(cudaMemsetAsync(cnt.p, 0, CC * sizeof(uint32_t), c->stream));
     {
         SqbLaunchScope scope(c, SQB_K_MISC);
         unsigned g = (unsigned)ceil_div64(h->n, 256);
@@ -2986,18 +2967,11 @@ static int nhood_count_batched_path(sqb_nhood* h, const uint32_t* labels, uint32
         else
             nhood_single_to_T_kernel<uint16_t><<<g, 256, 0, c->stream>>>(h->d_tmp_u32.p, reinterpret_cast<uint16_t*>(labT.p), h->n);
     }
-    rc = (h->lt_bytes == 1) ? launch_count<uint8_t>(h, labT.p, 64, 1, cnt.p)
-                            : launch_count<uint16_t>(h, reinterpret_cast<uint16_t*>(labT.p), 64, 1, cnt.p);
-    if (rc == SQB_OK) {
-        e = cudaMemcpyAsync(out, cnt.p, CC * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) {
-            sqb_set_error("sqb_nhood_count: %s", cudaGetErrorString(e));
-            rc = SQB_ERR_CUDA;
-        }
-    }
-    cleanup();
-    return rc;
+    SQB_TRY((h->lt_bytes == 1) ? launch_count<uint8_t>(h, labT.p, 64, 1, cnt.p)
+                               : launch_count<uint16_t>(h, reinterpret_cast<uint16_t*>(labT.p), 64, 1, cnt.p));
+    SQB_CUDA(cudaMemcpyAsync(out, cnt.p, CC * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    return SQB_OK;
 }
 
 
@@ -3011,35 +2985,26 @@ static int ensure_buffers(sqb_nhood* h, int64_t chunk) {
 static int nhood_build_records(sqb_nhood* h, const uint32_t* ptr, const uint32_t* idx, uint32_t* n_self_out) {
     sqb_ctx* ctx = h->ctx;
     const int64_t n = h->n;
-    DevBuf<uint32_t> cnt, rptr, cnt_self;
-    DevBuf<uint8_t> tmp;
-    cnt.bind(ctx->stream), rptr.bind(ctx->stream), cnt_self.bind(ctx->stream), tmp.bind(ctx->stream);
-    auto cleanup = [&]() { cnt.release(), rptr.release(), cnt_self.release(), tmp.release(); };
-    int rc;
+    DevBuf<uint32_t> cnt(ctx->stream), rptr(ctx->stream), cnt_self(ctx->stream);
+    DevBuf<uint8_t> tmp(ctx->stream);
     size_t tmp_bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(n + 1), ctx->stream);
-    if ((rc = cnt.alloc(n + 1)) != SQB_OK || (rc = rptr.alloc(n + 1)) != SQB_OK || (rc = cnt_self.alloc(1)) != SQB_OK ||
-        (rc = tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1)) != SQB_OK) {
-        cleanup();
-        return rc;
-    }
+    SQB_TRY(cnt.alloc(n + 1));
+    SQB_TRY(rptr.alloc(n + 1));
+    SQB_TRY(cnt_self.alloc(1));
+    SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
     nhood_rec_count_kernel<<<(unsigned)ceil_div64(n + 1, 256), 256, 0, ctx->stream>>>(ptr, n, cnt.p);
     cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, cnt.p, rptr.p, (int)(n + 1), ctx->stream);
     uint32_t total = 0, h_self = 0;
     cudaMemcpyAsync(&total, rptr.p + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess && total > 0 && (rc = h->d_recs.alloc(total)) == SQB_OK) {
+    SQB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (total > 0) {
+        SQB_TRY(h->d_recs.alloc(total));
         cudaMemsetAsync(cnt_self.p, 0, sizeof(uint32_t), ctx->stream);
         nhood_rec_fill_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, ctx->stream>>>(ptr, idx, n, rptr.p, h->d_recs.p, cnt_self.p);
         cudaMemcpyAsync(&h_self, cnt_self.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-        e = cudaStreamSynchronize(ctx->stream);
+        SQB_CUDA(cudaStreamSynchronize(ctx->stream));
     }
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_nhood_create: building the row records failed: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
-    if (rc != SQB_OK) return rc;
     h->n_recs = total;
     *n_self_out = h_self;
     return SQB_OK;
@@ -3055,111 +3020,66 @@ static int nhood_check_args(const char* where, sqb_ctx* ctx, int64_t n, int64_t 
     return SQB_OK;
 }
 
-// A handle whose buffers live in ctx->stream order, with the uint32 CSR (d_indptr, d_indices) allocated but not filled.
-static int nhood_new(sqb_ctx* ctx, int64_t n, int64_t nnz, int n_cls, sqb_nhood** out) {
-    sqb_nhood* h = new sqb_nhood();
-    h->ctx = ctx;
-    // all handle buffers are allocated, used and freed in ctx->stream order
-    h->d_indptr.bind(ctx->stream);
-    h->d_indices.bind(ctx->stream);
-    h->d_uptr.bind(ctx->stream);
-    h->d_uidx.bind(ctx->stream);
-    h->d_recs.bind(ctx->stream);
-    h->d_selfnodes.bind(ctx->stream);
-    h->d_base.bind(ctx->stream);
-    h->d_order.bind(ctx->stream);
-    h->d_seg_start.bind(ctx->stream);
-    h->d_seg_len.bind(ctx->stream);
-    h->d_states.bind(ctx->stream);
-    h->d_counts.bind(ctx->stream);
-    h->d_tmp_u32.bind(ctx->stream);
-    h->d_cum.bind(ctx->stream);
-    h->d_bkt.bind(ctx->stream);
+// A handle with the uint32 CSR (d_indptr, d_indices) allocated but not filled.
+static int nhood_new(sqb_ctx* ctx, int64_t n, int64_t nnz, int n_cls, std::unique_ptr<sqb_nhood>& h) {
+    h.reset(new sqb_nhood(ctx));
     h->n = n;
     h->nnz = nnz;
     h->n_cls = n_cls;
     h->lt_bytes = n_cls <= 256 ? 1 : 2;
     h->stride = ((n + 15) / 16) * 16;
-    int rc;
-    if ((rc = h->d_indptr.alloc(n + 1)) != SQB_OK || (rc = h->d_indices.alloc(nnz > 0 ? nnz : 1)) != SQB_OK) {
-        sqb_nhood_destroy(h);
-        return rc;
-    }
-    *out = h;
+    SQB_TRY(h->d_indptr.alloc(n + 1));
+    SQB_TRY(h->d_indices.alloc(nnz > 0 ? nnz : 1));
     return SQB_OK;
 }
 
 // The graph in h->d_indptr / d_indices (indptr[0] = 0 and indptr[n] = nnz already checked) -> symmetric check, upper CSR
-// and row records.  Destroys h on failure.
+// and row records.
 static int nhood_prepare(sqb_nhood* h, const char* where) {
     sqb_ctx* ctx = h->ctx;
     const int64_t n = h->n, nnz = h->nnz;
     const int n_cls = h->n_cls;
-    int rc = SQB_OK;
     // symmetric structure? then keep the entries with j >= i as a second CSR (3b)
     if (nnz > 0) {
-        DevBuf<uint32_t> flag, ucnt;
-        DevBuf<uint8_t> tmp;
-        flag.bind(ctx->stream);
-        ucnt.bind(ctx->stream);
-        tmp.bind(ctx->stream);
-        uint32_t hflag = 1;
-        auto cleanup = [&]() {
-            flag.release();
-            ucnt.release();
-            tmp.release();
-        };
-        rc = flag.alloc(1);
-        if (rc == SQB_OK) rc = ucnt.alloc(n + 1);
-        if (rc == SQB_OK) rc = h->d_uptr.alloc(n + 1);
-        size_t tmp_bytes = 0;
-        if (rc == SQB_OK) {
+        {
+            DevBuf<uint32_t> flag(ctx->stream), ucnt(ctx->stream);
+            DevBuf<uint8_t> tmp(ctx->stream);
+            uint32_t hflag = 1;
+            SQB_TRY(flag.alloc(1));
+            SQB_TRY(ucnt.alloc(n + 1));
+            SQB_TRY(h->d_uptr.alloc(n + 1));
+            size_t tmp_bytes = 0;
             cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, ucnt.p, h->d_uptr.p, (int)(n + 1), ctx->stream);
-            rc = tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1);
-        }
-        if (rc != SQB_OK) {
-            cleanup();
-            sqb_nhood_destroy(h);
-            return rc;
-        }
-        cudaMemsetAsync(flag.p, 0, sizeof(uint32_t), ctx->stream);
-        nhood_symcheck_kernel<<<(unsigned)ceil_div64(n + 1, 256), 256, 0, ctx->stream>>>(h->d_indptr.p, h->d_indices.p, n, flag.p, ucnt.p);
-        cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, ucnt.p, h->d_uptr.p, (int)(n + 1), ctx->stream);
-        cudaMemcpyAsync(&hflag, flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-        cudaError_t e = cudaStreamSynchronize(ctx->stream);
-        if (e == cudaSuccess && (hflag & 2u)) {  // the kernels index the label arrays with these values: refuse
-            cleanup();
-            sqb_nhood_destroy(h);
-            sqb_set_error("%s: invalid CSR (column index outside [0, %lld) or indptr not monotone)", where, (long long)n);
-            return SQB_ERR_INVALID;
-        }
-        if (e == cudaSuccess && hflag == 0) {
-            uint32_t total = 0;
-            cudaMemcpyAsync(&total, h->d_uptr.p + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-            e = cudaStreamSynchronize(ctx->stream);
-            if (e == cudaSuccess && (rc = h->d_uidx.alloc(total > 0 ? total : 1)) == SQB_OK) {
-                nhood_upper_fill_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, ctx->stream>>>(h->d_indptr.p, h->d_indices.p, n,
-                                                                                              h->d_uptr.p, h->d_uidx.p);
+            SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
+            cudaMemsetAsync(flag.p, 0, sizeof(uint32_t), ctx->stream);
+            nhood_symcheck_kernel<<<(unsigned)ceil_div64(n + 1, 256), 256, 0, ctx->stream>>>(h->d_indptr.p, h->d_indices.p, n, flag.p, ucnt.p);
+            cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, ucnt.p, h->d_uptr.p, (int)(n + 1), ctx->stream);
+            cudaMemcpyAsync(&hflag, flag.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
+            SQB_CUDA(cudaStreamSynchronize(ctx->stream));
+            // the kernels index the label arrays with these values: refuse
+            SQB_CHECK(!(hflag & 2u), SQB_ERR_INVALID, "%s: invalid CSR (column index outside [0, %lld) or indptr not monotone)", where,
+                      (long long)n);
+            if (hflag == 0) {
+                uint32_t total = 0;
+                cudaMemcpyAsync(&total, h->d_uptr.p + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
+                SQB_CUDA(cudaStreamSynchronize(ctx->stream));
+                SQB_TRY(h->d_uidx.alloc(total > 0 ? total : 1));
+                nhood_upper_fill_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, ctx->stream>>>(h->d_indptr.p, h->d_indices.p, n, h->d_uptr.p,
+                                                                                              h->d_uidx.p);
                 // the same entries as row records (3c) + the nodes with a self loop
                 uint32_t h_self = 0;
-                e = cudaStreamSynchronize(ctx->stream);
-                if (e == cudaSuccess && (rc = nhood_build_records(h, h->d_uptr.p, h->d_uidx.p, &h_self)) == SQB_OK) {
-                    if (h_self > 0 && (rc = h->d_selfnodes.alloc(h_self)) == SQB_OK) {
-                        cudaMemsetAsync(flag.p, 0, sizeof(uint32_t), ctx->stream);
-                        nhood_self_fill_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, ctx->stream>>>(h->d_uptr.p, h->d_uidx.p, n,
-                                                                                                     h->d_selfnodes.p, flag.p);
-                        e = cudaStreamSynchronize(ctx->stream);
-                    }
-                    h->n_self = h_self;
-                    h->sym = (e == cudaSuccess && rc == SQB_OK);
+                SQB_CUDA(cudaStreamSynchronize(ctx->stream));
+                SQB_TRY(nhood_build_records(h, h->d_uptr.p, h->d_uidx.p, &h_self));
+                if (h_self > 0) {
+                    SQB_TRY(h->d_selfnodes.alloc(h_self));
+                    cudaMemsetAsync(flag.p, 0, sizeof(uint32_t), ctx->stream);
+                    nhood_self_fill_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, ctx->stream>>>(h->d_uptr.p, h->d_uidx.p, n, h->d_selfnodes.p,
+                                                                                                 flag.p);
+                    SQB_CUDA(cudaStreamSynchronize(ctx->stream));
                 }
+                h->n_self = h_self;
+                h->sym = true;
             }
-        }
-        cleanup();
-        if (e != cudaSuccess || rc != SQB_OK) {
-            if (e != cudaSuccess) sqb_set_error("%s: symmetric-graph preparation failed: %s", where, cudaGetErrorString(e));
-            sqb_nhood_destroy(h);
-            return e != cudaSuccess ? SQB_ERR_CUDA : rc;
         }
         h->d_uptr.release();  // the count kernel walks the row records; the upper CSR was only their scaffolding
         h->d_uidx.release();
@@ -3173,12 +3093,7 @@ static int nhood_prepare(sqb_nhood* h, const char* where) {
             }
         }
     }
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-        sqb_set_error("%s: %s", where, cudaGetErrorString(e));
-        sqb_nhood_destroy(h);
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cudaStreamSynchronize(ctx->stream));
     return SQB_OK;
 }
 
@@ -3226,13 +3141,13 @@ int sqb_nhood_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indpt
               "sqb_nhood_create: indptr[0]=%u indptr[n]=%u inconsistent with nnz=%lld", indptr[0], indptr[n],
               (long long)nnz);
     SQB_CUDA(cudaSetDevice(ctx->device));
-    sqb_nhood* h = nullptr;
-    SQB_TRY(nhood_new(ctx, n, nnz, n_cls, &h));
+    std::unique_ptr<sqb_nhood> h;
+    SQB_TRY(nhood_new(ctx, n, nnz, n_cls, h));
     SQB_CUDA(cudaMemcpyAsync(h->d_indptr.p, indptr, (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     if (nnz > 0)
         SQB_TRY(sqb_h2d(ctx, h->d_indices.p, indices, nnz * sizeof(uint32_t)));
-    SQB_TRY(nhood_prepare(h, "sqb_nhood_create"));
-    *out = h;
+    SQB_TRY(nhood_prepare(h.get(), "sqb_nhood_create"));
+    *out = h.release();
     return SQB_OK;
 }
 
@@ -3245,54 +3160,32 @@ int sqb_nhood_create_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* in
               "%s: indptr_bits / index_bits must be 32 or 64", where);
     SQB_CUDA(cudaSetDevice(ctx->device));
     SQB_TRY(sqb_wait_producer(ctx, producer_stream));
-    sqb_nhood* h = nullptr;
-    SQB_TRY(nhood_new(ctx, n, nnz, n_cls, &h));
-    DevBuf<unsigned> err;
-    err.bind(ctx->stream);
-    int rc = err.alloc(1);
-    if (rc == SQB_OK) {
-        const cudaError_t e = cudaMemsetAsync(err.p, 0, sizeof(unsigned), ctx->stream);
-        if (e != cudaSuccess) {
-            sqb_set_error("%s: %s", where, cudaGetErrorString(e));
-            rc = SQB_ERR_CUDA;
-        }
-    }
-    if (rc == SQB_OK) {
+    std::unique_ptr<sqb_nhood> h;
+    SQB_TRY(nhood_new(ctx, n, nnz, n_cls, h));
+    auto body = [&]() -> int {
+        DevBuf<unsigned> err(ctx->stream);
+        SQB_TRY(err.alloc(1));
+        SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), ctx->stream));
         if (indptr_bits == 32)
-            rc = index_bits == 32 ? nhood_fill_device<int32_t, int32_t>(h, indptr, indices, err.p) : nhood_fill_device<int32_t, int64_t>(h, indptr, indices, err.p);
-        else
-            rc = index_bits == 32 ? nhood_fill_device<int64_t, int32_t>(h, indptr, indices, err.p) : nhood_fill_device<int64_t, int64_t>(h, indptr, indices, err.p);
-    }
-    if (rc != SQB_OK) cudaStreamSynchronize(ctx->stream);  // the caller's buffers are no longer read
-    err.release();
+            return index_bits == 32 ? nhood_fill_device<int32_t, int32_t>(h.get(), indptr, indices, err.p)
+                                    : nhood_fill_device<int32_t, int64_t>(h.get(), indptr, indices, err.p);
+        return index_bits == 32 ? nhood_fill_device<int64_t, int32_t>(h.get(), indptr, indices, err.p)
+                                : nhood_fill_device<int64_t, int64_t>(h.get(), indptr, indices, err.p);
+    };
+    const int rc = body();
     if (rc != SQB_OK) {
-        sqb_nhood_destroy(h);
+        cudaStreamSynchronize(ctx->stream);  // the caller's buffers are no longer read
         return rc;
     }
     // from here on the handle's own copy is all that is read: the chain of the host path
-    SQB_TRY(nhood_prepare(h, where));
-    *out = h;
+    SQB_TRY(nhood_prepare(h.get(), where));
+    *out = h.release();
     return SQB_OK;
 }
 
 int sqb_nhood_destroy(sqb_nhood* h) {
     if (!h) return SQB_OK;
     cudaSetDevice(h->ctx->device);
-    h->d_indptr.release();
-    h->d_indices.release();
-    h->d_uptr.release();
-    h->d_uidx.release();
-    h->d_recs.release();
-    h->d_selfnodes.release();
-    h->d_base.release();
-    h->d_order.release();
-    h->d_seg_start.release();
-    h->d_seg_len.release();
-    h->d_states.release();
-    h->d_counts.release();
-    h->d_cum.release();
-    h->d_bkt.release();
-    h->d_tmp_u32.release();
     delete h;
     return SQB_OK;
 }
@@ -3367,35 +3260,26 @@ int sqb_nhood_count(sqb_nhood* h, const uint32_t* labels, uint32_t* out) {
                   (long long)i, labels[i], h->n_cls);
     if (!h->count_single) return nhood_count_batched_path(h, labels, out);
     const int64_t CC = (int64_t)h->n_cls * h->n_cls;
-    DevBuf<uint32_t> cnt;
-    cnt.bind(c->stream);
-    int rc = SQB_OK;
-    if ((rc = h->d_tmp_u32.alloc(h->n)) != SQB_OK) return rc;
-    if ((rc = cnt.alloc(CC)) != SQB_OK) return rc;
-    cudaError_t e = cudaMemcpyAsync(h->d_tmp_u32.p, labels, h->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(cnt.p, 0, CC * sizeof(uint32_t), c->stream);
-    if (e == cudaSuccess) {
-        const size_t smem = (size_t)CC * sizeof(uint32_t);
-        const int hist_smem = smem <= 160 * 1024 ? 1 : 0;
-        if (hist_smem && smem > 48 * 1024) e = cudaFuncSetAttribute(nhood_count_single_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) {
-            SqbLaunchScope scope(c, SQB_K_NHOOD_COUNT);
-            int64_t ctas = ceil_div64(h->n, 8 * 16);  // >= 16 rows per warp
-            const int64_t cap = (int64_t)c->sm_count * (smem > 32 * 1024 ? 2 : 8);
-            if (ctas > cap) ctas = cap;
-            if (ctas < 1) ctas = 1;
-            nhood_count_single_kernel<<<(unsigned)ctas, 256, hist_smem ? smem : 0, c->stream>>>(h->d_indptr.p, h->d_indices.p, h->d_tmp_u32.p, h->n,
-                                                                                                 h->n_cls, hist_smem, cnt.p);
-            e = cudaGetLastError();
-        }
+    DevBuf<uint32_t> cnt(c->stream);
+    SQB_TRY(h->d_tmp_u32.alloc(h->n));
+    SQB_TRY(cnt.alloc(CC));
+    SQB_CUDA(cudaMemcpyAsync(h->d_tmp_u32.p, labels, h->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemsetAsync(cnt.p, 0, CC * sizeof(uint32_t), c->stream));
+    const size_t smem = (size_t)CC * sizeof(uint32_t);
+    const int hist_smem = smem <= 160 * 1024 ? 1 : 0;
+    if (hist_smem && smem > 48 * 1024) SQB_CUDA(cudaFuncSetAttribute(nhood_count_single_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    {
+        SqbLaunchScope scope(c, SQB_K_NHOOD_COUNT);
+        int64_t ctas = ceil_div64(h->n, 8 * 16);  // >= 16 rows per warp
+        const int64_t cap = (int64_t)c->sm_count * (smem > 32 * 1024 ? 2 : 8);
+        if (ctas > cap) ctas = cap;
+        if (ctas < 1) ctas = 1;
+        nhood_count_single_kernel<<<(unsigned)ctas, 256, hist_smem ? smem : 0, c->stream>>>(h->d_indptr.p, h->d_indices.p, h->d_tmp_u32.p, h->n,
+                                                                                             h->n_cls, hist_smem, cnt.p);
+        SQB_POST_LAUNCH();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, cnt.p, CC * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cnt.release();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_nhood_count: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cudaMemcpyAsync(out, cnt.p, CC * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 
@@ -3593,22 +3477,16 @@ int sqb_nhood_permute_stats(sqb_nhood* h, double* mean_out, double* std_out) {
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
     const int CC = h->n_cls * h->n_cls;
-    DevBuf<double> d;
-    d.bind(c->stream);
+    DevBuf<double> d(c->stream);
     SQB_TRY(d.alloc((size_t)2 * CC));
     {
         SqbLaunchScope scope(c, SQB_K_MISC);
         nhood_stats_kernel<<<(unsigned)ceil_div64(CC, 64), 64, 0, c->stream>>>(h->d_counts.p, h->n_perms, CC, d.p, d.p + CC);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(mean_out, d.p, CC * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(std_out, d.p + CC, CC * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    d.release();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_nhood_permute_stats: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_POST_LAUNCH();
+    SQB_CUDA(cudaMemcpyAsync(mean_out, d.p, CC * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(std_out, d.p + CC, CC * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 
@@ -3643,21 +3521,15 @@ int sqb_nhood_permute_sums(sqb_nhood* h, int64_t* sums_out) {
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
     const int CC = h->n_cls * h->n_cls;
-    DevBuf<unsigned long long> d;
-    d.bind(c->stream);
+    DevBuf<unsigned long long> d(c->stream);
     SQB_TRY(d.alloc(CC));
     {
         SqbLaunchScope scope(c, SQB_K_MISC);
         nhood_sums_kernel<<<(unsigned)ceil_div64(CC, 64), 64, 0, c->stream>>>(h->d_counts.p, h->n_perms, CC, d.p);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(sums_out, d.p, CC * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    d.release();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_nhood_permute_sums: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_POST_LAUNCH();
+    SQB_CUDA(cudaMemcpyAsync(sums_out, d.p, CC * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 
@@ -3667,23 +3539,17 @@ int sqb_nhood_permute_var_chain(sqb_nhood* h, const double* mean, const double* 
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
     const int CC = h->n_cls * h->n_cls;
-    DevBuf<double> d;
-    d.bind(c->stream);
+    DevBuf<double> d(c->stream);
     SQB_TRY(d.alloc((size_t)3 * CC));
-    cudaError_t e = cudaMemcpyAsync(d.p, mean, CC * sizeof(double), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.p + CC, acc_in, CC * sizeof(double), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
+    SQB_CUDA(cudaMemcpyAsync(d.p, mean, CC * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(d.p + CC, acc_in, CC * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    {
         SqbLaunchScope scope(c, SQB_K_MISC);
         nhood_var_chain_kernel<<<(unsigned)ceil_div64(CC, 64), 64, 0, c->stream>>>(h->d_counts.p, h->n_perms, CC, d.p, d.p + CC, d.p + 2 * CC);
-        e = cudaGetLastError();
+        SQB_POST_LAUNCH();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(acc_out, d.p + 2 * CC, CC * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    d.release();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_nhood_permute_var_chain: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cudaMemcpyAsync(acc_out, d.p + 2 * CC, CC * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 
@@ -3822,10 +3688,10 @@ __global__ void ligrec_compare_kernel(const double* __restrict__ G, int64_t np, 
 }
 
 // sqb_ligrec_counts over an observations x genes float64 matrix already on the device (d_data: the host copy of
-// sqb_ligrec_counts, or a gathered sqb_dense).  where: the entry point named in error messages.
+// sqb_ligrec_counts, or a gathered sqb_dense)
 static int ligrec_counts_impl(sqb_nhood* h, const double* d_data, int64_t n_genes, const double* inv_counts, const double* mean_obs,
                               const int32_t* interactions, int64_t n_inter, const int32_t* inter_clusters, int64_t n_cpairs,
-                              const uint8_t* valid, int64_t* out_counts, const char* where) {
+                              const uint8_t* valid, int64_t* out_counts) {
     sqb_ctx* c = h->ctx;
     const int C = h->n_cls;
     const size_t smem = (size_t)4 * C * 32 * sizeof(double);
@@ -3838,59 +3704,51 @@ static int ligrec_counts_impl(sqb_nhood* h, const double* d_data, int64_t n_gene
     DevBuf<int32_t> d_inter, d_cp;
     DevBuf<uint8_t> d_valid;
     DevBuf<long long> d_cnt;
-    auto cleanup = [&]() {
-        d_inv.release(), d_obs.release(), d_G.release(), d_inter.release(), d_cp.release(), d_valid.release(), d_cnt.release();
+    SQB_TRY(d_inv.alloc(C));
+    SQB_TRY(d_obs.alloc((size_t)C * n_genes));
+    SQB_TRY(d_G.alloc((size_t)chunk * C * n_genes));
+    SQB_TRY(d_inter.alloc(2 * n_inter));
+    SQB_TRY(d_cp.alloc(2 * n_cpairs));
+    SQB_TRY(d_valid.alloc(NT));
+    SQB_TRY(d_cnt.alloc(NT));
+    SQB_TRY(ensure_buffers(h, h->chunk));
+    auto body = [&]() -> int {
+        SQB_CUDA(cudaMemsetAsync(d_cnt.p, 0, NT * sizeof(long long), c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_inv.p, inv_counts, C * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_obs.p, mean_obs, (size_t)C * n_genes * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_inter.p, interactions, 2 * n_inter * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_cp.p, inter_clusters, 2 * n_cpairs * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_valid.p, valid, NT, cudaMemcpyHostToDevice, c->stream));
+        if (smem > 48 * 1024) {
+            SQB_CUDA(cudaFuncSetAttribute(ligrec_group_means_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            SQB_CUDA(cudaFuncSetAttribute(ligrec_group_means_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        }
+        for (int64_t p0 = 0; p0 < h->n_perms; p0 += chunk) {
+            const int64_t np = h->n_perms - p0 < chunk ? h->n_perms - p0 : chunk;
+            SQB_TRY(h->lt_bytes == 1 ? run_chunk<uint8_t>(h, p0, np, false) : run_chunk<uint16_t>(h, p0, np, false));
+            {
+                SqbLaunchScope scope(c, SQB_K_MISC);
+                dim3 grid((unsigned)ceil_div64(n_genes, 128), (unsigned)np);
+                if (h->lt_bytes == 1)
+                    ligrec_group_means_kernel<uint8_t><<<grid, 128, smem, c->stream>>>(c->scratch[0].p, h->stride, d_data, n, (int)n_genes, C, d_inv.p, d_G.p);
+                else
+                    ligrec_group_means_kernel<uint16_t><<<grid, 128, smem, c->stream>>>(reinterpret_cast<const uint16_t*>(c->scratch[0].p), h->stride,
+                                                                                         d_data, n, (int)n_genes, C, d_inv.p, d_G.p);
+            }
+            {
+                SqbLaunchScope scope(c, SQB_K_MISC);
+                ligrec_compare_kernel<<<(unsigned)ceil_div64(NT, 256), 256, 0, c->stream>>>(d_G.p, np, C, (int)n_genes, d_obs.p, d_inter.p, n_inter, d_cp.p,
+                                                                                            n_cpairs, d_valid.p, d_cnt.p);
+            }
+            SQB_POST_LAUNCH();
+        }
+        SQB_CUDA(cudaMemcpyAsync(out_counts, d_cnt.p, NT * sizeof(long long), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        return SQB_OK;
     };
-    int rc;
-    if ((rc = d_inv.alloc(C)) || (rc = d_obs.alloc((size_t)C * n_genes)) || (rc = d_G.alloc((size_t)chunk * C * n_genes)) ||
-        (rc = d_inter.alloc(2 * n_inter)) || (rc = d_cp.alloc(2 * n_cpairs)) || (rc = d_valid.alloc(NT)) || (rc = d_cnt.alloc(NT)) ||
-        (rc = ensure_buffers(h, h->chunk))) {
-        cleanup();
-        return rc;
-    }
-    cudaError_t e = cudaMemsetAsync(d_cnt.p, 0, NT * sizeof(long long), c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_inv.p, inv_counts, C * sizeof(double), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_obs.p, mean_obs, (size_t)C * n_genes * sizeof(double), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_inter.p, interactions, 2 * n_inter * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_cp.p, inter_clusters, 2 * n_cpairs * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_valid.p, valid, NT, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess && smem > 48 * 1024) {
-        e = cudaFuncSetAttribute(ligrec_group_means_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(ligrec_group_means_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    }
-    for (int64_t p0 = 0; p0 < h->n_perms && e == cudaSuccess; p0 += chunk) {
-        const int64_t np = h->n_perms - p0 < chunk ? h->n_perms - p0 : chunk;
-        rc = h->lt_bytes == 1 ? run_chunk<uint8_t>(h, p0, np, false) : run_chunk<uint16_t>(h, p0, np, false);
-        if (rc != SQB_OK) {
-            cudaStreamSynchronize(c->stream);
-            cleanup();
-            return rc;
-        }
-        {
-            SqbLaunchScope scope(c, SQB_K_MISC);
-            dim3 grid((unsigned)ceil_div64(n_genes, 128), (unsigned)np);
-            if (h->lt_bytes == 1)
-                ligrec_group_means_kernel<uint8_t><<<grid, 128, smem, c->stream>>>(c->scratch[0].p, h->stride, d_data, n, (int)n_genes, C, d_inv.p, d_G.p);
-            else
-                ligrec_group_means_kernel<uint16_t><<<grid, 128, smem, c->stream>>>(reinterpret_cast<const uint16_t*>(c->scratch[0].p), h->stride,
-                                                                                     d_data, n, (int)n_genes, C, d_inv.p, d_G.p);
-        }
-        {
-            SqbLaunchScope scope(c, SQB_K_MISC);
-            ligrec_compare_kernel<<<(unsigned)ceil_div64(NT, 256), 256, 0, c->stream>>>(d_G.p, np, C, (int)n_genes, d_obs.p, d_inter.p, n_inter, d_cp.p,
-                                                                                        n_cpairs, d_valid.p, d_cnt.p);
-        }
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_counts, d_cnt.p, NT * sizeof(long long), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    else cudaStreamSynchronize(c->stream);
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("%s: %s", where, cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
-    return SQB_OK;
+    const int rc = body();
+    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);
+    return rc;
 }
 
 // the argument checks shared by both entry points
@@ -3925,10 +3783,9 @@ int sqb_ligrec_counts(sqb_nhood* h, const double* data, int64_t n_genes, const d
     SQB_TRY(d_data.alloc((size_t)h->n * n_genes));
     int rc = sqb_h2d(c, d_data.p, data, (size_t)h->n * n_genes * sizeof(double));
     if (rc == SQB_OK)
-        rc = ligrec_counts_impl(h, d_data.p, n_genes, inv_counts, mean_obs, interactions, n_inter, inter_clusters, n_cpairs, valid, out_counts, where);
+        rc = ligrec_counts_impl(h, d_data.p, n_genes, inv_counts, mean_obs, interactions, n_inter, inter_clusters, n_cpairs, valid, out_counts);
     else
         cudaStreamSynchronize(c->stream);
-    d_data.release();
     return rc;
 }
 
@@ -3942,7 +3799,7 @@ int sqb_ligrec_counts_dense(sqb_nhood* h, const sqb_dense* x, const double* inv_
               "%s: expected a float64 observations x genes matrix of %lld observations", where, (long long)h->n);
     SQB_TRY(ligrec_counts_check(h, x->n_genes, interactions, n_inter, inter_clusters, n_cpairs, where));
     return ligrec_counts_impl(h, reinterpret_cast<const double*>(x->buf.p), x->n_genes, inv_counts, mean_obs, interactions, n_inter,
-                              inter_clusters, n_cpairs, valid, out_counts, where);
+                              inter_clusters, n_cpairs, valid, out_counts);
 }
 
 int sqb_nhood_permute(sqb_nhood* h, const uint64_t* states, int64_t n_perms, uint32_t* out_counts) {

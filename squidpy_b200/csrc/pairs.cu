@@ -221,39 +221,23 @@ static int pairs_run(sqb_ctx* c, const FT* xy /* interleaved, grouped */, int64_
     DevBuf<FT> d_thr;
     DevBuf<int> d_lut;
     DevBuf<unsigned long long> d_out;
-    int rc = SQB_OK;
-    auto cleanup = [&]() {
-        d_pts.release();
-        d_tiles.release();
-        d_thr.release();
-        d_lut.release();
-        d_out.release();
-    };
-    if ((rc = d_pts.alloc(n)) || (rc = d_tiles.alloc(ntiles)) || (rc = d_thr.alloc(L)) || (rc = d_lut.alloc(PAIRS_NC)) ||
-        (rc = d_out.alloc((size_t)nslots * L))) {
-        cleanup();
-        return rc;
-    }
-    cudaError_t e = cudaMemcpyAsync(d_pts.p, xy, n * sizeof(V2), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_tiles.p, tiles.data(), ntiles * sizeof(PairTile), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_thr.p, thr, L * sizeof(FT), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_lut.p, lut.data(), PAIRS_NC * sizeof(int), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_out.p, 0, (size_t)nslots * L * sizeof(unsigned long long), c->stream);
-    if (e != cudaSuccess) {
-        cleanup();
-        sqb_set_error("pairs: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_TRY(d_pts.alloc(n));
+    SQB_TRY(d_tiles.alloc(ntiles));
+    SQB_TRY(d_thr.alloc(L));
+    SQB_TRY(d_lut.alloc(PAIRS_NC));
+    SQB_TRY(d_out.alloc((size_t)nslots * L));
+    SQB_CUDA(cudaMemcpyAsync(d_pts.p, xy, n * sizeof(V2), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(d_tiles.p, tiles.data(), ntiles * sizeof(PairTile), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(d_thr.p, thr, L * sizeof(FT), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(d_lut.p, lut.data(), PAIRS_NC * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemsetAsync(d_out.p, 0, (size_t)nslots * L * sizeof(unsigned long long), c->stream));
     const size_t base_smem = PAIRS_JCHUNK * sizeof(V2) + (size_t)((L + 2) / 2 * 2) * sizeof(FT) + PAIRS_NC * sizeof(int);
     const size_t priv_smem = base_smem + (size_t)(PAIRS_THREADS / 32) * L * 32 * 4;
     const size_t shared_smem = base_smem + (size_t)(PAIRS_THREADS / 32) * L * 4;
     const bool lanepriv = priv_smem + 1024 <= c->smem_optin;
     const size_t smem = lanepriv ? priv_smem : shared_smem;
-    if (smem + 1024 > c->smem_optin) {
-        cleanup();
-        sqb_set_error("pairs: %d radial bins need %zu bytes of shared memory (> %zu)", L, smem, c->smem_optin);
-        return SQB_ERR_UNSUPPORTED;
-    }
+    SQB_CHECK(smem + 1024 <= c->smem_optin, SQB_ERR_UNSUPPORTED, "pairs: %d radial bins need %zu bytes of shared memory (> %zu)", L, smem,
+              c->smem_optin);
     int ctas_per_sm = (int)std::max<size_t>(1, std::min<size_t>(8, (c->smem_optin + 1024) / (smem + 1024)));
     int64_t my_tiles = (ntiles - shard_index + shard_count - 1) / shard_count;
     int64_t grid = std::min<int64_t>((int64_t)c->sm_count * ctas_per_sm, std::max<int64_t>(my_tiles, 1));
@@ -262,10 +246,9 @@ static int pairs_run(sqb_ctx* c, const FT* xy /* interleaved, grouped */, int64_
 #define PAIRS_LAUNCH(FMAV, LP)                                                                                        \
     do {                                                                                                              \
         auto kern = pairs_kernel<FT, FMAV, LP>;                                                                       \
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                      \
-        if (e == cudaSuccess)                                                                                         \
-            kern<<<(unsigned)grid, PAIRS_THREADS, smem, c->stream>>>(d_pts.p, d_tiles.p, ntiles, shard_index,         \
-                                                                     shard_count, d_thr.p, L, d_lut.p, scale, d_out.p); \
+        SQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                \
+        kern<<<(unsigned)grid, PAIRS_THREADS, smem, c->stream>>>(d_pts.p, d_tiles.p, ntiles, shard_index, shard_count, \
+                                                                 d_thr.p, L, d_lut.p, scale, d_out.p);                \
     } while (0)
         if (use_fma) {
             if (lanepriv)
@@ -279,15 +262,10 @@ static int pairs_run(sqb_ctx* c, const FT* xy /* interleaved, grouped */, int64_
                 PAIRS_LAUNCH(0, false);
         }
 #undef PAIRS_LAUNCH
-        if (e == cudaSuccess) e = cudaGetLastError();
+        SQB_POST_LAUNCH();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(hout.data(), d_out.p, (size_t)nslots * L * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("pairs: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
+    SQB_CUDA(cudaMemcpyAsync(hout.data(), d_out.p, (size_t)nslots * L * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 

@@ -140,12 +140,6 @@ static int sepal_check(const int32_t* sat, int64_t n_sat, const int32_t* sat_idx
 static int sepal_impl(sqb_ctx* c, const double* d_vals, int64_t n_genes, int64_t n, const int32_t* sat, int64_t n_sat, const int32_t* sat_idx,
                       int max_neighs, const int32_t* unsat, const int32_t* unsat_idx, int64_t n_unsat, int n_iter, double dt, double thresh,
                       double* out) {
-    DevBuf<double> d_out, d_scr;
-    DevBuf<int32_t> d_sat, d_idx, d_unsat, d_uidx;
-    DevBuf<int> d_cnt;
-    auto cleanup = [&]() {
-        d_out.release(), d_scr.release(), d_sat.release(), d_idx.release(), d_unsat.release(), d_uidx.release(), d_cnt.release();
-    };
     const size_t need = (size_t)2 * n * sizeof(double);
     const bool global = need + 1024 > c->smem_optin;
     const size_t smem = global ? 0 : need;
@@ -155,36 +149,38 @@ static int sepal_impl(sqb_ctx* c, const double* d_vals, int64_t n_genes, int64_t
     if (per_sm < 1) per_sm = 1;
     int64_t ctas = (int64_t)per_sm * c->sm_count;
     if (ctas > n_genes) ctas = n_genes;
-    int rc;
-    if ((rc = d_out.alloc(n_genes)) || (rc = d_sat.alloc(n_sat)) || (rc = d_idx.alloc((size_t)n_sat * max_neighs)) ||
-        (rc = d_unsat.alloc(n_unsat > 0 ? n_unsat : 1)) || (rc = d_uidx.alloc(n_unsat > 0 ? n_unsat : 1)) || (rc = d_cnt.alloc(1)) ||
-        (global && (rc = d_scr.alloc((size_t)ctas * 2 * n)))) {
-        cleanup();
-        return rc;
-    }
-    cudaError_t e = cudaMemsetAsync(d_cnt.p, 0, sizeof(int), c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_sat.p, sat, n_sat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_idx.p, sat_idx, (size_t)n_sat * max_neighs * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess && n_unsat > 0) e = cudaMemcpyAsync(d_unsat.p, unsat, n_unsat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess && n_unsat > 0) e = cudaMemcpyAsync(d_uidx.p, unsat_idx, n_unsat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        SepalParams p;
-        p.vals = d_vals, p.n_genes = n_genes, p.n = n, p.sat = d_sat.p, p.sat_idx = d_idx.p, p.n_sat = (int)n_sat, p.K = max_neighs;
-        p.unsat = d_unsat.p, p.unsat_idx = d_uidx.p, p.n_unsat = (int)n_unsat, p.use_hex = max_neighs == 6, p.n_iter = n_iter, p.dt = dt, p.thresh = thresh;
-        p.out = d_out.p, p.g_scratch = global ? d_scr.p : nullptr, p.counter = d_cnt.p;
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        sepal_kernel<<<(unsigned)ctas, SEPAL_T, smem, c->stream>>>(p);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out.p, n_genes * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    else cudaStreamSynchronize(c->stream);
-    cleanup();
-    if (e != cudaSuccess) {
-        sqb_set_error("sqb_sepal: %s", cudaGetErrorString(e));
-        return SQB_ERR_CUDA;
-    }
-    return SQB_OK;
+    DevBuf<double> d_out, d_scr;
+    DevBuf<int32_t> d_sat, d_idx, d_unsat, d_uidx;
+    DevBuf<int> d_cnt;
+    SQB_TRY(d_out.alloc(n_genes));
+    SQB_TRY(d_sat.alloc(n_sat));
+    SQB_TRY(d_idx.alloc((size_t)n_sat * max_neighs));
+    SQB_TRY(d_unsat.alloc(n_unsat > 0 ? n_unsat : 1));
+    SQB_TRY(d_uidx.alloc(n_unsat > 0 ? n_unsat : 1));
+    SQB_TRY(d_cnt.alloc(1));
+    if (global) SQB_TRY(d_scr.alloc((size_t)ctas * 2 * n));
+    auto body = [&]() -> int {
+        SQB_CUDA(cudaMemsetAsync(d_cnt.p, 0, sizeof(int), c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_sat.p, sat, n_sat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        SQB_CUDA(cudaMemcpyAsync(d_idx.p, sat_idx, (size_t)n_sat * max_neighs * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        if (n_unsat > 0) SQB_CUDA(cudaMemcpyAsync(d_unsat.p, unsat, n_unsat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        if (n_unsat > 0) SQB_CUDA(cudaMemcpyAsync(d_uidx.p, unsat_idx, n_unsat * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        {
+            SepalParams p;
+            p.vals = d_vals, p.n_genes = n_genes, p.n = n, p.sat = d_sat.p, p.sat_idx = d_idx.p, p.n_sat = (int)n_sat, p.K = max_neighs;
+            p.unsat = d_unsat.p, p.unsat_idx = d_uidx.p, p.n_unsat = (int)n_unsat, p.use_hex = max_neighs == 6, p.n_iter = n_iter, p.dt = dt, p.thresh = thresh;
+            p.out = d_out.p, p.g_scratch = global ? d_scr.p : nullptr, p.counter = d_cnt.p;
+            SqbLaunchScope scope(c, SQB_K_MISC);
+            sepal_kernel<<<(unsigned)ctas, SEPAL_T, smem, c->stream>>>(p);
+            SQB_POST_LAUNCH();
+        }
+        SQB_CUDA(cudaMemcpyAsync(out, d_out.p, n_genes * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        return SQB_OK;
+    };
+    const int rc = body();
+    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);
+    return rc;
 }
 
 extern "C" {
@@ -203,7 +199,6 @@ int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, cons
         rc = sepal_impl(c, d_vals.p, n_genes, n, sat, n_sat, sat_idx, max_neighs, unsat, unsat_idx, n_unsat, n_iter, dt, thresh, out);
     else
         cudaStreamSynchronize(c->stream);
-    d_vals.release();
     return rc;
 }
 

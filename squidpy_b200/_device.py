@@ -158,6 +158,15 @@ def index_bits(a: DevArray, what: str) -> int:
     return 8 * a.dtype.itemsize
 
 
+def sparse_args(d: DevSparse, major: int) -> tuple[int, int, int]:
+    """``(indptr_bits, index_bits, nnz)`` of a device CSR / CSC with ``major`` rows (columns for CSC), once its index arrays
+    are int32 / int64 and contiguous and ``indptr`` has ``major + 1`` entries."""
+    ip_bits, ix_bits = index_bits(d.indptr, "indptr"), index_bits(d.indices, "indices")
+    if d.indptr.shape[0] != major + 1:
+        raise ValueError(f"Expected `indptr` of length `{major + 1}`, found `{d.indptr.shape[0]}`.")
+    return ip_bits, ix_bits, int(d.indices.shape[0])
+
+
 @dataclass
 class DevGraph:
     """The ABI arguments of a device neighbour graph (``sqb_nhood_create_device`` / ``sqb_interaction_matrix_device``).
@@ -195,10 +204,7 @@ def graph_args(d: DevSparse, n_obs: int) -> DevGraph:
     """Check that ``d`` is an ``n_obs x n_obs`` graph with int32 / int64 index arrays and describe it for the C ABI."""
     if tuple(d.shape) != (n_obs, n_obs):
         raise ValueError(f"Expected the connectivity graph to be of shape `{(n_obs, n_obs)}`, found `{tuple(d.shape)}`.")
-    ip_bits, ix_bits = index_bits(d.indptr, "indptr"), index_bits(d.indices, "indices")
-    if d.indptr.shape[0] != n_obs + 1:
-        raise ValueError(f"Expected `indptr` of length `{n_obs + 1}`, found `{d.indptr.shape[0]}`.")
-    nnz = int(d.indices.shape[0])
+    ip_bits, ix_bits, nnz = sparse_args(d, n_obs)
     return DevGraph(d, n_obs, nnz, ip_bits, ix_bits, d.format == "csc", common_stream(d))
 
 
@@ -260,11 +266,7 @@ def matrix_args(d: DevArray | DevSparse, shape: tuple[int, int]) -> DevMatrix:
         raise ValueError(f"Expected the expression matrix to be of shape `{shape}`, found `{tuple(d.shape)}`.")
     stream = common_stream(d)
     if isinstance(d, DevSparse):
-        ip_bits, ix_bits = index_bits(d.indptr, "indptr"), index_bits(d.indices, "indices")
-        major = shape[0] if d.format == "csr" else shape[1]
-        if d.indptr.shape[0] != major + 1:
-            raise ValueError(f"Expected `indptr` of length `{major + 1}`, found `{d.indptr.shape[0]}`.")
-        nnz = int(d.indices.shape[0])
+        ip_bits, ix_bits, nnz = sparse_args(d, shape[0] if d.format == "csr" else shape[1])
         code = dtype_code(d.data)
         if len(d.data.shape) != 1 or d.data.shape[0] < nnz or (nnz > 1 and d.data.strides[0] != 1):
             raise ValueError(f"The matrix's values must be a contiguous 1-D array of `{nnz}` entries.")

@@ -194,28 +194,9 @@ __global__ void __launch_bounds__(256) ac_final_kernel(const double* __restrict_
 #define AC_T 256          // threads per CTA of the per-feature kernels
 #define AC_NW (AC_T / 32)
 
-enum { AC_ERR_INDEX = 1, AC_ERR_DUP = 2, AC_ERR_INDPTR = 4, AC_ERR_PERM = 8 };
+enum { AC_ERR_INDEX = 1, AC_ERR_DUP = 2, AC_ERR_PERM = 8 };
 
 // ---- input validation / transposition (load time) ----------------------------------------------------
-// Value conversion of the caller's data type to the device layout's (float16 goes through float32: exact)
-template <typename XT, typename VT>
-struct AcCvt {
-    __device__ __forceinline__ static XT f(VT v) { return (XT)v; }
-};
-template <typename XT>
-struct AcCvt<XT, __half> {
-    __device__ __forceinline__ static XT f(__half v) { return (XT)__half2float(v); }
-};
-
-// indptr must start at 0, be non-decreasing and end at nnz
-template <typename IP>
-__global__ void ac_check_indptr_kernel(const IP* __restrict__ ptr, int64_t rows, int64_t nnz, int* __restrict__ err) {
-    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t a = (int64_t)ptr[r], b = (int64_t)ptr[r + 1];
-        if (a > b || a < 0 || b > nnz || (r == 0 && a != 0)) atomicOr(err, AC_ERR_INDPTR);
-    }
-}
-
 // Output feature of input column c, or -1 to skip it (range errors raise *err unless err is null).  colmap == null: the shard [col_lo, col_lo + n_feat) of the columns,
 // anything outside is an error; else colmap[c] for c in [0, n_cols).
 __device__ __forceinline__ int64_t ac_map_col(int64_t c, int64_t n_feat, int32_t col_lo, const int32_t* __restrict__ colmap,
@@ -319,20 +300,6 @@ __global__ void __launch_bounds__(1024) ac_scan_counts_kernel(const unsigned int
     }
 }
 
-// padded starts for a caller-supplied CSR by feature: cnt[g] = ptr[g+1] - ptr[g]
-__global__ void ac_seglen_kernel(const int64_t* __restrict__ ptr, int64_t n_feat, int64_t n, unsigned int* __restrict__ cnt,
-                                 int* __restrict__ err) {
-    for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < n_feat; g += (int64_t)gridDim.x * blockDim.x) {
-        int64_t d = ptr[g + 1] - ptr[g];
-        if (d < 0) d = 0;  // flagged by ac_check_indptr_kernel
-        if (d > n) {
-            atomicOr(err, AC_ERR_DUP);  // more entries than observations: some index repeats
-            d = n;
-        }
-        cnt[g] = (unsigned int)d;
-    }
-}
-
 // segments of the selected features of a caller's CSR by feature: feature k is input row inv[k]
 template <typename IP>
 __global__ void ac_select_segs_kernel(const IP* __restrict__ ptr, const int32_t* __restrict__ inv, int64_t n_out,
@@ -366,7 +333,7 @@ __global__ void ac_coltranspose_kernel(const IP* __restrict__ xp, const II* __re
             if (c < 0) continue;
             const unsigned long long pos = atomicAdd(&cursor[c], 1ULL);
             oi[pos] = (int32_t)r;
-            ov[pos] = AcCvt<XT, VT>::f(xv[e]);
+            ov[pos] = sqb_cvt<XT>(xv[e]);
         }
     }
 }
@@ -380,7 +347,7 @@ __global__ void ac_gather_dense_kernel(const VT* __restrict__ x, int64_t n_obs, 
     for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = obs_major ? t / n_out : t % n_obs;
         const int64_t k = obs_major ? t - r * n_out : t / n_obs;
-        out[t] = AcCvt<XT, VT>::f(x[r * s_obs + (int64_t)inv[k] * s_feat]);
+        out[t] = sqb_cvt<XT>(x[r * s_obs + (int64_t)inv[k] * s_feat]);
     }
 }
 
@@ -473,7 +440,7 @@ __global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __res
             const unsigned int bit = 1u << (i & 31);
             const int64_t pos = os + s.y + __popc(s.x & (bit - 1u));
             out_idx[pos] = (int32_t)i;
-            out_val[pos] = AcCvt<XT, VT>::f(in_val[rb + e]);
+            out_val[pos] = sqb_cvt<XT>(in_val[rb + e]);
         }
         const int lenp = (len + 3) & ~3;
         for (int e = len + threadIdx.x; e < lenp; e += AC_T) {
@@ -863,7 +830,7 @@ struct sqb_autocorr {
     // loaded X
     int kind = 0;     // 0 none, 1 dense feat x obs, 2 dense obs x feat (zero copy tiles), 3 sparse (padded CSR by feature)
     int x_dtype = 0;  // 0 f32, 1 f64
-    int64_t n_feat = 0, x_nnz = 0;
+    int64_t n_feat = 0;
     DevBuf<uint8_t> d_x{ctx->stream};   // dense matrix or padded sparse values
     DevBuf<int64_t> d_xp{ctx->stream};  // padded segment starts (n_feat + 1)
     DevBuf<int32_t> d_xi{ctx->stream}, d_len{ctx->stream}, d_order{ctx->stream};
@@ -883,7 +850,6 @@ struct sqb_autocorr {
 static int xsize(int dt) { return dt == 0 ? 4 : 8; }
 
 static const char* ac_err_text(int f) {
-    if (f & AC_ERR_INDPTR) return "indptr is not a non-decreasing sequence from 0 to nnz";
     if (f & AC_ERR_INDEX) return "index out of range";
     if (f & AC_ERR_DUP) return "an observation is stored twice for one feature (sum duplicates first)";
     if (f & AC_ERR_PERM) return "row_perm is not a permutation";
@@ -1123,90 +1089,7 @@ static int ac_build_segments(sqb_autocorr* h, const int64_t* d_beg, const int64_
     return SQB_OK;
 }
 
-template <typename XT>
-static int ac_load_csr_typed(sqb_autocorr* h, const int64_t* h_xp, const int32_t* h_xi, const void* h_xv, int layout,
-                             int64_t n_feat, int64_t nnz, int32_t col_lo = 0, const int64_t* sub_start = nullptr,
-                             const int64_t* sub_cnt = nullptr) {
-    // sub_start / sub_cnt (layout 1 only): upload only the piece [sub_start[r], +sub_cnt[r]) of every observation's row (the
-    // columns col_lo .. col_lo + n_feat of rows with ascending indices); h_xp then is the indptr of the pieces, nnz their total
-    sqb_ctx* c = h->ctx;
-    const int64_t n = h->n;
-    const int64_t rows = layout == 0 ? n_feat : n;
-    const int64_t nz1 = nnz > 0 ? nnz : 1;
-    DevBuf<int64_t> r_ptr(c->stream), t_ptr(c->stream), pad(c->stream);
-    DevBuf<int32_t> r_idx(c->stream), t_idx(c->stream);
-    DevBuf<uint8_t> r_val(c->stream), t_val(c->stream);
-    DevBuf<unsigned int> cnt(c->stream);
-    DevBuf<unsigned long long> cursor(c->stream);
-    SQB_TRY(r_ptr.alloc(rows + 1));
-    SQB_TRY(r_idx.alloc(nz1));
-    SQB_TRY(r_val.alloc((size_t)nz1 * sizeof(XT)));
-    SQB_TRY(cnt.alloc(n_feat + 1));
-    SQB_TRY(pad.alloc(n_feat + 1));
-    SQB_TRY(h->d_flags.alloc(2));
-    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream));
-    SQB_CUDA(cudaMemcpyAsync(r_ptr.p, h_xp, (rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
-    if (nnz > 0) {  // a failed upload is reported as SQB_ERR_CUDA, whatever the copy returned
-        const bool failed = sub_start ? sqb_h2d_gather(c, r_idx.p, h_xi, sizeof(int32_t), sub_start, sub_cnt, h_xp, rows) ||
-                                            sqb_h2d_gather(c, r_val.p, h_xv, sizeof(XT), sub_start, sub_cnt, h_xp, rows)
-                                      : sqb_h2d(c, r_idx.p, h_xi, nnz * sizeof(int32_t)) || sqb_h2d(c, r_val.p, h_xv, (size_t)nnz * sizeof(XT));
-        if (failed) return SQB_ERR_CUDA;
-    }
-    {
-        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_check_indptr_kernel<int64_t><<<c->sm_count * 4, 256, 0, c->stream>>>(r_ptr.p, rows, nnz, h->d_flags.p);
-    }
-    // the kernels below follow indptr: a bad one must stop the load before they read or write outside [0, nnz)
-    SQB_TRY(ac_check_flags(h, "sqb_autocorr_load_csr"));
-    const int64_t* seg_ptr;
-    const int32_t* seg_idx;
-    const XT* seg_val;
-    if (layout == 0) {
-        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_seglen_kernel<<<c->sm_count * 2, 256, 0, c->stream>>>(r_ptr.p, n_feat, n, cnt.p, h->d_flags.p);
-        seg_ptr = r_ptr.p;
-        seg_idx = r_idx.p;
-        seg_val = reinterpret_cast<const XT*>(r_val.p);
-    } else {
-        SQB_TRY(t_ptr.alloc(n_feat + 1));
-        SQB_TRY(t_idx.alloc(nz1));
-        SQB_TRY(t_val.alloc((size_t)nz1 * sizeof(XT)));
-        SQB_TRY(cursor.alloc(n_feat + 1));
-        SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_feat + 1) * sizeof(unsigned int), c->stream));
-        {
-            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            const size_t hist_bytes = (size_t)n_feat * sizeof(unsigned int);
-            const int hist_smem = hist_bytes <= 160 * 1024 ? 1 : 0;
-            if (hist_smem && hist_bytes > 48 * 1024)
-                cudaFuncSetAttribute(ac_colcount_kernel<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_bytes);
-            ac_colcount_kernel<int32_t><<<c->sm_count * (hist_smem ? 1 : 8), 1024, hist_smem ? hist_bytes : 0, c->stream>>>(
-                r_idx.p, nnz, n_feat, col_lo, nullptr, 0, hist_smem, cnt.p, h->d_flags.p);
-        }
-    }
-    {
-        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        // layout 0: the caller's indptr already is the plain prefix, only the padded starts are needed
-        ac_scan_counts_kernel<<<1, 1024, 0, c->stream>>>(cnt.p, n_feat, layout == 0 ? nullptr : t_ptr.p, pad.p,
-                                                         layout == 0 ? nullptr : cursor.p);
-    }
-    if (layout != 0) {
-        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_coltranspose_kernel<int64_t, int32_t, XT, XT><<<c->sm_count * 8, 256, 0, c->stream>>>(
-            r_ptr.p, r_idx.p, reinterpret_cast<const XT*>(r_val.p), n, n_feat, col_lo, nullptr, 0, cursor.p, t_idx.p,
-            reinterpret_cast<XT*>(t_val.p));
-        seg_ptr = t_ptr.p;
-        seg_idx = t_idx.p;
-        seg_val = reinterpret_cast<const XT*>(t_val.p);
-    }
-    SQB_POST_LAUNCH();
-    int rc = ac_build_segments<int32_t, XT, XT>(h, seg_ptr, seg_ptr + 1, cnt.p, pad.p, seg_idx, seg_val, nnz, n_feat);
-    if (rc == SQB_OK) rc = ac_check_flags(h, "sqb_autocorr_load_csr");  // synchronises: the temporaries may go
-    else cudaStreamSynchronize(c->stream);
-    h->x_nnz = nnz;
-    return rc;
-}
-
-// ---- device-resident input (sqb_autocorr_load_*_device) ------------------------------------------------------------
+// ---- loading X: CSR relayout (host and device-resident), device-resident dense X ---------------------------------------
 // col_map[f] in [0, n_out) or -1 for every input feature f; every output feature must come from exactly one input feature.
 // inv[k] = the input feature of output feature k.
 static int ac_invert_col_map(const int32_t* col_map, int64_t n_cols, int64_t n_out, std::vector<int32_t>& inv, const char* where) {
@@ -1225,13 +1108,14 @@ static int ac_invert_col_map(const int32_t* col_map, int64_t n_cols, int64_t n_o
     return SQB_OK;
 }
 
-// The caller's CSR (indptr IP, indices II, values VT, all in device memory) -> the padded layout by feature (values XT).
-// Nothing of the caller's is staged: the count / transposition / rank-sort kernels read it in place.  indptr is validated
-// (one synchronisation) before any kernel follows it, so no read leaves [0, nnz).
+// A CSR of X in device memory (indptr IP, indices II, values VT: the caller's, read in place, or the host path's upload) -> the
+// padded layout by feature (values XT).  indptr is validated (one synchronisation) before any kernel follows it, so no read
+// leaves [0, nnz).  Layout 0 (rows = features): output feature k is input row inv[k].  Layout 1 (rows = observations): input
+// column j goes to output feature col_map[j] (n_cols entries, -1: skipped), or, with col_map null, to j - col_lo, any column
+// outside [col_lo, col_lo + n_out) being an error.  Synchronises on success.
 template <typename IP, typename II, typename VT, typename XT>
-static int ac_load_csr_device_typed(sqb_autocorr* h, const IP* xp, const II* xi, const VT* xv, int layout, int64_t n_cols,
-                                    const int32_t* col_map, const std::vector<int32_t>& inv, int64_t n_out) {
-    static const char* where = "sqb_autocorr_load_csr_device";
+static int ac_relayout_csr(sqb_autocorr* h, const IP* xp, const II* xi, const VT* xv, int layout, int64_t n_cols, const int32_t* col_map,
+                           int32_t col_lo, const std::vector<int32_t>& inv, int64_t n_out, const char* where) {
     sqb_ctx* c = h->ctx;
     const int64_t n = h->n;
     const int64_t rows = layout == 0 ? n_cols : n;
@@ -1240,87 +1124,97 @@ static int ac_load_csr_device_typed(sqb_autocorr* h, const IP* xp, const II* xi,
     DevBuf<int64_t> beg(c->stream), end(c->stream), t_ptr(c->stream), pad(c->stream);
     DevBuf<unsigned int> cnt(c->stream);
     DevBuf<unsigned long long> cursor(c->stream);
-    int64_t sel = 0;
-    auto body = [&]() -> int {
-        SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream));
-        IP last = 0;
-        SQB_CUDA(cudaMemcpyAsync(&last, xp + rows, sizeof(IP), cudaMemcpyDeviceToHost, c->stream));
-        SQB_CUDA(cudaStreamSynchronize(c->stream));
-        const int64_t nnz = (int64_t)last;
-        SQB_CHECK(nnz >= 0, SQB_ERR_INVALID, "%s: %s", where, ac_err_text(AC_ERR_INDPTR));
-        SQB_CHECK(nnz == 0 || (xi && xv), SQB_ERR_INVALID, "%s: null X arrays", where);
-        {
-            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            ac_check_indptr_kernel<IP><<<c->sm_count * 4, 256, 0, c->stream>>>(xp, rows, nnz, h->d_flags.p);
-            SQB_POST_LAUNCH();
-        }
-        SQB_TRY(ac_check_flags(h, where));
-        SQB_TRY(cnt.alloc(n_out + 1));
-        SQB_TRY(pad.alloc(n_out + 1));
-        SQB_TRY(t_ptr.alloc(n_out + 1));
-        if (layout == 0) {
-            SQB_TRY(map.alloc(n_out));
-            SQB_TRY(beg.alloc(n_out));
-            SQB_TRY(end.alloc(n_out));
-            SQB_CUDA(cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            ac_select_segs_kernel<IP><<<c->sm_count * 2, 256, 0, c->stream>>>(xp, map.p, n_out, beg.p, end.p, cnt.p, n, h->d_flags.p);
-            SQB_POST_LAUNCH();
-        } else {
+    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), c->stream));
+    IP last = 0;
+    SQB_CUDA(cudaMemcpyAsync(&last, xp + rows, sizeof(IP), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    const int64_t nnz = (int64_t)last;
+    SQB_TRY(sqb_check_indptr(c, SQB_K_AUTOCORR_PREP, xp, rows, nnz, nullptr, where));
+    SQB_CHECK(nnz == 0 || (xi && xv), SQB_ERR_INVALID, "%s: null X arrays", where);
+    SQB_TRY(cnt.alloc(n_out + 1));
+    SQB_TRY(pad.alloc(n_out + 1));
+    SQB_TRY(t_ptr.alloc(n_out + 1));
+    if (layout == 0) {
+        SQB_TRY(map.alloc(n_out));
+        SQB_TRY(beg.alloc(n_out));
+        SQB_TRY(end.alloc(n_out));
+        SQB_CUDA(cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_select_segs_kernel<IP><<<c->sm_count * 2, 256, 0, c->stream>>>(xp, map.p, n_out, beg.p, end.p, cnt.p, n, h->d_flags.p);
+        SQB_POST_LAUNCH();
+    } else {
+        if (col_map) {
             SQB_TRY(map.alloc(n_cols));
-            SQB_TRY(cursor.alloc(n_out + 1));
             SQB_CUDA(cudaMemcpyAsync(map.p, col_map, n_cols * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-            SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_out + 1) * sizeof(unsigned int), c->stream));
-            if (nnz > 0) {
-                SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-                const size_t hist_bytes = (size_t)n_out * sizeof(unsigned int);
-                const int hist_smem = hist_bytes <= 160 * 1024 ? 1 : 0;
-                if (hist_smem && hist_bytes > 48 * 1024)
-                    SQB_CUDA(cudaFuncSetAttribute(ac_colcount_kernel<II>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_bytes));
-                ac_colcount_kernel<II><<<c->sm_count * (hist_smem ? 1 : 8), 1024, hist_smem ? hist_bytes : 0, c->stream>>>(
-                    xi, nnz, n_out, 0, map.p, n_cols, hist_smem, cnt.p, h->d_flags.p);
-                SQB_POST_LAUNCH();
-            }
         }
-        {
+        SQB_TRY(cursor.alloc(n_out + 1));
+        SQB_CUDA(cudaMemsetAsync(cnt.p, 0, (n_out + 1) * sizeof(unsigned int), c->stream));
+        if (nnz > 0) {
             SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            ac_scan_counts_kernel<<<1, 1024, 0, c->stream>>>(cnt.p, n_out, t_ptr.p, pad.p, layout == 0 ? nullptr : cursor.p);
+            const size_t hist_bytes = (size_t)n_out * sizeof(unsigned int);
+            const int hist_smem = hist_bytes <= 160 * 1024 ? 1 : 0;
+            if (hist_smem && hist_bytes > 48 * 1024)
+                SQB_CUDA(cudaFuncSetAttribute(ac_colcount_kernel<II>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_bytes));
+            ac_colcount_kernel<II><<<c->sm_count * (hist_smem ? 1 : 8), 1024, hist_smem ? hist_bytes : 0, c->stream>>>(
+                xi, nnz, n_out, col_lo, map.p, n_cols, hist_smem, cnt.p, h->d_flags.p);
             SQB_POST_LAUNCH();
         }
-        // entries of the selected features: the relaid-out copy is sized by them, not by the whole matrix
-        SQB_CUDA(cudaMemcpyAsync(&sel, t_ptr.p + n_out, sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
-        SQB_CUDA(cudaStreamSynchronize(c->stream));
-        if (layout == 0) return ac_build_segments<II, VT, XT>(h, beg.p, end.p, cnt.p, pad.p, xi, xv, sel, n_out);
+    }
+    {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_scan_counts_kernel<<<1, 1024, 0, c->stream>>>(cnt.p, n_out, t_ptr.p, pad.p, layout == 0 ? nullptr : cursor.p);
+        SQB_POST_LAUNCH();
+    }
+    // entries of the selected features: the relaid-out copy is sized by them, not by the whole matrix
+    int64_t sel = 0;
+    SQB_CUDA(cudaMemcpyAsync(&sel, t_ptr.p + n_out, sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    if (layout == 0) {
+        SQB_TRY((ac_build_segments<II, VT, XT>(h, beg.p, end.p, cnt.p, pad.p, xi, xv, sel, n_out)));
+    } else {
         SQB_TRY(t_idx.alloc(sel));
         SQB_TRY(t_val.alloc(sel));
         if (sel > 0) {
             SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            ac_coltranspose_kernel<IP, II, VT, XT><<<c->sm_count * 8, 256, 0, c->stream>>>(xp, xi, xv, n, n_out, 0, map.p, n_cols, cursor.p,
-                                                                                          t_idx.p, t_val.p);
+            ac_coltranspose_kernel<IP, II, VT, XT><<<c->sm_count * 8, 256, 0, c->stream>>>(xp, xi, xv, n, n_out, col_lo, map.p, n_cols,
+                                                                                          cursor.p, t_idx.p, t_val.p);
             SQB_POST_LAUNCH();
         }
-        return ac_build_segments<int32_t, XT, XT>(h, t_ptr.p, t_ptr.p + 1, cnt.p, pad.p, t_idx.p, t_val.p, sel, n_out);
-    };
-    int rc = body();
-    if (rc == SQB_OK) rc = ac_check_flags(h, where);  // synchronises: the caller's buffers are no longer read
-    else cudaStreamSynchronize(c->stream);
-    h->x_nnz = sel;
-    return rc;
+        SQB_TRY((ac_build_segments<int32_t, XT, XT>(h, t_ptr.p, t_ptr.p + 1, cnt.p, pad.p, t_idx.p, t_val.p, sel, n_out)));
+    }
+    return ac_check_flags(h, where);  // synchronises: the inputs are no longer read
 }
 
-template <typename IP, typename II>
-static int ac_load_csr_device_v(sqb_autocorr* h, const void* xp, const void* xi, const void* xv, int data_dtype, int layout,
-                                int64_t n_cols, const int32_t* col_map, const std::vector<int32_t>& inv, int64_t n_out) {
-    const IP* p = reinterpret_cast<const IP*>(xp);
-    const II* i = reinterpret_cast<const II*>(xi);
-    switch (data_dtype) {  // float32 stays float32, everything else becomes float64 (the host path's dtype rule)
-        case 0: return ac_load_csr_device_typed<IP, II, float, float>(h, p, i, (const float*)xv, layout, n_cols, col_map, inv, n_out);
-        case 1: return ac_load_csr_device_typed<IP, II, double, double>(h, p, i, (const double*)xv, layout, n_cols, col_map, inv, n_out);
-        case 2: return ac_load_csr_device_typed<IP, II, __half, double>(h, p, i, (const __half*)xv, layout, n_cols, col_map, inv, n_out);
-        case 3: return ac_load_csr_device_typed<IP, II, int32_t, double>(h, p, i, (const int32_t*)xv, layout, n_cols, col_map, inv, n_out);
-        default: return ac_load_csr_device_typed<IP, II, int64_t, double>(h, p, i, (const int64_t*)xv, layout, n_cols, col_map, inv, n_out);
+// Host CSR of X (int64 indptr, int32 indices, values XT): uploaded, then re-laid out as device input is.  sub_start / sub_cnt
+// (layout 1 only): upload only the piece [sub_start[r], +sub_cnt[r]) of every observation's row (the columns col_lo .. col_lo +
+// n_feat of rows with ascending indices); xp then is the indptr of the pieces.
+template <typename XT>
+static int ac_load_csr_host(sqb_autocorr* h, const int64_t* xp, const int32_t* xi, const void* xv, int layout, int64_t n_feat,
+                            int32_t col_lo = 0, const int64_t* sub_start = nullptr, const int64_t* sub_cnt = nullptr) {
+    sqb_ctx* c = h->ctx;
+    const int64_t rows = layout == 0 ? n_feat : h->n, nnz = xp[rows];
+    DevBuf<int64_t> d_ptr(c->stream);
+    DevBuf<int32_t> d_idx(c->stream);
+    DevBuf<XT> d_val(c->stream);
+    SQB_TRY(d_ptr.alloc(rows + 1));
+    SQB_TRY(d_idx.alloc(nnz));
+    SQB_TRY(d_val.alloc(nnz));
+    SQB_CUDA(cudaMemcpyAsync(d_ptr.p, xp, (rows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+    if (nnz > 0) {  // a failed upload is reported as SQB_ERR_CUDA, whatever the copy returned
+        const bool failed = sub_start ? sqb_h2d_gather(c, d_idx.p, xi, sizeof(int32_t), sub_start, sub_cnt, xp, rows) ||
+                                            sqb_h2d_gather(c, d_val.p, xv, sizeof(XT), sub_start, sub_cnt, xp, rows)
+                                      : sqb_h2d(c, d_idx.p, xi, nnz * sizeof(int32_t)) || sqb_h2d(c, d_val.p, xv, (size_t)nnz * sizeof(XT));
+        if (failed) return SQB_ERR_CUDA;
     }
+    std::vector<int32_t> inv(layout == 0 ? n_feat : 0);  // layout 0: every row is a feature, in order
+    for (int64_t k = 0; k < (int64_t)inv.size(); ++k) inv[k] = (int32_t)k;
+    return ac_relayout_csr<int64_t, int32_t, XT, XT>(h, d_ptr.p, d_idx.p, d_val.p, layout, n_feat, nullptr, col_lo, inv, n_feat,
+                                                     "sqb_autocorr_load_csr");
 }
+
+// The value type of the loaded X: float32 stays float32, everything else becomes float64 (the host path's dtype rule).
+template <typename VT>
+using AcX = std::conditional_t<std::is_same<VT, float>::value, float, double>;
 
 template <typename VT, typename XT>
 static int ac_gather_dense(sqb_autocorr* h, const void* x, int64_t n_out, int64_t s_obs, int64_t s_feat, const int32_t* d_inv,
@@ -1452,9 +1346,9 @@ int sqb_autocorr_load_csr(sqb_autocorr* h, const int64_t* x_indptr, const int32_
     // index range, indptr monotonicity and duplicate observations are checked on the device while the matrix is
     // re-laid out (no host pass over the non-zeros)
     if (x_dtype == 0)
-        SQB_TRY(ac_load_csr_typed<float>(h, x_indptr, x_indices, x_data, layout, n_features, nnz));
+        SQB_TRY(ac_load_csr_host<float>(h, x_indptr, x_indices, x_data, layout, n_features));
     else
-        SQB_TRY(ac_load_csr_typed<double>(h, x_indptr, x_indices, x_data, layout, n_features, nnz));
+        SQB_TRY(ac_load_csr_host<double>(h, x_indptr, x_indices, x_data, layout, n_features));
     h->kind = 3;
     h->x_dtype = x_dtype;
     h->n_feat = n_features;
@@ -1510,9 +1404,9 @@ int sqb_autocorr_load_csr_cols(sqb_autocorr* h, const int64_t* x_indptr, const i
     // duplicate) while it re-lays the slice out
     const int64_t nf = col_hi - col_lo;
     if (x_dtype == 0)
-        SQB_TRY(ac_load_csr_typed<float>(h, ptr.data(), x_indices, x_data, 1, nf, ptr[n], (int32_t)col_lo, start.data(), cnt.data()));
+        SQB_TRY(ac_load_csr_host<float>(h, ptr.data(), x_indices, x_data, 1, nf, (int32_t)col_lo, start.data(), cnt.data()));
     else
-        SQB_TRY(ac_load_csr_typed<double>(h, ptr.data(), x_indices, x_data, 1, nf, ptr[n], (int32_t)col_lo, start.data(), cnt.data()));
+        SQB_TRY(ac_load_csr_host<double>(h, ptr.data(), x_indices, x_data, 1, nf, (int32_t)col_lo, start.data(), cnt.data()));
     h->kind = 3;
     h->x_dtype = x_dtype;
     h->n_feat = nf;
@@ -1524,27 +1418,25 @@ int sqb_autocorr_load_csr_device(sqb_autocorr* h, const void* indptr, int indptr
                                  uintptr_t producer_stream) {
     static const char* where = "sqb_autocorr_load_csr_device";
     SQB_CHECK(h && indptr && col_map, SQB_ERR_INVALID, "%s: null argument", where);
-    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
-              "%s: indptr_bits / index_bits must be 32 or 64", where);
-    SQB_CHECK(data_dtype >= 0 && data_dtype <= 4, SQB_ERR_INVALID, "%s: data_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32) or 4 (i64)",
-              where);
     SQB_CHECK(layout == 0 || layout == 1, SQB_ERR_INVALID, "%s: layout must be 0 or 1", where);
     std::vector<int32_t> inv;
     SQB_TRY(ac_invert_col_map(col_map, n_cols, n_out, inv, where));
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    SQB_TRY(sqb_wait_producer(c, producer_stream));
     h->kind = 0;
     h->aux_valid = false;
     h->ran = false;
-    int rc;
-    if (indptr_bits == 32)
-        rc = index_bits == 32 ? ac_load_csr_device_v<int32_t, int32_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out)
-                              : ac_load_csr_device_v<int32_t, int64_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out);
-    else
-        rc = index_bits == 32 ? ac_load_csr_device_v<int64_t, int32_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out)
-                              : ac_load_csr_device_v<int64_t, int64_t>(h, indptr, indices, data, data_dtype, layout, n_cols, col_map, inv, n_out);
-    SQB_TRY(rc);
+    SQB_TRY(sqb_read_caller_buffers(c, producer_stream, [&] {
+        return sqb_dispatch_index(indptr_bits, index_bits, where, [&](auto ipt, auto ixt) {
+            using IP = typename decltype(ipt)::type;
+            using II = typename decltype(ixt)::type;
+            return sqb_dispatch_value(data_dtype, where, "data_dtype", [&](auto vt) {
+                using VT = typename decltype(vt)::type;
+                return ac_relayout_csr<IP, II, VT, AcX<VT>>(h, (const IP*)indptr, (const II*)indices, (const VT*)data, layout, n_cols, col_map, 0,
+                                                            inv, n_out, where);
+            });
+        });
+    }));
     h->kind = 3;
     h->x_dtype = data_dtype == 0 ? 0 : 1;
     h->n_feat = n_out;
@@ -1555,7 +1447,6 @@ int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, 
                                    int64_t stride_col, int layout, const int32_t* col_map, int64_t n_out, uintptr_t producer_stream) {
     static const char* where = "sqb_autocorr_load_dense_device";
     SQB_CHECK(h && x && col_map, SQB_ERR_INVALID, "%s: null argument", where);
-    SQB_CHECK(x_dtype >= 0 && x_dtype <= 4, SQB_ERR_INVALID, "%s: x_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32) or 4 (i64)", where);
     SQB_CHECK(layout == 0 || layout == 1, SQB_ERR_INVALID, "%s: layout must be 0 or 1", where);
     const int64_t n_obs = layout == 1 ? rows : cols, n_cols = layout == 1 ? cols : rows;
     SQB_CHECK(n_obs == h->n, SQB_ERR_INVALID, "%s: expected %lld observations, found %lld", where, (long long)h->n, (long long)n_obs);
@@ -1564,7 +1455,6 @@ int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, 
     SQB_TRY(ac_invert_col_map(col_map, n_cols, n_out, inv, where));
     sqb_ctx* c = h->ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    SQB_TRY(sqb_wait_producer(c, producer_stream));
     h->kind = 0;
     h->aux_valid = false;
     h->ran = false;
@@ -1574,20 +1464,15 @@ int sqb_autocorr_load_dense_device(sqb_autocorr* h, const void* x, int x_dtype, 
     SQB_TRY(h->d_out.alloc((size_t)n_out));
     DevBuf<int32_t> map(c->stream);
     SQB_TRY(map.alloc(n_out));
-    auto gather = [&]() -> int {
+    SQB_TRY(sqb_read_caller_buffers(c, producer_stream, [&]() -> int {
         SQB_CUDA(cudaMemcpyAsync(map.p, inv.data(), n_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-        switch (x_dtype) {
-            case 0: return ac_gather_dense<float, float>(h, x, n_out, s_obs, s_feat, map.p, layout);
-            case 1: return ac_gather_dense<double, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
-            case 2: return ac_gather_dense<__half, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
-            case 3: return ac_gather_dense<int32_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
-            default: return ac_gather_dense<int64_t, double>(h, x, n_out, s_obs, s_feat, map.p, layout);
-        }
-    };
-    const int rc = gather();
-    const cudaError_t e = cudaStreamSynchronize(c->stream);  // the caller's buffer is no longer read
-    SQB_TRY(rc);
-    SQB_CUDA(e);
+        SQB_TRY(sqb_dispatch_value(x_dtype, where, "x_dtype", [&](auto vt) {
+            using VT = typename decltype(vt)::type;
+            return ac_gather_dense<VT, AcX<VT>>(h, x, n_out, s_obs, s_feat, map.p, layout);
+        }));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffer is no longer read
+        return SQB_OK;
+    }));
     h->kind = layout == 0 ? 1 : 2;
     h->x_dtype = xt;
     h->n_feat = n_out;

@@ -1,5 +1,6 @@
 // common.cuh — shared host/device plumbing for libsquidpy_b200 (sm_90a only).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -7,6 +8,7 @@
 
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/squidpy_b200.h"
@@ -207,4 +209,85 @@ __global__ void sqb_check_indptr_kernel(const IP* __restrict__ ptr, int64_t n, i
 static inline unsigned sqb_grid_rows(const sqb_ctx* c, int64_t rows, int threads) {
     const int64_t b = ceil_div64(rows, threads), cap = (int64_t)c->sm_count * 8;
     return (unsigned)(b < 1 ? 1 : b > cap ? cap : b);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Caller arrays in device memory (the *_device entry points): the ABI's type codes, the indptr check, and the way out of an
+// entry point that reads them.
+// ---------------------------------------------------------------------------------------------
+// A stored value in the type XT a kernel works in: float16 goes through float32 (exact), the one-byte bool of interaction
+// graphs is 1 for any non-zero byte, everything else is a plain conversion (int64 rounds to nearest, like numpy's astype).
+template <typename XT, typename VT>
+__device__ __forceinline__ XT sqb_cvt(VT v) {
+    if constexpr (std::is_same<VT, __half>::value)
+        return (XT)__half2float(v);
+    else if constexpr (std::is_same<VT, uint8_t>::value)
+        return v != 0 ? (XT)1 : (XT)0;
+    else
+        return (XT)v;
+}
+
+// The type a dispatch below hands to its callback: SqbType<T>::type.
+template <typename T>
+struct SqbType {
+    using type = T;
+};
+
+// indptr_bits / index_bits of a caller's CSR (32 or 64 each) -> f(SqbType<IP>(), SqbType<II>()), IP / II int32_t or int64_t.
+template <typename F>
+int sqb_dispatch_index(int indptr_bits, int index_bits, const char* where, F&& f) {
+    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
+              "%s: indptr_bits / index_bits must be 32 or 64", where);
+    const auto with_ip = [&](auto ip) { return index_bits == 32 ? f(ip, SqbType<int32_t>()) : f(ip, SqbType<int64_t>()); };
+    return indptr_bits == 64 ? with_ip(SqbType<int64_t>()) : with_ip(SqbType<int32_t>());
+}
+
+// The value dtype code of the ABI (DTYPE_CODES of _device.py: 0 f32, 1 f64, 2 f16, 3 i32, 4 i64) -> f(SqbType<VT>()).
+// WITH_BOOL adds code 5, the one-byte bool of interaction graphs; callers without it compile no bool instances.
+// name: the code's argument name in the error message.
+template <bool WITH_BOOL = false, typename F>
+int sqb_dispatch_value(int code, const char* where, const char* name, F&& f) {
+    switch (code) {
+        case 0: return f(SqbType<float>());
+        case 1: return f(SqbType<double>());
+        case 2: return f(SqbType<__half>());
+        case 3: return f(SqbType<int32_t>());
+        case 4: return f(SqbType<int64_t>());
+    }
+    if constexpr (WITH_BOOL)
+        if (code == 5) return f(SqbType<uint8_t>());
+    sqb_set_error("%s: %s must be 0 (f32), 1 (f64), 2 (f16), 3 (i32)%s", where, name, WITH_BOOL ? ", 4 (i64) or 5 (bool)" : " or 4 (i64)");
+    return SQB_ERR_INVALID;
+}
+
+// Checks a caller's indptr (n + 1 entries) against nnz with sqb_check_indptr_kernel and reads the verdict back (one
+// synchronisation): SQB_ERR_INVALID unless it runs from 0 to nnz without decreasing.  Kernels that follow indptr may run
+// only after SQB_OK.  dst (or null) receives the kernel's uint32 copy; kclass is the launch's class.
+template <typename IP>
+int sqb_check_indptr(sqb_ctx* c, int kclass, const IP* ptr, int64_t n, int64_t nnz, uint32_t* dst, const char* where) {
+    DevBuf<unsigned> err(c->stream);
+    SQB_TRY(err.alloc(1));
+    SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), c->stream));
+    {
+        SqbLaunchScope scope(c, kclass);
+        sqb_check_indptr_kernel<IP><<<sqb_grid_rows(c, n + 1, 256), 256, 0, c->stream>>>(ptr, n, nnz, dst, err.p);
+        SQB_POST_LAUNCH();
+    }
+    unsigned flag = 0;
+    SQB_CUDA(cudaMemcpyAsync(&flag, err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    SQB_CHECK(flag == 0, SQB_ERR_INVALID, "%s: indptr inconsistent with nnz=%lld (it must run from 0 to nnz without decreasing)", where,
+              (long long)nnz);
+    return SQB_OK;
+}
+
+// Runs body() for an entry point that reads caller-owned device buffers: the context's stream first waits for the caller's
+// producer stream (sqb_wait_producer; 0: none), and when body fails the stream is synchronised, so that the caller's buffers
+// are no longer read when the entry point returns.  body synchronises on its own way to success.
+template <typename F>
+int sqb_read_caller_buffers(sqb_ctx* c, uintptr_t producer, F&& body) {
+    SQB_TRY(sqb_wait_producer(c, producer));
+    const int rc = body();
+    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);  // the caller's buffers are no longer read
+    return rc;
 }

@@ -15,14 +15,13 @@
 // sum per (cluster, gene) in cell order, whose NaN compensation is reset (so +-inf inputs give +-inf), divided by the count
 // — plus the number of positive values (the expression-fraction mask).  Lane = gene, cells walked in order, accumulators
 // [cluster][lane] in shared memory; __dadd_rn / __dsub_rn / __ddiv_rn keep the compiler from contracting or reassociating.
-#include <cuda_fp16.h>
 #include <math.h>
 
 #include "common.cuh"
 
 namespace {
 
-enum { DG_ERR_INDPTR = 1u, DG_ERR_INDEX = 2u, DG_ERR_DUP = 4u };
+enum { DG_ERR_INDEX = 2u, DG_ERR_DUP = 4u };
 
 template <typename T>
 __device__ __forceinline__ T dg_nan0(T v) { return v; }  // integers have no NaN
@@ -30,19 +29,13 @@ __device__ __forceinline__ float dg_nan0(float v) { return v != v ? 0.0f : v; }
 __device__ __forceinline__ double dg_nan0(double v) { return v != v ? 0.0 : v; }
 __device__ __forceinline__ __half dg_nan0(__half v) { return __hisnan(v) ? __float2half(0.0f) : v; }
 
-__device__ __forceinline__ double dg_f64(float v) { return (double)v; }
-__device__ __forceinline__ double dg_f64(double v) { return v; }
-__device__ __forceinline__ double dg_f64(__half v) { return (double)__half2float(v); }
-__device__ __forceinline__ double dg_f64(int32_t v) { return (double)v; }
-__device__ __forceinline__ double dg_f64(int64_t v) { return (double)v; }  // round to nearest, like numpy's astype
-
 template <typename VT>
 __device__ __forceinline__ void dg_store(void* out, int64_t cell, VT v, bool nan0, bool keep) {
     if (nan0) v = dg_nan0(v);
     if (keep)
         reinterpret_cast<VT*>(out)[cell] = v;
     else
-        reinterpret_cast<double*>(out)[cell] = dg_f64(v);
+        reinterpret_cast<double*>(out)[cell] = sqb_cvt<double>(v);
 }
 
 // CSR (major = observations) or CSC (major = genes): one warp per selected major segment.  maj_map / min_map: the output index
@@ -95,29 +88,6 @@ __global__ void __launch_bounds__(256, 1) dg_dense_kernel(const VT* __restrict__
     }
 }
 
-template <typename IP, typename II>
-int dg_sparse_launch(sqb_ctx* c, const void* indptr, const void* indices, const void* vals, int x_dtype, int64_t n_major, int64_t n_minor,
-                     const int32_t* maj_map, const int32_t* min_map, int csr, sqb_dense* d, int nan0, int keep, unsigned* bitmap, unsigned* err) {
-    const unsigned grid = sqb_grid_rows(c, n_major * 32, 256);
-    const IP* ip = reinterpret_cast<const IP*>(indptr);
-    const II* ix = reinterpret_cast<const II*>(indices);
-    SqbLaunchScope scope(c, SQB_K_MISC);
-#define SQB_DG(VT)                                                                                                                  \
-    dg_sparse_kernel<IP, II, VT><<<grid, 256, 0, c->stream>>>(ip, ix, reinterpret_cast<const VT*>(vals), n_major, n_minor, maj_map,  \
-                                                              min_map, csr, d->layout, d->n_obs, d->n_genes, nan0, keep, d->buf.p, \
-                                                              bitmap, err)
-    switch (x_dtype) {
-        case 0: SQB_DG(float); break;
-        case 1: SQB_DG(double); break;
-        case 2: SQB_DG(__half); break;
-        case 3: SQB_DG(int32_t); break;
-        default: SQB_DG(int64_t); break;
-    }
-#undef SQB_DG
-    SQB_POST_LAUNCH();
-    return SQB_OK;
-}
-
 const size_t kDtypeSize[5] = {4, 8, 2, 4, 8};
 
 }  // namespace
@@ -164,7 +134,6 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
     static const char* where = "sqb_dense_gather_device";
     SQB_CHECK(ctx && out && cols && (x || (format != 0 && nnz == 0)), SQB_ERR_INVALID, "%s: null argument", where);
     SQB_CHECK(format >= 0 && format <= 2, SQB_ERR_INVALID, "%s: format must be 0 (dense), 1 (CSR) or 2 (CSC)", where);
-    SQB_CHECK(x_dtype >= 0 && x_dtype <= 4, SQB_ERR_INVALID, "%s: x_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32) or 4 (i64)", where);
     SQB_CHECK(layout == 0 || layout == 1, SQB_ERR_INVALID, "%s: layout must be 0 or 1", where);
     SQB_CHECK((flags & ~3) == 0, SQB_ERR_INVALID, "%s: unknown flags %d", where, flags);
     SQB_CHECK(n_rows >= 1 && n_rows < 2147483647LL && n_cols >= 1 && n_cols < 2147483647LL, SQB_ERR_INVALID, "%s: bad shape (%lld, %lld)",
@@ -175,8 +144,6 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
               (long long)n_cols);
     if (format != 0) {
         SQB_CHECK(indptr && (indices || nnz == 0), SQB_ERR_INVALID, "%s: null sparse arrays", where);
-        SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
-                  "%s: indptr_bits / index_bits must be 32 or 64", where);
         SQB_CHECK(nnz >= 0, SQB_ERR_INVALID, "%s: nnz=%lld", where, (long long)nnz);
     }
     // row / column maps on the host: input index -> output index or -1
@@ -201,7 +168,6 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
     }
     sqb_ctx* c = ctx;
     SQB_CUDA(cudaSetDevice(c->device));
-    SQB_TRY(sqb_wait_producer(c, producer_stream));
     const bool keep = flags & 2, nan0 = flags & 1;
     std::unique_ptr<sqb_dense> d(new sqb_dense(c));
     d->n_obs = n_rows_out, d->n_genes = n_cols_out, d->layout = layout, d->dtype = keep ? x_dtype : 1, d->nan_zero = nan0;
@@ -210,7 +176,8 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
     DevBuf<int64_t> d_rlist(c->stream);
     DevBuf<unsigned> d_bits(c->stream), d_err(c->stream);
     unsigned flag = 0;
-    auto body = [&]() -> int {
+    auto gather = [&](auto vt) -> int {
+        using VT = typename decltype(vt)::type;
         SQB_TRY(d->buf.alloc((size_t)cells * kDtypeSize[d->dtype]));
         SQB_TRY(d_cmap.alloc(format == 0 ? n_cols_out : n_cols));
         if (format == 0) {
@@ -218,18 +185,9 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
             SQB_CUDA(cudaMemcpyAsync(d_cmap.p, cols, n_cols_out * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
             SQB_CUDA(cudaMemcpyAsync(d_rlist.p, rlist.data(), n_rows_out * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
             SqbLaunchScope scope(c, SQB_K_MISC);
-            const unsigned grid = sqb_grid_rows(c, cells, 256);
-#define SQB_DGD(VT)                                                                                                              \
-    dg_dense_kernel<VT><<<grid, 256, 0, c->stream>>>(reinterpret_cast<const VT*>(x), stride_row, stride_col, d_rlist.p, d_cmap.p, \
-                                                     layout, n_rows_out, n_cols_out, nan0, keep, d->buf.p)
-            switch (x_dtype) {
-                case 0: SQB_DGD(float); break;
-                case 1: SQB_DGD(double); break;
-                case 2: SQB_DGD(__half); break;
-                case 3: SQB_DGD(int32_t); break;
-                default: SQB_DGD(int64_t); break;
-            }
-#undef SQB_DGD
+            dg_dense_kernel<VT><<<sqb_grid_rows(c, cells, 256), 256, 0, c->stream>>>(reinterpret_cast<const VT*>(x), stride_row, stride_col,
+                                                                                     d_rlist.p, d_cmap.p, layout, n_rows_out, n_cols_out,
+                                                                                     nan0, keep, d->buf.p);
             SQB_POST_LAUNCH();
             SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffer is no longer read
             return SQB_OK;
@@ -244,31 +202,18 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
         SQB_CUDA(cudaMemsetAsync(d->buf.p, 0, (size_t)cells * kDtypeSize[d->dtype], c->stream));
         SQB_CUDA(cudaMemsetAsync(d_bits.p, 0, (size_t)ceil_div64(cells, 32) * sizeof(unsigned), c->stream));
         SQB_CUDA(cudaMemsetAsync(d_err.p, 0, sizeof(unsigned), c->stream));
-        // indptr first (one synchronisation): the gather follows it
-        {
+        SQB_TRY(sqb_dispatch_index(indptr_bits, index_bits, where, [&](auto ipt, auto ixt) -> int {
+            using IP = typename decltype(ipt)::type;
+            using II = typename decltype(ixt)::type;
+            const IP* ip = reinterpret_cast<const IP*>(indptr);
+            SQB_TRY(sqb_check_indptr(c, SQB_K_MISC, ip, n_major, nnz, nullptr, where));  // the gather follows it
             SqbLaunchScope scope(c, SQB_K_MISC);
-            if (indptr_bits == 32)
-                sqb_check_indptr_kernel<int32_t><<<sqb_grid_rows(c, n_major + 1, 256), 256, 0, c->stream>>>(
-                    reinterpret_cast<const int32_t*>(indptr), n_major, nnz, nullptr, d_err.p);
-            else
-                sqb_check_indptr_kernel<int64_t><<<sqb_grid_rows(c, n_major + 1, 256), 256, 0, c->stream>>>(
-                    reinterpret_cast<const int64_t*>(indptr), n_major, nnz, nullptr, d_err.p);
+            dg_sparse_kernel<IP, II, VT><<<sqb_grid_rows(c, n_major * 32, 256), 256, 0, c->stream>>>(
+                ip, reinterpret_cast<const II*>(indices), reinterpret_cast<const VT*>(x), n_major, n_minor, csr ? d_rmap.p : d_cmap.p,
+                csr ? d_cmap.p : d_rmap.p, csr, layout, n_rows_out, n_cols_out, nan0, keep, d->buf.p, d_bits.p, d_err.p);
             SQB_POST_LAUNCH();
-        }
-        SQB_CUDA(cudaMemcpyAsync(&flag, d_err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
-        SQB_CUDA(cudaStreamSynchronize(c->stream));
-        SQB_CHECK(flag == 0, SQB_ERR_INVALID, "%s: indptr inconsistent with nnz=%lld (it must run from 0 to nnz without decreasing)", where,
-                  (long long)nnz);
-        const int32_t* maj = csr ? d_rmap.p : d_cmap.p;
-        const int32_t* mnr = csr ? d_cmap.p : d_rmap.p;
-        int rc;
-        if (indptr_bits == 32)
-            rc = index_bits == 32 ? dg_sparse_launch<int32_t, int32_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p)
-                                  : dg_sparse_launch<int32_t, int64_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p);
-        else
-            rc = index_bits == 32 ? dg_sparse_launch<int64_t, int32_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p)
-                                  : dg_sparse_launch<int64_t, int64_t>(c, indptr, indices, x, x_dtype, n_major, n_minor, maj, mnr, csr, d.get(), nan0, keep, d_bits.p, d_err.p);
-        SQB_TRY(rc);
+            return SQB_OK;
+        }));
         SQB_CUDA(cudaMemcpyAsync(&flag, d_err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
         SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffers are no longer read
         SQB_CHECK(!(flag & DG_ERR_INDEX), SQB_ERR_INVALID, "%s: index out of range [0, %lld)", where, (long long)n_minor);
@@ -278,11 +223,7 @@ int sqb_dense_gather_device(sqb_ctx* ctx, int format, const void* x, const void*
                   where);
         return SQB_OK;
     };
-    const int rc = body();
-    if (rc != SQB_OK) {
-        cudaStreamSynchronize(c->stream);  // the caller's buffers are no longer read
-        return rc;
-    }
+    SQB_TRY(sqb_read_caller_buffers(c, producer_stream, [&] { return sqb_dispatch_value(x_dtype, where, "x_dtype", gather); }));
     *out = d.release();
     return SQB_OK;
 }

@@ -7,17 +7,7 @@
 //   weights = true : out[a][b] = sum of their values, accumulated in float64                             (order free:
 //                    exact for integer-valued weights, |rel err| ~1e-16 * entries otherwise)
 // HBM-bound: the CSR is streamed once (8-12 bytes per stored entry); the label gather hits L2.
-#include <cuda_fp16.h>
-
 #include "common.cuh"
-
-// value of a stored entry as float64 (float16 through float32: exact; bool arrives as one byte, any non-zero byte is true)
-__device__ __forceinline__ double inter_f64(float v) { return (double)v; }
-__device__ __forceinline__ double inter_f64(double v) { return v; }
-__device__ __forceinline__ double inter_f64(__half v) { return (double)__half2float(v); }
-__device__ __forceinline__ double inter_f64(int32_t v) { return (double)v; }
-__device__ __forceinline__ double inter_f64(int64_t v) { return (double)v; }
-__device__ __forceinline__ double inter_f64(uint8_t v) { return v != 0 ? 1.0 : 0.0; }
 
 // IP / II: index types of indptr / indices (uint32 for the host path's staged copy, int32 / int64 for a caller's device
 // CSR read in place).  A column index outside [0, n) is skipped and raises bit 2 of *err (null: host input, validated on
@@ -63,7 +53,7 @@ __global__ void __launch_bounds__(256) interaction_kernel(const IP* __restrict__
             if ((unsigned)b >= (unsigned)C) continue;  // no label (< 0); >= C is flagged by row j
             const int bin = a * C + b;
             if (WEIGHTED) {
-                const double v = inter_f64(data[e]);
+                const double v = sqb_cvt<double>(data[e]);
                 if (use_smem)
                     atomicAdd(&s_w[bin], v);
                 else
@@ -169,33 +159,19 @@ static int inter_device_typed(sqb_ctx* c, int64_t n, int64_t nnz, const void* in
     static const char* where = "sqb_interaction_matrix_device";
     const IP* ip = reinterpret_cast<const IP*>(indptr);
     const II* ix = reinterpret_cast<const II*>(indices);
-    unsigned flag = 0;
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        sqb_check_indptr_kernel<IP><<<sqb_grid_rows(c, n + 1, 256), 256, 0, c->stream>>>(ip, n, nnz, nullptr, d_err);
-        SQB_POST_LAUNCH();
-    }
-    SQB_CUDA(cudaMemcpyAsync(&flag, d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
-    SQB_CUDA(cudaStreamSynchronize(c->stream));
-    SQB_CHECK(flag == 0, SQB_ERR_INVALID, "%s: indptr inconsistent with nnz=%lld (it must run from 0 to nnz without decreasing)", where,
-              (long long)nnz);
+    SQB_TRY(sqb_check_indptr(c, SQB_K_MISC, ip, n, nnz, nullptr, where));
     const InterLaunch L(c, n, n_cls);
     double* ow = reinterpret_cast<double*>(d_out);
-    SqbLaunchScope scope(c, SQB_K_MISC);
-#define SQB_INTER(VT, W) \
-    interaction_kernel<IP, II, VT, W><<<L.blocks, 256, L.smem, c->stream>>>(ip, ix, reinterpret_cast<const VT*>(data), d_codes, n, n_cls, L.use_smem, ow, d_out, d_err)
-    if (!weighted) SQB_INTER(float, false);
-    else switch (data_dtype) {
-        case 0: SQB_INTER(float, true); break;
-        case 1: SQB_INTER(double, true); break;
-        case 2: SQB_INTER(__half, true); break;
-        case 3: SQB_INTER(int32_t, true); break;
-        case 4: SQB_INTER(int64_t, true); break;
-        default: SQB_INTER(uint8_t, true); break;
-    }
-#undef SQB_INTER
-    SQB_POST_LAUNCH();
-    return SQB_OK;
+    auto launch = [&](auto vt, auto w) -> int {
+        using VT = typename decltype(vt)::type;
+        SqbLaunchScope scope(c, SQB_K_MISC);
+        interaction_kernel<IP, II, VT, decltype(w)::value><<<L.blocks, 256, L.smem, c->stream>>>(
+            ip, ix, reinterpret_cast<const VT*>(data), d_codes, n, n_cls, L.use_smem, ow, d_out, d_err);
+        SQB_POST_LAUNCH();
+        return SQB_OK;
+    };
+    if (!weighted) return launch(SqbType<float>(), std::false_type());
+    return sqb_dispatch_value<true>(data_dtype, where, "data_dtype", [&](auto vt) { return launch(vt, std::true_type()); });
 }
 
 extern "C" int sqb_interaction_matrix_device(sqb_ctx* c, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
@@ -205,44 +181,32 @@ extern "C" int sqb_interaction_matrix_device(sqb_ctx* c, int64_t n, int64_t nnz,
     SQB_CHECK(c, SQB_ERR_INVALID, "%s: null ctx", where);
     SQB_CHECK(n >= 1 && n < 0x7FFFFFFFLL, SQB_ERR_INVALID, "%s: n=%lld out of range", where, (long long)n);
     SQB_CHECK(nnz >= 0 && nnz < 0xFFFFFFFFLL, SQB_ERR_INVALID, "%s: nnz=%lld does not fit uint32", where, (long long)nnz);
-    SQB_CHECK(indptr && (indices || nnz == 0) && codes, SQB_ERR_INVALID, "%s: null argument", where);
-    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
-              "%s: indptr_bits / index_bits must be 32 or 64", where);
-    SQB_CHECK(n_cls >= 1 && n_cls <= 4096, SQB_ERR_INVALID, "%s: n_cls=%d out of range [1, 4096]", where, n_cls);
     const bool weighted = out_weighted != nullptr;  // data may be null only when there are no entries
-    SQB_CHECK(!weighted || ((data || nnz == 0) && data_dtype >= 0 && data_dtype <= 5), SQB_ERR_INVALID,
-              "%s: data_dtype must be 0 (f32), 1 (f64), 2 (f16), 3 (i32), 4 (i64) or 5 (bool)", where);
+    SQB_CHECK(indptr && (indices || nnz == 0) && codes && (!weighted || data || nnz == 0), SQB_ERR_INVALID, "%s: null argument", where);
+    SQB_CHECK(n_cls >= 1 && n_cls <= 4096, SQB_ERR_INVALID, "%s: n_cls=%d out of range [1, 4096]", where, n_cls);
     SQB_CHECK(weighted || out_counts != nullptr, SQB_ERR_INVALID, "%s: null output", where);
     SQB_CUDA(cudaSetDevice(c->device));
-    SQB_TRY(sqb_wait_producer(c, producer_stream));
     const int CC = n_cls * n_cls;
     DevBuf<int32_t> d_codes(c->stream);
     DevBuf<unsigned long long> d_out(c->stream);  // 8 bytes per bin: double or uint64
     DevBuf<unsigned> d_err(c->stream);
     unsigned flag = 0;
-    auto body = [&]() -> int {
+    return sqb_read_caller_buffers(c, producer_stream, [&]() -> int {
         SQB_TRY(d_codes.alloc(n));
         SQB_TRY(d_out.alloc(CC));
         SQB_TRY(d_err.alloc(1));
         SQB_CUDA(cudaMemcpyAsync(d_codes.p, codes, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
         SQB_CUDA(cudaMemsetAsync(d_out.p, 0, (size_t)CC * 8, c->stream));
         SQB_CUDA(cudaMemsetAsync(d_err.p, 0, sizeof(unsigned), c->stream));
-        int rc;
-        if (indptr_bits == 32)
-            rc = index_bits == 32 ? inter_device_typed<int32_t, int32_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p)
-                                  : inter_device_typed<int32_t, int64_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p);
-        else
-            rc = index_bits == 32 ? inter_device_typed<int64_t, int32_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p)
-                                  : inter_device_typed<int64_t, int64_t>(c, n, nnz, indptr, indices, weighted, data, data_dtype, d_codes.p, n_cls, d_out.p, d_err.p);
-        SQB_TRY(rc);
+        SQB_TRY(sqb_dispatch_index(indptr_bits, index_bits, where, [&](auto ip, auto ix) {
+            return inter_device_typed<typename decltype(ip)::type, typename decltype(ix)::type>(c, n, nnz, indptr, indices, weighted, data,
+                                                                                                data_dtype, d_codes.p, n_cls, d_out.p, d_err.p);
+        }));
         SQB_CUDA(cudaMemcpyAsync(weighted ? (void*)out_weighted : (void*)out_counts, d_out.p, (size_t)CC * 8, cudaMemcpyDeviceToHost, c->stream));
         SQB_CUDA(cudaMemcpyAsync(&flag, d_err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
         SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffers are no longer read
         SQB_CHECK(!(flag & 2u), SQB_ERR_INVALID, "%s: column index out of range [0, %lld)", where, (long long)n);
         SQB_CHECK(!(flag & 4u), SQB_ERR_INVALID, "%s: a code is >= n_cls=%d", where, n_cls);
         return SQB_OK;
-    };
-    const int rc = body();
-    if (rc != SQB_OK) cudaStreamSynchronize(c->stream);  // the caller's buffers are no longer read
-    return rc;
+    });
 }

@@ -3108,27 +3108,17 @@ __global__ void nhood_cvt_indices_kernel(const II* __restrict__ src, int64_t nnz
     }
 }
 
+// The indices are converted first: the indptr check's synchronisation then ends every read of the caller's buffers.
 template <typename IP, typename II>
-static int nhood_fill_device(sqb_nhood* h, const void* indptr, const void* indices, unsigned* d_err) {
+static int nhood_fill_device(sqb_nhood* h, const void* indptr, const void* indices) {
     sqb_ctx* ctx = h->ctx;
-    unsigned flag = 0;
-    {
-        SqbLaunchScope scope(ctx, SQB_K_NHOOD_FILL);
-        sqb_check_indptr_kernel<IP><<<sqb_grid_rows(ctx, h->n + 1, 256), 256, 0, ctx->stream>>>(
-            reinterpret_cast<const IP*>(indptr), h->n, h->nnz, h->d_indptr.p, d_err);
-        SQB_POST_LAUNCH();
-    }
     if (h->nnz > 0) {
         SqbLaunchScope scope(ctx, SQB_K_NHOOD_FILL);
         nhood_cvt_indices_kernel<II><<<sqb_grid_rows(ctx, h->nnz, 256), 256, 0, ctx->stream>>>(reinterpret_cast<const II*>(indices), h->nnz,
                                                                                                h->n, h->d_indices.p);
         SQB_POST_LAUNCH();
     }
-    SQB_CUDA(cudaMemcpyAsync(&flag, d_err, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
-    SQB_CUDA(cudaStreamSynchronize(ctx->stream));  // the caller's buffers are no longer read
-    SQB_CHECK(flag == 0, SQB_ERR_INVALID, "sqb_nhood_create_device: indptr inconsistent with nnz=%lld (it must run from 0 to nnz without decreasing)",
-              (long long)h->nnz);
-    return SQB_OK;
+    return sqb_check_indptr(ctx, SQB_K_NHOOD_FILL, reinterpret_cast<const IP*>(indptr), h->n, h->nnz, h->d_indptr.p, "sqb_nhood_create_device");
 }
 
 extern "C" {
@@ -3156,27 +3146,14 @@ int sqb_nhood_create_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* in
     static const char* where = "sqb_nhood_create_device";
     SQB_TRY(nhood_check_args(where, ctx, n, nnz, n_cls, out));
     SQB_CHECK(indptr && (indices || nnz == 0), SQB_ERR_INVALID, "%s: null CSR arrays", where);
-    SQB_CHECK((indptr_bits == 32 || indptr_bits == 64) && (index_bits == 32 || index_bits == 64), SQB_ERR_INVALID,
-              "%s: indptr_bits / index_bits must be 32 or 64", where);
     SQB_CUDA(cudaSetDevice(ctx->device));
-    SQB_TRY(sqb_wait_producer(ctx, producer_stream));
     std::unique_ptr<sqb_nhood> h;
     SQB_TRY(nhood_new(ctx, n, nnz, n_cls, h));
-    auto body = [&]() -> int {
-        DevBuf<unsigned> err(ctx->stream);
-        SQB_TRY(err.alloc(1));
-        SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), ctx->stream));
-        if (indptr_bits == 32)
-            return index_bits == 32 ? nhood_fill_device<int32_t, int32_t>(h.get(), indptr, indices, err.p)
-                                    : nhood_fill_device<int32_t, int64_t>(h.get(), indptr, indices, err.p);
-        return index_bits == 32 ? nhood_fill_device<int64_t, int32_t>(h.get(), indptr, indices, err.p)
-                                : nhood_fill_device<int64_t, int64_t>(h.get(), indptr, indices, err.p);
-    };
-    const int rc = body();
-    if (rc != SQB_OK) {
-        cudaStreamSynchronize(ctx->stream);  // the caller's buffers are no longer read
-        return rc;
-    }
+    SQB_TRY(sqb_read_caller_buffers(ctx, producer_stream, [&] {
+        return sqb_dispatch_index(indptr_bits, index_bits, where, [&](auto ip, auto ix) {
+            return nhood_fill_device<typename decltype(ip)::type, typename decltype(ix)::type>(h.get(), indptr, indices);
+        });
+    }));
     // from here on the handle's own copy is all that is read: the chain of the host path
     SQB_TRY(nhood_prepare(h.get(), where));
     *out = h.release();

@@ -22,7 +22,7 @@ torch = pytest.importorskip("torch")
 import squidpy_b200 as sq  # noqa: E402
 from squidpy_b200 import AnnDataLite  # noqa: E402
 from squidpy_b200._lib import check, load  # noqa: E402
-from squidpy_b200.gr import GridBuilder, KNNBuilder, NhoodPlan, RadiusBuilder  # noqa: E402
+from squidpy_b200.gr import AutocorrPlan, GridBuilder, KNNBuilder, NhoodPlan, RadiusBuilder  # noqa: E402
 from tests.test_gpu_autocorr_device_input import CuSparse  # noqa: E402
 from tests.test_gpu_autocorr_device_input import _adata as _ac_adata  # noqa: E402
 from tests.test_gpu_autocorr_device_input import _corrupt as _ac_corrupt  # noqa: E402
@@ -193,9 +193,12 @@ def _sepal_indptr():
 
 def _autocorr_error(where, kind):
     """The invalid feature matrices of test_gpu_autocorr_device_input.test_invalid_input_raises_like_the_host_and_context_survives,
-    on the host (checked on the device while the matrix is re-laid out) and in device memory."""
+    on the host (checked on the device while the matrix is re-laid out) and in device memory.  where="host_by_feature": the
+    host CSR of features x observations, loaded as such (layout 0 of sqb_autocorr_load_csr)."""
     w = _w()
     x = _ac_x(w.shape[0], g=10, density=0.3)
+    if where == "host_by_feature":
+        x = x.T.tocsr()
     r = int(np.flatnonzero(np.diff(x.indptr) >= 2)[0])
     a = x.indptr[r]
     if kind == "duplicate":
@@ -204,13 +207,23 @@ def _autocorr_error(where, kind):
         arrays, match = {"indices": ix}, "stored twice"
     elif kind == "index_out_of_range":
         ix = x.indices.copy()
-        ix[a] = 10
+        ix[a] = x.shape[1]
         arrays, match = {"indices": ix}, "out of range"
     else:
         ip = x.indptr.copy()
         ip[r + 1] = ip[r] - 1 if ip[r] > 0 else ip[r + 2] + 1
         arrays, match = {"indptr": ip}, "indptr"
     host, dev = _ac_corrupt(x, **arrays)
+    if where == "host_by_feature":
+
+        def load():
+            plan = AutocorrPlan(w)
+            try:
+                plan.load(host, obs_major=False)
+            finally:
+                plan.close()
+
+        return _raises(ValueError, match, load)
     m = host if where == "host" else dev
     return _raises(ValueError, match, lambda: sq.gr.spatial_autocorr(_ac_adata(m, w, 10), copy=True))
 
@@ -255,7 +268,7 @@ CASES = {
     "ligrec_indptr": lambda: _ligrec_error("indptr"),
     "sepal_device_indptr": _sepal_indptr,
     **{f"autocorr_{where}_{kind}": (lambda where=where, kind=kind: _autocorr_error(where, kind))
-       for where in ("host", "device") for kind in ("duplicate", "index_out_of_range", "indptr")},
+       for where in ("host", "host_by_feature", "device") for kind in ("duplicate", "index_out_of_range", "indptr")},
 }
 
 

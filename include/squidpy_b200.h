@@ -27,6 +27,7 @@
  *   sqb_ligrec_observed        <- data.groupby("clusters").mean() / the expression-fraction mask of _analysis  src/squidpy/gr/_ligrec.py:679-700
  *   sqb_ligrec_counts_dense    <- _score_permutations on a gathered device matrix  src/squidpy/gr/_ligrec.py:616-676
  *   sqb_sepal_dense            <- _diffusion on a gathered device matrix  src/squidpy/gr/_sepal.py:186-233
+ *   sqb_nn_dist_hist_f64       <- NearestNeighbors(...).fit(ref).kneighbors(qry) + np.histogram  src/squidpy/gr/_ripley.py:140-150,160-169,206-209
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
  *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
@@ -41,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 7
+#define SQB_ABI_VERSION 8
 
 typedef enum {
     SQB_OK = 0,
@@ -316,6 +317,19 @@ int sqb_cooc_counts(sqb_ctx* ctx, const float* x, const float* y, int64_t n, con
  * i.e. sklearn KDTree.two_point_correlation(points_g, support).  support ascending.                        */
 int sqb_pair_counts_f64(sqb_ctx* ctx, const double* pts, const int64_t* group_ptr, int n_groups,
                         const double* support, int S, int shard_index, int shard_count, int64_t* out);
+
+/* ---- ripley F / G ----------------------------------------------------------------------------------------
+ * Histograms of nearest-neighbour distances (src/squidpy/gr/_ripley.py:140-150,160-169: kneighbors of a query set against a
+ * tree of a reference set, and :206-209: np.histogram of the distances).  pts: n_pts x 2 float64 point pool (interleaved x,y).
+ * tasks: n_tasks x 6 int64 {ref_begin, ref_end, qry_begin, qry_end, k, out_row}, ranges into the pool: the k nearest
+ * distances of every query point among the reference points (no point excluded: zero distances count) are binned into row
+ * out_row.  Distances are sqrt(dx*dx + dy*dy) in float64 without contraction (scikit-learn's kd_tree).  Binning is
+ * np.histogram(d, bins=support) for ascending support (S >= 2 edges): S - 1 bins, the last one closed, distances outside
+ * [support[0], support[S-1]] dropped.  out: n_rows x (S - 1) int64, the sums over the tasks of each row.  k in [1, 64] and
+ * k <= ref_end - ref_begin.  Query blocks of 1024 points, numbered over the tasks in order, are evaluated when
+ * block % shard_count == shard_index (multi-GPU sharding; pass 0,1 for everything); partial results add up across shards. */
+int sqb_nn_dist_hist_f64(sqb_ctx* ctx, const double* pts, int64_t n_pts, const int64_t* tasks, int64_t n_tasks,
+                         const double* support, int S, int n_rows, int shard_index, int shard_count, int64_t* out);
 
 /* ---- sepal ---------------------------------------------------------------------------------------------------------
  * `_diffusion` for every gene (src/squidpy/gr/_sepal.py:186-289): vals = n_genes x n float64 (one row per gene), sat / unsat =

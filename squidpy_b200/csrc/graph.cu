@@ -13,9 +13,14 @@
 // are gathered into cell order so that a query streams its 3x3 / 5x5 ... rings of cells from contiguous memory; one thread per
 // query, the k best (d2, index) pairs in registers.  The search of a point stops after ring r as soon as its k-th distance
 // is below r cells (nothing unseen can be closer).
+#include <algorithm>
+#include <cmath>
+#include <limits>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <map>
 #include <math.h>
+#include <vector>
 
 #include "graph.cuh"
 
@@ -52,21 +57,52 @@ __global__ void graph_gather_kernel(const double* __restrict__ xy, const uint32_
 }
 
 // ---- exact kNN -------------------------------------------------------------------------------------------------------
-template <int KMAX>
-__global__ void __launch_bounds__(128) graph_knn_kernel(const double2* __restrict__ pts, const int32_t* __restrict__ idx_sorted,
-                                                        const int32_t* __restrict__ cell_start, int64_t n, GridGeom gm, int k,
-                                                        int32_t* __restrict__ out_idx, double* __restrict__ out_dist) {
-    const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    const double2 q = pts[s];
-    const int32_t qi = idx_sorted[s];
+// Lower bound on the squared distance from q to every point of the grid outside the visited square of cells
+// [cx - r, cx + r] x [cy - r, cy + r]: the minimum over the square's sides that still have cells beyond them of (separation
+// along that axis)^2 + (distance from q to the grid box along the other axis)^2.  It holds for queries outside the box too
+// (their cell is clamped to the box), where r cells alone would be a loose bound.  Both terms are shrunk by a slack
+// proportional to the box's coordinates: the cell assignment of a point is a rounded computation.  Returns -1 when no cell
+// is left (the walk is complete).
+__device__ __forceinline__ double grid_unvisited_bound(const GridGeom gm, double2 q, int cx, int cy, int r) {
+    const double bx1 = gm.x0 + gm.gx * gm.cell, by1 = gm.y0 + gm.gy * gm.cell;
+    const double slack = 1e-12 * (fabs(gm.x0) + fabs(gm.y0) + fabs(bx1) + fabs(by1));
+    const double ox = fmax(fmax(gm.x0 - q.x, q.x - bx1) - slack, 0.0), oy = fmax(fmax(gm.y0 - q.y, q.y - by1) - slack, 0.0);
+    const double oy2 = __dmul_rn(oy, oy), ox2 = __dmul_rn(ox, ox);
+    double lb = INFINITY;
+    bool left = false;
+    if (cx + r + 1 < gm.gx) {
+        const double s = fmax(gm.x0 + (cx + r + 1) * gm.cell - q.x - slack, 0.0);
+        lb = fmin(lb, s * s + oy2), left = true;
+    }
+    if (cx - r - 1 >= 0) {
+        const double s = fmax(q.x - (gm.x0 + (cx - r) * gm.cell) - slack, 0.0);
+        lb = fmin(lb, s * s + oy2), left = true;
+    }
+    if (cy + r + 1 < gm.gy) {
+        const double s = fmax(gm.y0 + (cy + r + 1) * gm.cell - q.y - slack, 0.0);
+        lb = fmin(lb, s * s + ox2), left = true;
+    }
+    if (cy - r - 1 >= 0) {
+        const double s = fmax(q.y - (gm.y0 + (cy - r) * gm.cell) - slack, 0.0);
+        lb = fmin(lb, s * s + ox2), left = true;
+    }
+    return left ? lb : -1.0;
+}
+
+// The ring walk of the exact kNN searches: the k smallest d2 from q to the points of one grid (points pts[cell_start[c] ..
+// cell_start[c + 1]) of cell c) in bd[0 .. k), in DESCENDING order: bd[0] is the k-th smallest, so the list is only ever read at
+// constant indices and stays in registers.  BY_INDEX (graph search): the point with index qi is skipped and ties at the k-th
+// distance go to the smaller index, kept in bi.  Without it (distance histograms) no point is skipped, only the multiset of
+// the k distances is kept and bi is not written.
+template <int KMAX, bool BY_INDEX>
+__device__ __forceinline__ void grid_knn_walk(const double2* __restrict__ pts, const int32_t* __restrict__ idx_sorted,
+                                              const int32_t* __restrict__ cell_start, const GridGeom gm, double2 q, int32_t qi, int k,
+                                              double (&bd)[KMAX], int32_t (&bi)[KMAX]) {
     const int cx = grid_cell_coord(q.x, gm.x0, gm.inv_cell, gm.gx), cy = grid_cell_coord(q.y, gm.y0, gm.inv_cell, gm.gy);
-    double bd[KMAX];
-    int32_t bi[KMAX];
 #pragma unroll
     for (int t = 0; t < KMAX; ++t) {
         bd[t] = INFINITY;
-        bi[t] = 0x7fffffff;
+        if (BY_INDEX) bi[t] = 0x7fffffff;
     }
     const int rmax = gm.gx > gm.gy ? gm.gx : gm.gy;
     for (int r = 0; r <= rmax; ++r) {
@@ -80,24 +116,30 @@ __global__ void __launch_bounds__(128) graph_knn_kernel(const double2* __restric
                 const int64_t c = (int64_t)yy * gm.gx + xx;
                 const int32_t b = cell_start[c], e = cell_start[c + 1];
                 for (int32_t t = b; t < e; ++t) {
-                    const int32_t j = idx_sorted[t];
-                    if (j == qi) continue;  // the query point itself is not its own neighbour (kneighbors() without X)
+                    int32_t j = 0;
+                    if (BY_INDEX) {
+                        j = idx_sorted[t];
+                        if (j == qi) continue;  // the query point itself is not its own neighbour (kneighbors() without X)
+                    }
                     const double2 p = pts[t];
                     const double dx = q.x - p.x, dy = q.y - p.y;
                     const double d2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
-                    if (d2 < bd[k - 1] || (d2 == bd[k - 1] && j < bi[k - 1])) {
-                        // insert (d2, j) into the ascending list of the k best
-                        double cd = d2;
-                        int32_t ci = j;
+                    if (d2 < bd[0] || (BY_INDEX && d2 == bd[0] && j < bi[0])) {
+                        // drop the k-th entry, shift the larger ones down and put (d2, j) in place
+                        bool placed = false;
 #pragma unroll
                         for (int u = 0; u < KMAX; ++u) {
-                            if (u < k && (cd < bd[u] || (cd == bd[u] && ci < bi[u]))) {
-                                const double td = bd[u];
-                                const int32_t ti = bi[u];
-                                bd[u] = cd;
-                                bi[u] = ci;
-                                cd = td;
-                                ci = ti;
+                            if (u < k && !placed) {
+                                const double nd = (u + 1 < KMAX && u + 1 < k) ? bd[u + 1 < KMAX ? u + 1 : u] : -INFINITY;
+                                const int32_t ni = (BY_INDEX && u + 1 < KMAX && u + 1 < k) ? bi[u + 1 < KMAX ? u + 1 : u] : 0;
+                                if (nd > d2 || (BY_INDEX && nd == d2 && ni > j)) {
+                                    bd[u] = nd;
+                                    if (BY_INDEX) bi[u] = ni;
+                                } else {
+                                    bd[u] = d2;
+                                    if (BY_INDEX) bi[u] = j;
+                                    placed = true;
+                                }
                             }
                         }
                     }
@@ -105,10 +147,23 @@ __global__ void __launch_bounds__(128) graph_knn_kernel(const double2* __restric
                 if (r == 0) break;
             }
         }
-        // everything not yet visited lies beyond r cells; slightly shrunk bound: cell assignment is a rounded computation
-        const double reach = (double)r * gm.cell * (1.0 - 1e-12);
-        if (bd[k - 1] < reach * reach) break;
+        // every unvisited point is at least sqrt(lb) away: stop once the k-th distance is below that
+        const double lb = grid_unvisited_bound(gm, q, cx, cy, r);
+        if (lb < 0.0 || bd[0] < lb) break;
     }
+}
+
+template <int KMAX>
+__global__ void __launch_bounds__(128) graph_knn_kernel(const double2* __restrict__ pts, const int32_t* __restrict__ idx_sorted,
+                                                        const int32_t* __restrict__ cell_start, int64_t n, GridGeom gm, int k,
+                                                        int32_t* __restrict__ out_idx, double* __restrict__ out_dist) {
+    const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const double2 q = pts[s];
+    const int32_t qi = idx_sorted[s];
+    double bd[KMAX];
+    int32_t bi[KMAX];
+    grid_knn_walk<KMAX, true>(pts, idx_sorted, cell_start, gm, q, qi, k, bd, bi);
     // rows of a CSR matrix hold ascending column indices: order the k neighbours by index (k is small)
     for (int a = 1; a < k; ++a) {
         const double vd = bd[a];
@@ -283,6 +338,145 @@ int radius_launch(sqb_ctx* c, const PointGrid& g, int64_t n, double radius, int6
     return SQB_OK;
 }
 
+// ---- nearest-neighbour distance histograms (Ripley's F and G) -----------------------------------------------------------
+// Every reference set is bucketed into its own grid; the grids are concatenated (set s owns the global cells cell_off ..
+// cell_off + gx * gy), so one radix sort of (global cell, pool index) buckets all of them.
+struct NnSet {
+    GridGeom gm;
+    int64_t cell_off;   // first global cell of the set's grid
+    int64_t ref_begin;  // pool index of the set's first point
+    int64_t entry_off;  // first entry of the set in the concatenated bucketing input
+};
+
+// One CTA's share of a task: queries q0 .. q1 of the pool against set `set`, k distances each, into histogram row `row`.
+struct NnBlock {
+    int32_t q0, q1, set, row, k, pad;
+};
+
+#define NN_THREADS 128
+#define NN_QPB 1024            // queries per block descriptor (NN_QPB / NN_THREADS per thread)
+#define NN_SHARED_BINS 8192    // histograms of up to this many bins are kept in shared memory per block
+
+__global__ void nnd_cell_id_kernel(const double* __restrict__ xy, const NnSet* __restrict__ sets, int n_sets, int64_t n_entries,
+                                   uint32_t* __restrict__ cell, int32_t* __restrict__ idx) {
+    const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (e >= n_entries) return;
+    int lo = 0, hi = n_sets - 1;  // the last set whose entry_off <= e
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (sets[mid].entry_off <= e) lo = mid; else hi = mid - 1;
+    }
+    const NnSet st = sets[lo];
+    const int64_t i = st.ref_begin + (e - st.entry_off);
+    const int cx = grid_cell_coord(xy[2 * i], st.gm.x0, st.gm.inv_cell, st.gm.gx);
+    const int cy = grid_cell_coord(xy[2 * i + 1], st.gm.y0, st.gm.inv_cell, st.gm.gy);
+    cell[e] = (uint32_t)(st.cell_off + (int64_t)cy * st.gm.gx + cx);
+    idx[e] = (int32_t)i;
+}
+
+// np.histogram(sqrt(d2), bins=e) for ascending edges e[0 .. S) (numpy's cumulative searchsorted: side 'left' for every edge but
+// the last, 'right' for the last): d = sqrt(d2) falls into bin i = #{j < S - 1 : e[j] <= d} - 1 when e[0] <= d <= e[S - 1], and
+// is dropped otherwise.  The comparisons are made on d2 against thresholds of the host (nnd_thresholds): thr[j] = min{t : sqrt(t)
+// >= e[j]} for j < S - 1 and thr[S - 1] = max{t : sqrt(t) <= e[S - 1]}, so that e[j] <= sqrt(d2) <=> thr[j] <= d2 and
+// sqrt(d2) <= e[S - 1] <=> d2 <= thr[S - 1] exactly (sqrt is correctly rounded and monotone).  Returns -1 for a dropped value.
+__device__ __forceinline__ int nnd_bin(double d2, const double* __restrict__ thr, int S) {
+    if (!(d2 >= thr[0]) || !(d2 <= thr[S - 1])) return -1;
+    int lo = 0, hi = S - 1;  // first j in [0, S - 1) with thr[j] > d2, or S - 1
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (thr[mid] > d2) hi = mid; else lo = mid + 1;
+    }
+    return lo - 1;
+}
+
+template <int KMAX, bool SHARED>
+__global__ void __launch_bounds__(NN_THREADS, 1) nnd_hist_kernel(const double2* __restrict__ pool, const double2* __restrict__ pts,
+                                                              const int32_t* __restrict__ cell_start, const NnSet* __restrict__ sets,
+                                                              const NnBlock* __restrict__ blocks, const double* __restrict__ thr, int S,
+                                                              unsigned long long* __restrict__ out) {
+    extern __shared__ uint32_t s_hist[];
+    const NnBlock blk = blocks[blockIdx.x];
+    const int nb = S - 1;
+    if (SHARED) {
+        for (int b = threadIdx.x; b < nb; b += NN_THREADS) s_hist[b] = 0u;
+        __syncthreads();
+    }
+    const NnSet st = sets[blk.set];
+    const int32_t* cs = cell_start + st.cell_off;
+    for (int32_t qi = blk.q0 + threadIdx.x; qi < blk.q1; qi += NN_THREADS) {
+        double bd[KMAX];
+        int32_t bi[KMAX];
+        grid_knn_walk<KMAX, false>(pts, nullptr, cs, st.gm, pool[qi], -1, blk.k, bd, bi);
+#pragma unroll
+        for (int u = 0; u < KMAX; ++u) {
+            if (u < blk.k) {
+                const int b = nnd_bin(bd[u], thr, S);
+                if (b >= 0) {
+                    if (SHARED)
+                        atomicAdd(&s_hist[b], 1u);
+                    else
+                        atomicAdd(&out[(int64_t)blk.row * nb + b], 1ULL);
+                }
+            }
+        }
+    }
+    if (SHARED) {
+        __syncthreads();
+        unsigned long long* row = out + (int64_t)blocks[blockIdx.x].row * nb;
+        for (int b = threadIdx.x; b < nb; b += NN_THREADS) {
+            const uint32_t v = s_hist[b];
+            if (v) atomicAdd(&row[b], (unsigned long long)v);
+        }
+    }
+}
+
+template <int KMAX>
+static int nnd_launch(sqb_ctx* c, int64_t nblk, const double2* pool, const double2* pts, const int32_t* cell_start, const NnSet* sets,
+                      const NnBlock* blocks, const double* thr, int S, unsigned long long* out) {
+    if (nblk == 0) return SQB_OK;
+    SqbLaunchScope scope(c, SQB_K_MISC);
+    if (S - 1 <= NN_SHARED_BINS)
+        nnd_hist_kernel<KMAX, true><<<(unsigned)nblk, NN_THREADS, (size_t)(S - 1) * sizeof(uint32_t), c->stream>>>(pool, pts, cell_start, sets,
+                                                                                                                 blocks, thr, S, out);
+    else
+        nnd_hist_kernel<KMAX, false><<<(unsigned)nblk, NN_THREADS, 0, c->stream>>>(pool, pts, cell_start, sets, blocks, thr, S, out);
+    SQB_POST_LAUNCH();
+    return SQB_OK;
+}
+
+// The d2 thresholds of nnd_bin for the edges e[0 .. S).
+static void nnd_thresholds(const double* e, int S, double* thr) {
+    const double inf = std::numeric_limits<double>::infinity();
+    for (int j = 0; j < S - 1; ++j) {  // min{t >= 0 : sqrt(t) >= e[j]}
+        const double r = e[j];
+        if (r <= 0.0 || std::isinf(r)) {
+            thr[j] = r <= 0.0 ? 0.0 : inf;
+            continue;
+        }
+        double t = r * r;
+        while (std::sqrt(t) < r) t = std::nextafter(t, inf);  // r * r overflowed: t reaches inf, sqrt(inf) >= r
+        while (t > 0.0 && std::sqrt(std::nextafter(t, 0.0)) >= r) t = std::nextafter(t, 0.0);
+        thr[j] = t;
+    }
+    const double r = e[S - 1];  // max{t : sqrt(t) <= e[S - 1]}
+    if (r < 0.0 || std::isinf(r)) {
+        thr[S - 1] = r < 0.0 ? -1.0 : inf;
+        return;
+    }
+    double t = r * r;
+    while (std::sqrt(t) > r) t = std::nextafter(t, 0.0);
+    for (;;) {
+        const double u = std::nextafter(t, inf);
+        if (std::isfinite(u) && std::sqrt(u) <= r)
+            t = u;
+        else
+            break;
+    }
+    thr[S - 1] = t;
+}
+
+static int nnd_kclass(int k) { return k <= 2 ? 0 : k <= 8 ? 1 : k <= 16 ? 2 : k <= 32 ? 3 : 4; }
+
 extern "C" {
 
 int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_idx, double* out_dist, double* median_out) {
@@ -346,6 +540,158 @@ int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int6
         SQB_CUDA(cudaMemcpyAsync(out_dist, d_dist.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
         SQB_CUDA(cudaStreamSynchronize(c->stream));
     }
+    return SQB_OK;
+}
+
+int sqb_nn_dist_hist_f64(sqb_ctx* ctx, const double* pts, int64_t n_pts, const int64_t* tasks, int64_t n_tasks, const double* support, int S,
+                         int n_rows, int shard_index, int shard_count, int64_t* out) {
+    SQB_CHECK(ctx && pts && support && out && (tasks || n_tasks == 0), SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: null argument");
+    SQB_CHECK(n_pts >= 0 && n_pts < 2147483647LL, SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: n_pts=%lld out of range", (long long)n_pts);
+    SQB_CHECK(n_tasks >= 0, SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: n_tasks=%lld out of range", (long long)n_tasks);
+    SQB_CHECK(S >= 2 && S <= (1 << 24), SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: S=%d out of range [2,%d]", S, 1 << 24);
+    SQB_CHECK(n_rows >= 1, SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: n_rows=%d out of range", n_rows);
+    SQB_CHECK(shard_count >= 1 && shard_index >= 0 && shard_index < shard_count, SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: bad shard %d/%d",
+              shard_index, shard_count);
+    SQB_CHECK((int64_t)n_rows * (S - 1) < (1LL << 40), SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: output too large");
+    for (int s = 0; s < S; ++s) {
+        SQB_CHECK(!(support[s] != support[s]), SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: support[%d] is NaN", s);
+        SQB_CHECK(s == 0 || support[s] >= support[s - 1], SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: support must be ascending (support[%d])", s);
+    }
+    for (int64_t i = 0; i < n_pts; ++i)
+        SQB_CHECK(std::isfinite(pts[2 * i]) && std::isfinite(pts[2 * i + 1]), SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: point %lld is not finite",
+                  (long long)i);
+    // reference sets: one grid per distinct (ref_begin, ref_end), sized for the largest k searched in it
+    std::map<std::pair<int64_t, int64_t>, int> set_of;
+    std::vector<std::pair<int64_t, int64_t>> ranges;
+    std::vector<int> set_k, task_set(n_tasks);
+    for (int64_t t = 0; t < n_tasks; ++t) {
+        const int64_t* tk = tasks + 6 * t;
+        const int64_t rb = tk[0], re = tk[1], qb = tk[2], qe = tk[3], k = tk[4], row = tk[5];
+        SQB_CHECK(0 <= rb && rb <= re && re <= n_pts && 0 <= qb && qb <= qe && qe <= n_pts, SQB_ERR_INVALID,
+                  "sqb_nn_dist_hist_f64: task %lld has a range outside [0, %lld]", (long long)t, (long long)n_pts);
+        SQB_CHECK(k >= 1 && k <= 64, SQB_ERR_UNSUPPORTED, "sqb_nn_dist_hist_f64: task %lld: k=%lld outside [1, 64]", (long long)t, (long long)k);
+        SQB_CHECK(k <= re - rb, SQB_ERR_INVALID, "Expected n_neighbors <= n_samples_fit, but n_neighbors = %lld, n_samples_fit = %lld (task %lld)",
+                  (long long)k, (long long)(re - rb), (long long)t);
+        SQB_CHECK(row >= 0 && row < n_rows, SQB_ERR_INVALID, "sqb_nn_dist_hist_f64: task %lld: row %lld outside [0, %d)", (long long)t,
+                  (long long)row, n_rows);
+        auto it = set_of.find({rb, re});
+        if (it == set_of.end()) {
+            it = set_of.emplace(std::make_pair(rb, re), (int)ranges.size()).first;
+            ranges.push_back({rb, re});
+            set_k.push_back(0);
+        }
+        task_set[t] = it->second;
+        set_k[it->second] = std::max(set_k[it->second], (int)k);
+    }
+    const int n_sets = (int)ranges.size();
+    std::vector<NnSet> sets(n_sets);
+    int64_t n_entries = 0, n_cells = 0;
+    for (int s = 0; s < n_sets; ++s) {
+        const int64_t rb = ranges[s].first, re = ranges[s].second;
+        double x0 = INFINITY, y0 = INFINITY, x1 = -INFINITY, y1 = -INFINITY;
+        for (int64_t i = rb; i < re; ++i) {
+            const double x = pts[2 * i], y = pts[2 * i + 1];
+            x0 = x < x0 ? x : x0, x1 = x > x1 ? x : x1, y0 = y < y0 ? y : y0, y1 = y > y1 ? y : y1;
+        }
+        sets[s].gm = grid_geometry(x0, y0, x1, y1, re - rb, 0.0, knn_pts_per_cell(set_k[s]));
+        sets[s].cell_off = n_cells;
+        sets[s].ref_begin = rb;
+        sets[s].entry_off = n_entries;
+        n_cells += (int64_t)sets[s].gm.gx * sets[s].gm.gy;
+        n_entries += re - rb;
+    }
+    SQB_CHECK(n_entries < 2147483647LL && n_cells < 2147483647LL, SQB_ERR_UNSUPPORTED,
+              "sqb_nn_dist_hist_f64: %lld reference points in %lld cells do not fit int32", (long long)n_entries, (long long)n_cells);
+    // query blocks in task order, dealt to the shards round robin; grouped by the kernel's k class
+    std::vector<NnBlock> blocks[5];
+    int64_t nblk_all = 0;
+    for (int64_t t = 0; t < n_tasks; ++t) {
+        const int64_t* tk = tasks + 6 * t;
+        for (int64_t q0 = tk[2]; q0 < tk[3]; q0 += NN_QPB, ++nblk_all) {
+            if (nblk_all % shard_count != shard_index) continue;
+            NnBlock b;
+            b.q0 = (int32_t)q0, b.q1 = (int32_t)std::min<int64_t>(q0 + NN_QPB, tk[3]), b.set = task_set[t], b.row = (int32_t)tk[5];
+            b.k = (int32_t)tk[4], b.pad = 0;
+            blocks[nnd_kclass(b.k)].push_back(b);
+        }
+    }
+    const size_t out_n = (size_t)n_rows * (S - 1);
+    int64_t nblk = 0;
+    for (auto& v : blocks) nblk += (int64_t)v.size();
+    if (nblk == 0) {
+        std::fill(out, out + out_n, (int64_t)0);
+        return SQB_OK;
+    }
+    sqb_ctx* c = ctx;
+    SQB_CUDA(cudaSetDevice(c->device));
+    PointGrid g(c->stream);  // d_xy: the pool; d_pts / d_idx_sorted / d_cell_start: every reference set in cell order
+    DevBuf<NnSet> d_sets(c->stream);
+    DevBuf<NnBlock> d_blocks(c->stream);
+    DevBuf<double> d_thr(c->stream);
+    DevBuf<unsigned long long> d_out(c->stream);
+    SQB_TRY(g.d_xy.alloc(2 * (size_t)std::max<int64_t>(n_pts, 1)));
+    SQB_TRY(d_sets.alloc(n_sets));
+    SQB_TRY(d_blocks.alloc(nblk));
+    SQB_TRY(d_thr.alloc(S));
+    SQB_TRY(d_out.alloc(out_n));
+    SQB_CUDA(cudaMemcpyAsync(g.d_xy.p, pts, 2 * n_pts * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(d_sets.p, sets.data(), n_sets * sizeof(NnSet), cudaMemcpyHostToDevice, c->stream));
+    {
+        int64_t off = 0;
+        for (auto& v : blocks) {
+            if (!v.empty()) SQB_CUDA(cudaMemcpyAsync(d_blocks.p + off, v.data(), v.size() * sizeof(NnBlock), cudaMemcpyHostToDevice, c->stream));
+            off += (int64_t)v.size();
+        }
+    }
+    std::vector<double> thr(S);
+    nnd_thresholds(support, S, thr.data());
+    SQB_CUDA(cudaMemcpyAsync(d_thr.p, thr.data(), S * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    SQB_CUDA(cudaMemsetAsync(d_out.p, 0, out_n * sizeof(unsigned long long), c->stream));
+    {
+        DevBuf<uint32_t> cell_a(c->stream), cell_b(c->stream);
+        DevBuf<int32_t> idx_a(c->stream);
+        DevBuf<uint8_t> tmp(c->stream);
+        const int64_t ne = std::max<int64_t>(n_entries, 1);
+        SQB_TRY(g.d_pts.alloc(ne));
+        SQB_TRY(g.d_idx_sorted.alloc(ne));
+        SQB_TRY(g.d_cell_start.alloc(n_cells + 1));
+        SQB_TRY(cell_a.alloc(ne));
+        SQB_TRY(cell_b.alloc(ne));
+        SQB_TRY(idx_a.alloc(ne));
+        if (n_entries > 0) {
+            c->launches += 1;
+            nnd_cell_id_kernel<<<(unsigned)ceil_div64(n_entries, 256), 256, 0, c->stream>>>(g.d_xy.p, d_sets.p, n_sets, n_entries, cell_a.p, idx_a.p);
+            SQB_POST_LAUNCH();
+            int bits = 1;
+            while (bits < 32 && ((uint64_t)(n_cells - 1) >> bits) != 0) ++bits;
+            size_t tmp_bytes = 0;
+            SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cell_a.p, cell_b.p, idx_a.p, g.d_idx_sorted.p, (int)n_entries, 0, bits,
+                                                     c->stream));
+            SQB_TRY(tmp.alloc(tmp_bytes > 0 ? tmp_bytes : 1));
+            SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, cell_a.p, cell_b.p, idx_a.p, g.d_idx_sorted.p, (int)n_entries, 0, bits,
+                                                     c->stream));
+            c->launches += 2;
+            graph_gather_kernel<<<(unsigned)ceil_div64(n_entries, 256), 256, 0, c->stream>>>(g.d_xy.p, cell_b.p, g.d_idx_sorted.p, n_entries, n_cells,
+                                                                                            g.d_pts.p, g.d_cell_start.p);
+            SQB_POST_LAUNCH();
+        }
+    }
+    const double2* pool = reinterpret_cast<const double2*>(g.d_xy.p);
+    const int64_t n_cls[5] = {(int64_t)blocks[0].size(), (int64_t)blocks[1].size(), (int64_t)blocks[2].size(), (int64_t)blocks[3].size(),
+                              (int64_t)blocks[4].size()};
+    const NnBlock* b = d_blocks.p;
+    SQB_TRY(nnd_launch<2>(c, n_cls[0], pool, g.d_pts.p, g.d_cell_start.p, d_sets.p, b, d_thr.p, S, d_out.p));
+    b += n_cls[0];
+    SQB_TRY(nnd_launch<8>(c, n_cls[1], pool, g.d_pts.p, g.d_cell_start.p, d_sets.p, b, d_thr.p, S, d_out.p));
+    b += n_cls[1];
+    SQB_TRY(nnd_launch<16>(c, n_cls[2], pool, g.d_pts.p, g.d_cell_start.p, d_sets.p, b, d_thr.p, S, d_out.p));
+    b += n_cls[2];
+    SQB_TRY(nnd_launch<32>(c, n_cls[3], pool, g.d_pts.p, g.d_cell_start.p, d_sets.p, b, d_thr.p, S, d_out.p));
+    b += n_cls[3];
+    SQB_TRY(nnd_launch<64>(c, n_cls[4], pool, g.d_pts.p, g.d_cell_start.p, d_sets.p, b, d_thr.p, S, d_out.p));
+    static_assert(sizeof(unsigned long long) == sizeof(int64_t), "counts are copied as int64");
+    SQB_CUDA(cudaMemcpyAsync(out, d_out.p, out_n * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
     return SQB_OK;
 }
 

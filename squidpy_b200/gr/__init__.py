@@ -5,7 +5,7 @@ from ._build import (GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsRes
 from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
 from ._nhood import NhoodEnrichmentResult, NhoodPlan, interaction_matrix, nhood_enrichment
 from ._ppatterns import AutocorrPlan, co_occurrence, cooc_counts, spatial_autocorr
-from ._ripley import pair_counts, ripley
+from ._ripley import nn_distance_hist, pair_counts, ripley
 from ._sepal import sepal, sepal_scores
 
 __all__ = [
@@ -33,4 +33,5 @@ __all__ = [
     "AutocorrPlan",
     "cooc_counts",
     "pair_counts",
+    "nn_distance_hist",
 ]

@@ -2,9 +2,14 @@
 
 Mode ``L``: the expensive step — cumulative ordered-pair counts per cluster, ``KDTree.two_point_correlation`` in the
 reference (:218-223) — runs on the H100 (``sqb_pair_counts_f64``: float64, bit-identical counts), for the observed
-clusters and for all Poisson-point-process simulations in ONE launch.  Modes ``F``/``G`` need only 1-/2-nearest
-neighbour distances of ~1000 points and stay on the host with scikit-learn, like in the reference; so do the convex
-hull, the rejection-sampled simulations (they must consume numpy's RNG stream exactly) and the long-format reshaping.
+clusters and for all Poisson-point-process simulations in ONE launch.  Modes ``F``/``G``: the nearest-neighbour searches
+(:140-150, :160-169) and the histogram of their distances (:206-209) run on the H100 too (``sqb_nn_dist_hist_f64``: float64,
+bit-identical bin counts) for the euclidean metric, again in ONE call for the observed clusters and every simulation.  G is
+the heavy one: its observed statistic queries every point outside a cluster against the cluster, and every simulation
+queries all N points.  A reference set goes to the device only when scikit-learn would search it with its kd_tree (whose
+distances the kernel reproduces bit for bit); smaller sets, where scikit-learn switches to brute force and its GEMM-form
+distances, and every other metric stay on the host with scikit-learn.  The convex hull, the rejection-sampled simulations
+(they must consume numpy's RNG stream exactly), the cumulative fractions and the long-format reshaping stay on the host.
 """
 
 from __future__ import annotations
@@ -23,7 +28,11 @@ from .._rng import spawn_generators
 from .._validators import assert_categorical_obs, assert_spatial_basis, extract_adata_if_sdata
 from ._utils import _save_data, logg
 
-__all__ = ["ripley", "pair_counts"]
+__all__ = ["ripley", "pair_counts", "nn_distance_hist"]
+
+# metrics NearestNeighbors searches with the euclidean distance (minkowski: its default p = 2)
+_EUCLIDEAN = ("euclidean", "l2", "minkowski")
+_NN_MAX_K = 64  # largest k of the kernel
 
 
 def pair_counts(groups: list[np.ndarray], support: np.ndarray, *, ctx: Context | None = None, shard: tuple[int, int] = (0, 1)) -> np.ndarray:
@@ -38,6 +47,27 @@ def pair_counts(groups: list[np.ndarray], support: np.ndarray, *, ctx: Context |
     out = np.empty((len(groups), support.size), dtype=np.int64)
     check(lib.sqb_pair_counts_f64(ctx.handle, pts.ctypes.data, ptr.ctypes.data, len(groups), support.ctypes.data, support.size,
                                   int(shard[0]), int(shard[1]), out.ctypes.data))
+    return out
+
+
+def nn_distance_hist(points: np.ndarray, tasks: np.ndarray, support: np.ndarray, n_rows: int, *, ctx: Context | None = None,
+                     shard: tuple[int, int] = (0, 1)) -> np.ndarray:
+    """Histograms of nearest-neighbour distances on the GPU: int64 (n_rows, len(support) - 1).
+
+    ``points`` is an (n, 2) pool of float64 coordinates; every row of ``tasks`` (int64, 6 columns) is ``(ref_begin, ref_end,
+    qry_begin, qry_end, k, row)``: the k nearest distances of every query point ``points[qry_begin:qry_end]`` among
+    ``points[ref_begin:ref_end]`` (no point excluded) are added to histogram ``row``, i.e.
+    ``np.histogram(NearestNeighbors().fit(ref).kneighbors(qry, k)[0], bins=support)[0]`` with scikit-learn's kd_tree
+    distances.  ``support`` must be ascending; 1 <= k <= min(64, ref_end - ref_begin).  ``shard=(r, n)``: this device's share of
+    the query blocks (the shares add up to the whole)."""
+    lib = load()
+    ctx = ctx or default_context()
+    pts = np.ascontiguousarray(np.asarray(points, dtype=np.float64).reshape(-1, 2))
+    tk = np.ascontiguousarray(np.asarray(tasks, dtype=np.int64).reshape(-1, 6))
+    support = np.ascontiguousarray(support, dtype=np.float64)
+    out = np.empty((int(n_rows), max(support.size - 1, 0)), dtype=np.int64)
+    check(lib.sqb_nn_dist_hist_f64(ctx.handle, pts.ctypes.data if pts.size else np.zeros(2).ctypes.data, pts.shape[0], tk.ctypes.data, tk.shape[0],
+                                   support.ctypes.data, support.size, int(n_rows), int(shard[0]), int(shard[1]), out.ctypes.data))
     return out
 
 
@@ -64,7 +94,6 @@ def ripley(
     (bins, cluster, stats), ``'sims_stat'``: long DataFrame, ``'bins'``: float64[n_steps], ``'pvalues'``:
     float64[n_clusters, n_steps]``}``."""
     from scipy.spatial import ConvexHull
-    from sklearn.neighbors import NearestNeighbors
     from sklearn.preprocessing import LabelEncoder
 
     adata = extract_adata_if_sdata(adata, table_key=table_key)
@@ -108,27 +137,11 @@ def ripley(
         obs_arr[: len(groups)] = l_all[: len(groups)]
         sims = l_all[len(groups) :].reshape(n_simulations, n_steps)
     else:
-        random = None
-        for i in np.arange(np.max(cluster_idx) + 1):
-            coord_c = coordinates[cluster_idx == i, :]
-            if mode == RipleyStat.F:
-                random = _ppp(hull, n_simulations=1, n_observations=n_observations, rng=obs_rng)
-                tree_c = NearestNeighbors(metric=metric, n_neighbors=n_neigh).fit(coord_c)
-                distances, _ = tree_c.kneighbors(random, n_neighbors=n_neigh)
-            else:
-                tree_c = NearestNeighbors(metric=metric, n_neighbors=n_neigh).fit(coord_c)
-                distances, _ = tree_c.kneighbors(coordinates[cluster_idx != i, :], n_neighbors=n_neigh)
-            bins, obs_stats = _f_g_function(distances.squeeze(), support)
-            obs_arr[i] = obs_stats
-        sims = np.empty((n_simulations, len(bins)))
-        for i in range(n_simulations):
-            random_i = _ppp(hull, n_simulations=1, n_observations=n_observations, rng=sim_rngs[i])
-            tree_i = NearestNeighbors(metric=metric, n_neighbors=n_neigh).fit(random_i)
-            if mode == RipleyStat.F:
-                distances_i, _ = tree_i.kneighbors(random, n_neighbors=1)
-            else:
-                distances_i, _ = tree_i.kneighbors(coordinates, n_neighbors=1)
-            _, sims[i] = _f_g_function(distances_i.squeeze(), support)
+        counts = _f_g_counts(mode, coordinates, cluster_idx, hull, support, metric, n_neigh, n_simulations, n_observations, obs_rng,
+                             sim_rngs, device)
+        stats = _f_g_from_counts(counts)
+        obs_arr[: counts.shape[0] - n_simulations] = stats[: counts.shape[0] - n_simulations]
+        sims = stats[counts.shape[0] - n_simulations :]
 
     pvalues = np.ones((n_cls, len(bins)))
     for i in range(n_simulations):
@@ -165,6 +178,102 @@ def _l_from_counts(counts: np.ndarray, sizes: np.ndarray, n: int, area: float) -
     return np.sqrt(k_estimate / np.pi)
 
 
+def _kd_tree_euclidean(metric: str, n_neigh: Any, n_fit: int) -> bool:
+    """Whether ``NearestNeighbors(metric=metric, n_neighbors=n_neigh).fit(X)`` with ``n_fit`` 2-D points searches with its
+    kd_tree under the euclidean distance (sklearn's ``auto`` rule: ``n_neighbors < n_fit // 2``) and k fits the kernel.  Below
+    that size sklearn runs brute force, whose distances come from a GEMM form with other last bits."""
+    if metric not in _EUCLIDEAN or isinstance(n_neigh, bool) or not isinstance(n_neigh, (int, np.integer)):
+        return False
+    return 1 <= int(n_neigh) <= _NN_MAX_K and int(n_neigh) < n_fit // 2
+
+
+def _knn_hist_host(ref: np.ndarray, qry: np.ndarray, metric: str, n_neigh: Any, k: Any, support: np.ndarray) -> np.ndarray:
+    """The reference's search and histogram with scikit-learn (``_ripley.py:145-150, 162-169, 206-207``)."""
+    from sklearn.neighbors import NearestNeighbors
+
+    tree = NearestNeighbors(metric=metric, n_neighbors=n_neigh).fit(ref)
+    distances, _ = tree.kneighbors(qry, n_neighbors=k)
+    return np.histogram(distances.squeeze(), bins=support)[0]
+
+
+def _f_g_plan(mode: RipleyStat, coordinates: np.ndarray, cluster_idx: np.ndarray, draws_obs: list[np.ndarray], draws_sim: list[np.ndarray],
+              support: np.ndarray, metric: str, n_neigh: Any) -> tuple[np.ndarray, np.ndarray, list[tuple]]:
+    """The histograms of F / G as one point pool and task list for ``nn_distance_hist``, and the rows left to the host.
+
+    Row c < n_clusters is the observed statistic of cluster c, row n_clusters + i simulation i.  G: cluster c against every
+    point outside it (the two ranges on either side of c in the cluster-sorted pool), simulation i: all N points against draw
+    i (k = 1).  F: draw c (one per cluster) against cluster c, simulation i: the last cluster's draw against draw i (k = 1).
+    Returns (pool, tasks, host) where host lists ``(row, ref, qry, k)`` for the rows the device does not take."""
+    n_cls = len(draws_obs) if mode == RipleyStat.F else int(np.max(cluster_idx)) + 1
+    order = np.argsort(cluster_idx, kind="stable")
+    ptr = np.zeros(n_cls + 1, dtype=np.int64)
+    ptr[1:] = np.cumsum(np.bincount(cluster_idx, minlength=n_cls)[:n_cls])
+    N = coordinates.shape[0]
+    planar = coordinates.ndim == 2 and coordinates.shape[1] == 2
+    ok_support = support.size >= 2 and bool(np.all(np.isfinite(support))) and bool(np.all(np.diff(support) >= 0))
+    blocks = [np.asarray(coordinates, dtype=np.float64)[order]] if planar else []
+    off = N
+    draw_ptr = []
+    for d in list(draws_obs) + list(draws_sim):
+        planar_d = d.ndim == 2 and d.shape[1] == 2
+        draw_ptr.append((off, off + d.shape[0]) if planar_d else None)
+        if planar and planar_d:
+            blocks.append(np.asarray(d, dtype=np.float64))
+            off += d.shape[0]
+    n_obs_draws = len(draws_obs)
+    tasks: list[tuple[int, ...]] = []
+    host: list[tuple] = []
+
+    def add(row, ref_rng, qry_rngs, sets, k):
+        """``sets()`` gives the (reference, query) arrays of the host call; built only for a row the device does not take."""
+        ok = planar and ok_support and ref_rng is not None and all(q is not None for q in qry_rngs)
+        if ok and sum(q[1] - q[0] for q in qry_rngs) > 0 and _kd_tree_euclidean(metric, n_neigh, int(ref_rng[1] - ref_rng[0])):
+            tasks.extend((ref_rng[0], ref_rng[1], q[0], q[1], int(k), row) for q in qry_rngs if q[1] > q[0])
+        else:
+            host.append((row, *sets(), k))
+
+    for c in range(n_cls):
+        if mode == RipleyStat.F:
+            add(c, (ptr[c], ptr[c + 1]), [draw_ptr[c]], lambda c=c: (coordinates[cluster_idx == c, :], draws_obs[c]), n_neigh)
+        else:
+            add(c, (ptr[c], ptr[c + 1]), [(0, ptr[c]), (ptr[c + 1], N)],
+                lambda c=c: (coordinates[cluster_idx == c, :], coordinates[cluster_idx != c, :]), n_neigh)
+    for i, d in enumerate(draws_sim):
+        if mode == RipleyStat.F:
+            add(n_cls + i, draw_ptr[n_obs_draws + i], [draw_ptr[n_obs_draws - 1]], lambda d=d: (d, draws_obs[-1]), 1)
+        else:
+            add(n_cls + i, draw_ptr[n_obs_draws + i], [(0, N)], lambda d=d: (d, coordinates), 1)
+    pool = np.concatenate(blocks) if blocks else np.zeros((0, 2))
+    return pool, np.asarray(tasks, dtype=np.int64).reshape(-1, 6), host
+
+
+def _f_g_counts(mode: RipleyStat, coordinates: np.ndarray, cluster_idx: np.ndarray, hull, support: np.ndarray, metric: str, n_neigh: Any,
+                n_simulations: int, n_observations: int, obs_rng: np.random.Generator, sim_rngs: list, device: int | None) -> np.ndarray:
+    """int64 (n_clusters + n_simulations, n_steps - 1) histogram counts of F or G: every draw first (in the reference's RNG
+    order: F's observed draws from ``obs_rng`` in cluster order, one generator per simulation), then ONE device call for the
+    sets scikit-learn searches with its kd_tree, and scikit-learn for the rest in row order."""
+    from scipy.spatial import Delaunay
+
+    deln = Delaunay(hull.points[hull.vertices])  # the triangulation _ppp would build on every call
+    n_cls = int(np.max(cluster_idx)) + 1
+    draws_obs = [_ppp(hull, 1, n_observations, rng=obs_rng, deln=deln) for _ in range(n_cls)] if mode == RipleyStat.F else []
+    draws_sim = [_ppp(hull, 1, n_observations, rng=sim_rngs[i], deln=deln) for i in range(n_simulations)]
+    pool, tasks, host = _f_g_plan(mode, coordinates, cluster_idx, draws_obs, draws_sim, support, metric, n_neigh)
+    counts = np.zeros((n_cls + n_simulations, max(len(support) - 1, 0)), dtype=np.int64)
+    if tasks.shape[0]:
+        rank, ws = world()
+        counts = all_reduce_sum(nn_distance_hist(pool, tasks, support, counts.shape[0], ctx=default_context(device), shard=(rank, ws)))
+    for row, ref, qry, k in host:
+        counts[row] = _knn_hist_host(ref, qry, metric, n_neigh, k, support)
+    return counts
+
+
+def _f_g_from_counts(counts: np.ndarray) -> np.ndarray:
+    """``_f_g_function`` (``_ripley.py:206-209``) of every row of histogram counts: [0, cumsum(counts) / counts.sum()]."""
+    fracs = np.cumsum(counts, axis=-1) / counts.sum(axis=-1, keepdims=True)
+    return np.concatenate((np.zeros(counts.shape[:-1] + (1,), dtype=float), fracs), axis=-1)
+
+
 def _reshape_res(results: np.ndarray, columns, index: np.ndarray, var_name: str) -> pd.DataFrame:
     df = pd.DataFrame(results, columns=columns, index=index)
     df.index.set_names(["bins"], inplace=True)
@@ -172,12 +281,6 @@ def _reshape_res(results: np.ndarray, columns, index: np.ndarray, var_name: str)
     df[var_name] = df[var_name].astype("category")
     df.reset_index(inplace=True)
     return df
-
-
-def _f_g_function(distances: np.ndarray, support: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
-    counts, bins = np.histogram(distances, bins=support)
-    fracs = np.cumsum(counts) / counts.sum()
-    return bins, np.concatenate((np.zeros((1,), dtype=float), fracs))
 
 
 def _ppp(hull, n_simulations: int, n_observations: int, rng: np.random.Generator, deln=None) -> np.ndarray:

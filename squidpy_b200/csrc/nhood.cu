@@ -641,17 +641,17 @@ __device__ __forceinline__ int sqb_list_latest_before(const uint16_t* __restrict
 //     same CTA (nhood_part_warp).  The generator only stores the target of step i at word part_idx(i - bL) of one of two
 //     block buffers and hands a complete block over through an mbarrier pair (full / empty per buffer), so it fills block
 //     b - 1 while block b is being partitioned.  The partition warp walks the same (permutation, segment, block) sequence.
-//     Lane l owns the 64 steps t in [64 l, 64 l + 64) of the block: it counts its entries per region, one 16-region
+//     Lane l owns the 64 steps t in [64 l, 64 l + 64) of the block: it counts its entries per region, one 32-region
 //     suffix scan over the lanes turns the counts into slots (higher t = earlier step comes first), it scatters its entries
 //     in step order into an output block in shared memory, and the warp streams that block out to J in whole lines.  The
 //     region of a target is a multiply-high by a per-segment magic number, exact for every j < 2^31 (sqb_part_magic).
 // ------------------------------------------------------------------------------------------------
 #define SQB_PART_L 2048    // steps per block of the partitioned target layout
-#define SQB_PART_RMAX 16   // regions per segment, at most (one u16 count per region and block: a 32-byte row)
+#define SQB_PART_RMAX 32   // regions per segment, at most (one u16 count per region and block: a 64-byte row)
 #define SQB_PART_LP (SQB_PART_L + SQB_PART_L / 64)  // words of a block buffer: one pad word per 64 (lane l reads words 65 l + s)
 // shared memory words of a generator / partition pair: mbarriers full[2], empty[2]; two block buffers; the output block;
-// the per-lane region table [SQB_PART_RMAX][32]
-#define SQB_PART_PAIR_WORDS (8 + 2 * SQB_PART_LP + SQB_PART_L + SQB_PART_RMAX * 32)
+// the per-lane region table [SQB_PART_RMAX][32] of u16 (a lane's count per region is <= 64 and its slots are < 2048)
+#define SQB_PART_PAIR_WORDS (8 + 2 * SQB_PART_LP + SQB_PART_L + SQB_PART_RMAX * 32 / 2)
 __host__ __device__ __forceinline__ void sqb_part_regions(int m, int cap, int& R, int& B) {
     R = (m + cap - 1) / cap;
     B = (((m + R - 1) / R + 15) / 16) * 16;  // balanced regions, <= cap (a multiple of 16)
@@ -684,6 +684,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* b, unsigned parity) {
 }
 
 // Partition warp of nhood_jgen_kernel<Q, true>: block seq of its generator arrives in buffer seq & 1 (use seq >> 1 of it).
+// NW = packed words of the region scan: 8 when no segment has more than 16 regions, else 16.  The partition warp shares the
+// SM's issue slots with the generators, so the narrow scan is kept for the inputs that fit it.
+template <int NW>
 __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uint32_t* __restrict__ J, int64_t stride,
                                                 int64_t perm0, int64_t n_perms, int64_t warps_total, int nseg,
                                                 const int64_t* __restrict__ seg_start, const int64_t* __restrict__ seg_len,
@@ -691,7 +694,7 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
     constexpr int L = SQB_PART_L;
     uint64_t* bar = reinterpret_cast<uint64_t*>(pair);  // full[0], full[1], empty[0], empty[1]
     uint32_t* __restrict__ out = pair + 8 + 2 * SQB_PART_LP;
-    uint32_t* __restrict__ tab = out + L;  // tab[r * 32 + lane]: this lane's entries of region r, then its next slot
+    uint16_t* __restrict__ tab = reinterpret_cast<uint16_t*>(out + L);  // tab[r * 32 + lane]: this lane's entries of region r, then its next slot
     unsigned seq = 0;
     for (int64_t perm = perm0; perm < n_perms; perm += warps_total) {
         int64_t row = perm * nb_total;  // count row of the current block's segment, block 0
@@ -708,35 +711,35 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
                     const int s0 = max(t0 - 64 * lane, 0), s1 = min(t1 - 64 * lane, 64);  // this lane's steps t = 64 lane + s
                     const uint32_t* __restrict__ in = pair + 8 + (seq & 1) * SQB_PART_LP + 65 * lane;
 #pragma unroll
-                    for (int r = 0; r < SQB_PART_RMAX; ++r) tab[r * 32 + lane] = 0;
+                    for (int r = 0; r < 2 * NW; ++r) tab[r * 32 + lane] = 0;
                     mbar_wait(&bar[seq & 1], (seq >> 1) & 1);
 #pragma unroll 4
                     for (int s = s0; s < s1; ++s) ++tab[(__umulhi(in[s], M) >> sh) * 32 + lane];
                     // slots: region base + entries of the same region on higher lanes (earlier steps); 16-bit fields, 2 regions a word
-                    uint32_t w[SQB_PART_RMAX / 2], x[SQB_PART_RMAX / 2];
+                    uint32_t w[NW], x[NW];
 #pragma unroll
-                    for (int k = 0; k < SQB_PART_RMAX / 2; ++k) x[k] = w[k] = tab[2 * k * 32 + lane] | (tab[(2 * k + 1) * 32 + lane] << 16);
+                    for (int k = 0; k < NW; ++k) x[k] = w[k] = (uint32_t)tab[2 * k * 32 + lane] | ((uint32_t)tab[(2 * k + 1) * 32 + lane] << 16);
 #pragma unroll
                     for (int d = 1; d < 32; d <<= 1)
 #pragma unroll
-                        for (int k = 0; k < SQB_PART_RMAX / 2; ++k) {
+                        for (int k = 0; k < NW; ++k) {
                             const uint32_t y = __shfl_down_sync(0xffffffffu, x[k], d);
                             if (lane + d < 32) x[k] += y;
                         }
-                    uint32_t run = 0, tot[SQB_PART_RMAX / 2];
+                    uint32_t run = 0, tot[NW];
 #pragma unroll
-                    for (int k = 0; k < SQB_PART_RMAX / 2; ++k) {
+                    for (int k = 0; k < NW; ++k) {
                         tot[k] = __shfl_sync(0xffffffffu, x[k], 0);
                         const uint32_t lo = tot[k] & 0xFFFFu;
                         const uint32_t slot = (run | ((run + lo) << 16)) + x[k] - w[k];
                         run += lo + (tot[k] >> 16);
-                        tab[2 * k * 32 + lane] = slot & 0xFFFFu;
-                        tab[(2 * k + 1) * 32 + lane] = slot >> 16;
+                        tab[2 * k * 32 + lane] = (uint16_t)(slot & 0xFFFFu);
+                        tab[(2 * k + 1) * 32 + lane] = (uint16_t)(slot >> 16);
                     }
-                    if (lane == 0) {  // the count row: u16 counts of regions 0..15, little-endian pairs = tot[]
+                    if (lane == 0) {  // the count row: u16 counts of regions 0 .. 2 NW - 1, little-endian pairs = tot[]
                         uint4* crow = reinterpret_cast<uint4*>(cnt + (row + blk) * SQB_PART_RMAX);
-                        crow[0] = make_uint4(tot[0], tot[1], tot[2], tot[3]);
-                        crow[1] = make_uint4(tot[4], tot[5], tot[6], tot[7]);
+#pragma unroll
+                        for (int q = 0; q < NW / 4; ++q) crow[q] = make_uint4(tot[4 * q], tot[4 * q + 1], tot[4 * q + 2], tot[4 * q + 3]);
                     }
                     __syncwarp();  // every lane has streamed the previous output block out
 #pragma unroll 4
@@ -744,7 +747,7 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
                         const uint32_t j = in[s];
                         const uint32_t r = __umulhi(j, M) >> sh;
                         const uint32_t slot = tab[r * 32 + lane];
-                        tab[r * 32 + lane] = slot + 1;
+                        tab[r * 32 + lane] = (uint16_t)(slot + 1);
                         out[slot] = ((uint32_t)(64 * lane + s) << 18) | (j - r * (uint32_t)B);
                     }
                     mbar_arrive(&bar[2 + (seq & 1)]);  // the buffer is free for the generator
@@ -794,8 +797,17 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
         if (warp < wpb && lane < 4) mbar_init(&bar[lane], 32);
         __syncthreads();
         if (warp >= wpb) {
-            nhood_part_warp(pair, J, stride, (int64_t)blockIdx.x * wpb + warp - wpb, n_perms, warps_total, nseg, seg_start,
-                            seg_len, cnt, nb_total, region_cap, lane);
+            int rmax = 0;
+            for (int seg = 0; seg < nseg; ++seg) {
+                int R = 0, B;
+                if (seg_len[seg] >= 2) sqb_part_regions((int)seg_len[seg], region_cap, R, B);
+                rmax = max(rmax, R);
+            }
+            const int64_t perm0 = (int64_t)blockIdx.x * wpb + warp - wpb;
+            if (rmax <= 16)
+                nhood_part_warp<8>(pair, J, stride, perm0, n_perms, warps_total, nseg, seg_start, seg_len, cnt, nb_total, region_cap, lane);
+            else
+                nhood_part_warp<16>(pair, J, stride, perm0, n_perms, warps_total, nseg, seg_start, seg_len, cnt, nb_total, region_cap, lane);
             return;
         }
     }
@@ -1311,6 +1323,14 @@ __device__ unsigned long long g_part_clk[SQB_PCLK_N];
 #define SQB_PCLK_COUNT(ph)
 #endif
 
+// A table entry is (position << SQB_PART_IDB) | slot id in 32 bits: positions are < 2^18 (region offsets) and ids < HS <= 2048
+#define SQB_PART_IDB 11
+#define SQB_PART_IDMASK ((1u << SQB_PART_IDB) - 1u)
+#define SQB_EMPTY32 0xFFFFFFFFu
+// words of s_bpref (and of s_bslot) for segments of at most nbmax step blocks: nbmax + 1 prefixes and 3 pad words that the
+// slot -> block lookup may read, a multiple of 4 words so that the slab stays 16-byte aligned
+__host__ __device__ __forceinline__ int sqb_part_bwords(int nbmax) { return (nbmax + 7) & ~3; }
+
 template <typename LT, int NT>
 __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __restrict__ labels, const uint32_t* __restrict__ J,
                                                                          const uint16_t* __restrict__ cnt,
@@ -1318,29 +1338,29 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                                                                          int64_t n_perms, int nseg,
                                                                          const int64_t* __restrict__ seg_start,
                                                                          const int64_t* __restrict__ seg_len, int64_t nb_total,
-                                                                         int region_cap) {
+                                                                         int region_cap, int bwords) {
     constexpr int L = SQB_PART_L;
     constexpr uint32_t full_mask = 0xFFFFFFFFu;  // (SQB_CONVERGE)
     constexpr int HS = 2 * NT;   // slots per window = hash slots per table
     constexpr int NWB = 2 * HS;  // filter words (16 buckets of 2 bits each)
     constexpr int LOG_HS = (HS == 1024 ? 10 : HS == 2048 ? 11 : 12);
     static_assert(HS == (1 << LOG_HS), "HS must be a power of two");
+    static_assert(HS <= (1 << SQB_PART_IDB), "slot ids must fit a table entry");
     constexpr int HS_SHIFT = 32 - LOG_HS;
     extern __shared__ __align__(16) unsigned char sqb_shuffle_smem[];
-    unsigned long long* s_tabT = reinterpret_cast<unsigned long long*>(sqb_shuffle_smem);  // [HS] (position << 32) | head of its targeter list
-    unsigned long long* s_tabO = s_tabT + HS;                                              // [HS] (position << 32) | slot whose top it is
-    uint32_t* s_bits = reinterpret_cast<uint32_t*>(s_tabO + HS);                            // [NWB] duplicate filter
-    int* s_top = reinterpret_cast<int*>(s_bits + NWB);                                      // [HS] top position of every slot
-    int* s_bpref = s_top + HS;                                                              // [NT + 4] region run prefix per block
-    int* s_bslot = s_bpref + NT + 4;                                                        // [NT] J slot of the run per block
-                                                                                            // (+ 4: the slab stays 16-byte aligned)
-    int* s_wsum = s_bslot + NT;                                                             // [32] scan partials
-    uint16_t* s_next = reinterpret_cast<uint16_t*>(s_wsum + 32);                            // [HS] list links
-    uint32_t* s_gath = reinterpret_cast<uint32_t*>(s_next + HS);                            // [HS] next window's tops above
-    LT* s_otop = reinterpret_cast<LT*>(s_gath + HS);                                        // [HS] original top values
-    LT* s_slab = s_otop + HS;                                                               // [region_cap] the region
+    uint32_t* s_tabT = reinterpret_cast<uint32_t*>(sqb_shuffle_smem);  // [HS] (position << 11) | head of its targeter list
+    uint32_t* s_tabO = s_tabT + HS;                                    // [HS] (position << 11) | slot whose top it is
+    uint32_t* s_bits = s_tabO + HS;                                    // [NWB] duplicate filter
+    int* s_top = reinterpret_cast<int*>(s_bits + NWB);                 // [HS] top position of every slot
+    int* s_bpref = s_top + HS;                                         // [bwords] region run prefix per block
+    int* s_bslot = s_bpref + bwords;                                   // [bwords] J slot of the run per block
+    int* s_wsum = s_bslot + bwords;                                    // [32] scan partials
+    uint16_t* s_next = reinterpret_cast<uint16_t*>(s_wsum + 32);       // [HS] list links
+    uint32_t* s_gath = reinterpret_cast<uint32_t*>(s_next + HS);       // [HS] next window's tops above
+    LT* s_otop = reinterpret_cast<LT*>(s_gath + HS);                   // [HS] original top values
+    LT* s_slab = s_otop + HS;                                          // [region_cap] the region
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int h = tid; h < 2 * HS; h += NT) s_tabT[h] = SQB_EMPTY64;  // both tables
+    for (int h = tid; h < 2 * HS; h += NT) s_tabT[h] = SQB_EMPTY32;  // both tables
     for (int w = tid; w < NWB; w += NT) s_bits[w] = 0u;
     __syncthreads();
     SQB_PCLK_START();
@@ -1354,14 +1374,14 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
     auto marked_again = [&](uint32_t pl) -> bool { return (s_bits[(pl >> 4) & (NWB - 1)] >> ((pl & 15u) * 2u + 1u)) & 1u; };
     auto push_targeter = [&](uint32_t pl, int id) -> uint32_t {
         uint32_t h = (pl * 2654435761u) >> HS_SHIFT;
-        const unsigned long long mine = ((unsigned long long)pl << 32) | (unsigned)id;
+        const uint32_t mine = (pl << SQB_PART_IDB) | (uint32_t)id;
         uint32_t nxt = SQB_NONE16;
         while (true) {
-            const unsigned long long prev = atomicCAS(&s_tabT[h], SQB_EMPTY64, mine);
-            if (prev == SQB_EMPTY64) break;
-            if ((uint32_t)(prev >> 32) == pl) {  // same position: push in front of the current head
+            const uint32_t prev = atomicCAS(&s_tabT[h], SQB_EMPTY32, mine);
+            if (prev == SQB_EMPTY32) break;
+            if ((prev >> SQB_PART_IDB) == pl) {  // same position: push in front of the current head
                 if (atomicCAS(&s_tabT[h], prev, mine) == prev) {
-                    nxt = (uint32_t)prev & 0xFFFFu;
+                    nxt = prev & SQB_PART_IDMASK;
                     break;
                 }
                 continue;
@@ -1373,16 +1393,16 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
     };
     auto insert_owner = [&](uint32_t pl, int id) -> uint32_t {  // tops are distinct: plain insertion
         uint32_t h = (pl * 2654435761u) >> HS_SHIFT;
-        const unsigned long long mine = ((unsigned long long)pl << 32) | (unsigned)id;
-        while (atomicCAS(&s_tabO[h], SQB_EMPTY64, mine) != SQB_EMPTY64) h = (h + 1) & (HS - 1);
+        const uint32_t mine = (pl << SQB_PART_IDB) | (uint32_t)id;
+        while (atomicCAS(&s_tabO[h], SQB_EMPTY32, mine) != SQB_EMPTY32) h = (h + 1) & (HS - 1);
         return h;
     };
-    auto find_key = [&](const unsigned long long* tab, uint32_t pl) -> int {
+    auto find_key = [&](const uint32_t* tab, uint32_t pl) -> int {
         uint32_t h = (pl * 2654435761u) >> HS_SHIFT;
         for (int probes = 0; probes < HS; ++probes) {
-            const unsigned long long e = tab[h];
-            if (e == SQB_EMPTY64) return -1;
-            if ((uint32_t)(e >> 32) == pl) return (int)h;
+            const uint32_t e = tab[h];
+            if (e == SQB_EMPTY32) return -1;
+            if ((e >> SQB_PART_IDB) == pl) return (int)h;
             h = (h + 1) & (HS - 1);
         }
         return -1;
@@ -1411,7 +1431,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                 const int lo = r * B;
                 const int len = min(B, m - lo);
                 const int hi = lo + len;
-                const int nblk = bt - lo / L + 1;  // <= NT (checked by the host)
+                const int nblk = bt - lo / L + 1;  // < bwords (sized by the host)
                 {  // slab <- base labels [lo, hi)
                     const LT* __restrict__ src = b0 + lo;
                     int x0 = 0;
@@ -1425,21 +1445,29 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                     }
                     for (int x = x0 + tid; x < len; x += NT) s_slab[x] = src[x];
                 }
-                {  // region r's run in every block (thread t: block bt - t), exclusive prefix over the blocks
-                    int run = 0, slot = 0;
-                    if (tid < nblk) {
-                        const int b = bt - tid;
+                {  // region r's run in every block (block index t: block bt - t), exclusive prefix over the blocks.  Thread
+                   // tid takes the consecutive block indices [tid * per, tid * per + per): a serial prefix over its own,
+                   // then one block-wide scan of the threads' sums.  A block's count row is read only as far as region r.
+                    const int per = (nblk + NT - 1) / NT;
+                    const int t0 = tid * per, t1 = min(t0 + per, nblk);
+                    int run = 0;
+                    for (int t = t0; t < t1; ++t) {
+                        const int b = bt - t;
                         const uint4* row = reinterpret_cast<const uint4*>(crow + (int64_t)b * SQB_PART_RMAX);
-                        const uint4 q0 = __ldcg(row), q1 = __ldcg(row + 1);
-                        const uint32_t w[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-                        int pre = 0;
+                        int pre = 0, c_r = 0;
+                        for (int q = 0; q <= (r >> 3); ++q) {  // regions 8q .. 8q + 7
+                            const uint4 v = __ldcg(row + q);
+                            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-                        for (int k = 0; k < SQB_PART_RMAX; ++k) {
-                            const int c = (int)((w[k >> 1] >> ((k & 1) * 16)) & 0xFFFFu);
-                            if (k < r) pre += c;
-                            if (k == r) run = c;
+                            for (int k = 0; k < 8; ++k) {
+                                const int c = (int)((w[k >> 1] >> ((k & 1) * 16)) & 0xFFFFu);
+                                if (8 * q + k < r) pre += c;
+                                if (8 * q + k == r) c_r = c;
+                            }
                         }
-                        slot = b * L + pre;
+                        s_bpref[t] = run;  // local: the thread's offset is added below
+                        s_bslot[t] = b * L + pre;
+                        run += c_r;
                     }
                     int incl = run;
 #pragma unroll
@@ -1460,19 +1488,23 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                     }
                     __syncthreads();
                     const int ex = incl - run + (warp > 0 ? s_wsum[warp - 1] : 0);
-                    if (tid < nblk) {
-                        s_bpref[tid] = ex;
-                        s_bslot[tid] = slot;
+                    for (int t = t0; t < t1; ++t) s_bpref[t] += ex;
+                    if (t0 < t1 && t1 == nblk) {  // the total, repeated into the pad words the lookup reads
+#pragma unroll
+                        for (int x = 0; x < 4; ++x) s_bpref[nblk + x] = ex + run;
                     }
-                    if (tid == nblk - 1) s_bpref[nblk] = ex + run;
                 }
                 __syncthreads();
                 const int total = s_bpref[nblk];
                 // Window slot g holds the entry at offset g - s_bpref[t] of block t's run, t = the largest t with
                 // s_bpref[t] <= g (never a block with an empty run).  A thread's slot of the next window, g + HS, lies in
-                // the same block or a later one, so the thread walks its block index forward from the last one it used.
+                // the same block or a later one, so the thread walks its block index forward from the last one it used: four
+                // blocks a step, then two and one (a window spans several blocks' runs, and each step is a dependent shared
+                // load).  t stays below nblk (s_bpref[nblk] = total > g), so the reads stop at the pad word nblk + 3.
                 auto block_of = [&](int g, int t) {
-                    while (s_bpref[t + 1] <= g) ++t;
+                    while (s_bpref[t + 4] <= g) t += 4;
+                    if (s_bpref[t + 2] <= g) t += 2;
+                    if (s_bpref[t + 1] <= g) t += 1;
                     return t;
                 };
                 auto entry = [&](int g, int t) { return __ldcs(Jb + s_bslot[t] + (g - s_bpref[t])); };
@@ -1528,16 +1560,34 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
 #pragma unroll
                     for (int k = 0; k < 2; ++k) {
                         const int s = tid + k * NT;
-                        const int g = w0 + HS + s;
                         ntop[k] = -1, njl[k] = 0;
-                        if (g < total) {
+                        if (w0 + HS + s < total) {
                             ntop[k] = (bt - jb[k]) * L + (int)(jn[k] >> 18);
                             njl[k] = jn[k] & 0x3FFFFu;
                             if (ntop[k] >= hi) gather_top(s, ntop[k]);
-                            if (g + HS < total) {
-                                jb[k] = block_of(g + HS, jb[k]);
-                                jn[k] = entry(g + HS, jb[k]);
+                        }
+                    }
+                    {  // the two slots' lookups side by side (block_of's steps, interleaved: their dependent loads overlap);
+                       // the later slot g1 needs one only if the earlier g0 does
+                        const int g0 = w0 + 2 * HS + tid, g1 = g0 + NT;
+                        if (g1 < total) {
+                            int t0 = jb[0], t1 = jb[1];
+                            while (true) {
+                                const bool a = s_bpref[t0 + 4] <= g0, b = s_bpref[t1 + 4] <= g1;
+                                if (!(a || b)) break;
+                                t0 += a ? 4 : 0;
+                                t1 += b ? 4 : 0;
                             }
+                            t0 += s_bpref[t0 + 2] <= g0 ? 2 : 0;
+                            t1 += s_bpref[t1 + 2] <= g1 ? 2 : 0;
+                            t0 += s_bpref[t0 + 1] <= g0 ? 1 : 0;
+                            t1 += s_bpref[t1 + 1] <= g1 ? 1 : 0;
+                            jb[0] = t0, jb[1] = t1;
+                            jn[0] = entry(g0, t0);
+                            jn[1] = entry(g1, t1);
+                        } else if (g0 < total) {
+                            jb[0] = block_of(g0, jb[0]);
+                            jn[0] = entry(g0, jb[0]);
                         }
                     }
                     asm volatile("cp.async.commit_group;" ::: "memory");
@@ -1591,7 +1641,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                             const int h = find_key(s_tabT, (uint32_t)(ix - lo));
                             if (h < 0) break;
                             int mx = -1;
-                            for (uint32_t e = (uint32_t)s_tabT[h] & 0xFFFFu; e != SQB_NONE16; e = s_next[e]) mx = max(mx, (int)e);
+                            for (uint32_t e = s_tabT[h] & SQB_PART_IDMASK; e != SQB_NONE16; e = s_next[e]) mx = max(mx, (int)e);
                             x = mx;  // the latest targeter of x's top (every targeter of a top precedes its step)
                         }
                         return s_otop[x];
@@ -1610,7 +1660,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                             } else {
                                 bool last = true;  // the only (or the last) slot of this window that targets the position
                                 if (stfl[k]) {
-                                    const uint32_t head = (uint32_t)s_tabT[slotT[k]] & 0xFFFFu;
+                                    const uint32_t head = s_tabT[slotT[k]] & SQB_PART_IDMASK;
                                     int mx;
                                     const int p = sqb_list_latest_before(s_next, head, s, &mx);
                                     if (p >= 0) val = T_of(p);
@@ -1629,8 +1679,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
                     // ---- the table entries of this window are cleared (ordered before the next pushes by its first barrier) ----
 #pragma unroll
                     for (int k = 0; k < 2; ++k) {
-                        if (stfl[k] && !sself[k]) s_tabT[slotT[k]] = SQB_EMPTY64;
-                        if (sofl[k]) s_tabO[slotO[k]] = SQB_EMPTY64;
+                        if (stfl[k] && !sself[k]) s_tabT[slotT[k]] = SQB_EMPTY32;
+                        if (sofl[k]) s_tabO[slotO[k]] = SQB_EMPTY32;
                     }
 #pragma unroll
                     for (int k = 0; k < 2; ++k) top[k] = ntop[k], jl[k] = njl[k];
@@ -2559,21 +2609,29 @@ static int launch_jgen(sqb_nhood* h, uint32_t* J, const uint64_t* states, int64_
     return SQB_OK;
 }
 
+// step blocks of the longest segment: sizes the region replay's per-block run tables
+static int part_max_blocks(const sqb_nhood* h) {
+    int64_t nb = 0;
+    for (int64_t m : h->h_seg_len) nb = std::max<int64_t>(nb, (m + SQB_PART_L - 1) / SQB_PART_L);
+    return (int)nb;
+}
+
 // shared memory of nhood_apply_part_kernel besides the slab:
-// [tabT, tabO u64 x HS][bits u32 x 2 HS][top int x HS][bpref int x NT + 4][bslot int x NT][wsum int x 32][next u16 x HS]
+// [tabT, tabO u32 x HS][bits u32 x 2 HS][top int x HS][bpref, bslot int x bwords][wsum int x 32][next u16 x HS]
 // [gath u32 x HS][otop LT x HS]
-static size_t part_tables_bytes(int nt, int lt_bytes) {
+static size_t part_tables_bytes(int nt, int lt_bytes, int nbmax) {
     const size_t HS = 2 * (size_t)nt;
-    return 2 * HS * 8 + 2 * HS * 4 + HS * 4 + (2 * (size_t)nt + 4) * 4 + 32 * 4 + HS * 2 + HS * 4 + HS * lt_bytes;
+    return 2 * HS * 4 + 2 * HS * 4 + HS * 4 + 2 * (size_t)sqb_part_bwords(nbmax) * 4 + 32 * 4 + HS * 2 + HS * 4 + HS * lt_bytes;
 }
 
 // positions per region of shuffle_algo 9 with nt threads and per_sm resident CTAs per SM (a multiple of 16; 0 = not even 16
-// positions fit): one CTA takes the opt-in limit of a block, two share the SM's shared memory less a block's reservation each
+// positions fit): one CTA takes the opt-in limit of a block, several share the SM's shared memory less a block's reservation
+// each
 static int64_t part_region_cap(const sqb_nhood* h, int nt, int per_sm) {
     const sqb_ctx* c = h->ctx;
     int64_t budget = (int64_t)c->smem_optin;
     if (per_sm > 1) budget = std::min(budget, (int64_t)(c->smem_per_sm / per_sm) - (int64_t)c->smem_reserved);
-    int64_t cap = (budget - (int64_t)part_tables_bytes(nt, h->lt_bytes)) / h->lt_bytes;
+    int64_t cap = (budget - (int64_t)part_tables_bytes(nt, h->lt_bytes, part_max_blocks(h))) / h->lt_bytes;
     if (cap > (1 << 18) - 16) cap = (1 << 18) - 16;                                 // region offsets are stored in 18 bits
     if (h->shuffle_region > 0 && cap > h->shuffle_region) cap = h->shuffle_region;  // test hook: small regions
     cap = (cap / 16) * 16;
@@ -2597,46 +2655,48 @@ static int part_apply_attributes(size_t smem) {
 
 // Shape of the region replay over partitioned targets (shuffle_algo 9) for np permutations; nt = 0 when it does not run.  It
 // runs when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that
-// every segment fits SQB_PART_RMAX regions and its step blocks fit one thread each; otherwise the list replay (algo 7) runs.
-// Its 32 warps spend much of a window waiting at the window's three block barriers, so the first choice is two resident
-// 512-thread CTAs per SM, each with half of the SM's shared memory (1M u8 labels: 14 regions of 71 440 positions).  When a
-// segment does not fit that (u16 labels at 1M, arrays above ~1.05M) or two such CTAs do not fit an SM, one 1024-thread CTA
-// per SM takes a block's opt-in limit (1M u8 labels: 7 regions).  shuffle_threads = 1024 with shuffle_algo 9 asks for the
-// latter.  Measured on an H100 80GB HBM3 (700 W power limit), tools/apply_time.py, 1M spots x 1000 permutations, before the
-// window loop stopped waiting on global memory: the apply took 18.4-18.5 ms with two CTAs per SM against 19.8-19.9 ms with
-// one 1024-thread CTA per SM, and 30.9 ms with 13 regions but one 512-thread CTA per SM.  At 300 K cells x 10 000
+// every segment fits SQB_PART_RMAX regions; otherwise the list replay (algo 7) runs.  Its 32 warps spend much of a window
+// waiting at the window's three block barriers, so the first choice is two resident 512-thread CTAs per SM, each with half
+// of the SM's shared memory (1M u8 labels: 12 regions of 83 344 positions; 1M u16 labels: 25 regions; u8 arrays up to about
+// 2.5M elements).  When a segment does not fit that or two such CTAs do not fit an SM, one 1024-thread CTA per SM takes a
+// block's opt-in limit (1M u8 labels: 6 regions).  shuffle_threads = 1024 with shuffle_algo 9 asks for the latter.
+// Measured on an H100 80GB HBM3 (700 W power limit), tools/apply_time.py, 1M spots x 1000 permutations, before the window
+// loop stopped waiting on global memory: the apply took 18.4-18.5 ms with two CTAs per SM against 19.8-19.9 ms with one
+// 1024-thread CTA per SM, and 30.9 ms with 13 regions but one 512-thread CTA per SM.  Four 256-thread CTAs per SM (26
+// regions of ~39 K positions, 512-slot windows) do not pay: 15.0 ms against 14.47 ms for two 512-thread CTAs with the same
+// 32-bit tables (same card, DESIGN.md §3.1), because a half-size window no longer hides its J loads.  At 300 K cells x 10 000
 // permutations (tools/apply_time.py cfg5, H100 80GB HBM3, 400 W power limit) algo 9 takes 92.5 ms against 84.2 ms for auto
 // (list replay): its apply now ties (46.2 against 46.0 ms) but its target generation costs 9 ms more, so auto keeps the list
 // replay below 512 K elements (DESIGN.md §3.1).
+// The NT-thread shape with per_sm resident CTAs per SM, when every segment fits SQB_PART_RMAX of its regions and (per_sm > 1)
+// per_sm such CTAs are resident on an SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor); out is left alone otherwise
+template <typename LT, int NT>
+static int part_try_shape(const sqb_nhood* h, int per_sm, PartShape* out) {
+    const int cap = (int)part_region_cap(h, NT, per_sm);
+    if (cap == 0) return SQB_OK;
+    for (int64_t m : h->h_seg_len) {
+        int R, B;
+        sqb_part_regions((int)m, cap, R, B);
+        if (R > SQB_PART_RMAX) return SQB_OK;
+    }
+    if (per_sm > 1) {
+        const size_t smem = part_tables_bytes(NT, (int)sizeof(LT), part_max_blocks(h)) + (size_t)cap * sizeof(LT);
+        SQB_TRY((part_apply_attributes<LT, NT>(smem)));
+        int got = 0;
+        SQB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&got, nhood_apply_part_kernel<LT, NT>, NT, smem));
+        if (got < per_sm) return SQB_OK;
+    }
+    *out = PartShape{NT, per_sm, cap};
+    return SQB_OK;
+}
+
 template <typename LT>
 static int part_replay_shape(const sqb_nhood* h, int64_t np, PartShape* out) {
     sqb_ctx* c = h->ctx;
     *out = PartShape{};
     if (h->shuffle_algo != 9 && !(h->shuffle_algo < 0 && np > 2 * (int64_t)c->sm_count && h->n >= 524288)) return SQB_OK;
-    const auto fits = [&](int nt, int cap) {
-        if (cap == 0) return false;
-        for (int64_t m : h->h_seg_len) {
-            int R, B;
-            sqb_part_regions((int)m, cap, R, B);
-            if (R > SQB_PART_RMAX || (m + SQB_PART_L - 1) / SQB_PART_L > nt) return false;
-        }
-        return true;
-    };
-    if (!(h->shuffle_algo == 9 && h->shuffle_threads == 1024)) {
-        const int cap = (int)part_region_cap(h, 512, 2);
-        if (fits(512, cap)) {
-            const size_t smem = part_tables_bytes(512, (int)sizeof(LT)) + (size_t)cap * sizeof(LT);
-            SQB_TRY((part_apply_attributes<LT, 512>(smem)));
-            int per_sm = 0;
-            SQB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nhood_apply_part_kernel<LT, 512>, 512, smem));
-            if (per_sm >= 2) {
-                *out = PartShape{512, 2, cap};
-                return SQB_OK;
-            }
-        }
-    }
-    const int cap = (int)part_region_cap(h, 1024, 1);
-    if (fits(1024, cap)) *out = PartShape{1024, 1, cap};
+    if (!(h->shuffle_algo == 9 && h->shuffle_threads == 1024)) SQB_TRY((part_try_shape<LT, 512>(h, 2, out)));
+    if (!out->nt) SQB_TRY((part_try_shape<LT, 1024>(h, 1, out)));
     return SQB_OK;
 }
 
@@ -2644,14 +2704,15 @@ template <typename LT, int NT>
 static int launch_apply_part(sqb_nhood* h, LT* lab, const uint32_t* J, const uint16_t* cnt, int64_t nb_total, const PartShape& ps,
                              int64_t np) {
     sqb_ctx* c = h->ctx;
-    const size_t smem = part_tables_bytes(NT, (int)sizeof(LT)) + (size_t)ps.cap * sizeof(LT);
+    const int nbmax = part_max_blocks(h);
+    const size_t smem = part_tables_bytes(NT, (int)sizeof(LT), nbmax) + (size_t)ps.cap * sizeof(LT);
     SQB_TRY((part_apply_attributes<LT, NT>(smem)));
     int64_t grid = h->shuffle_ctas;
     if (grid <= 0) grid = (int64_t)ps.per_sm * c->sm_count;  // every CTA resident, persistent over the permutations
     if (grid > np) grid = np;
     nhood_apply_part_kernel<LT, NT><<<(unsigned)grid, NT, smem, c->stream>>>(
         lab, J, cnt, reinterpret_cast<const LT*>(h->d_base.p), h->stride, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, nb_total,
-        ps.cap);
+        ps.cap, sqb_part_bwords(nbmax));
     return SQB_OK;
 }
 

@@ -18,15 +18,25 @@
 //           z'Wz   = A - m * (D - m*(S0 - E) - B)        A = sum_S z_i acc_i, B = sum_S acc_i,
 //                                                         D = sum_S c_j z_j,   E = sum_S c_j
 //           sum z^2 = sum_S z_i^2 + (N - |S|) m^2
-//        (every term is formed from centred values, so nothing of order m^2*N is subtracted from something of the same
-//        size except S0 - E, which is exact when nothing is stored and ~0 when everything is);  Geary likewise:
+//        Geary likewise:
 //           sum_ij w_ij (x_i-x_j)^2 = sum_{i in S} sum_j w_ij [(x_i-x_j)^2 - [j in S] x_j^2] + sum_{j in S} c_j x_j^2.
+//        The correction terms are NOT centred: Moran's carries m^2 * (S0 - E), Geary's two sums of size S0 * m^2.  When
+//        every observation is stored they are 0 in exact arithmetic and rounding noise times m^2 in float64, which swamps
+//        the result once m >> std(x).  A feature stored at every observation (|S| = N: uniform per CTA, and true for every
+//        row permutation) therefore takes num = A for Moran, and for Geary every value is shifted by m (the terms are
+//        translation invariant, so they become centred); the other features keep the formulas above, instruction for
+//        instruction.  Features stored at all but a few observations keep the uncentred terms (~1e-11 of the result).
+//     4. constant feature -> NaN: the definition is 0/0, and the rounded mean of a constant is not always the constant (then
+//        every z is the same tiny delta and I comes out ~1, C 0).  It is decided by exact comparison, not by sum z^2 == 0:
+//        stored at every observation with all values equal (found by the rank sort at load time; sum z^2 is then taken as
+//        its exact value, 0), or every stored value 0 (m = 0 exactly, so sum z^2 is 0 already).
 //   A row permutation of W (g[idx, :], the permutation variant) changes neither c nor S0; D, E, sum z^2, m and the
 //   Geary column term are kept per feature from the unpermuted pass.
 //   Reductions are fixed-order (entry -> lane assignment, shuffle tree, sequential combine over warps) and one CTA
 //   owns a feature whatever the grid size: results are bit-reproducible run to run and GPU to GPU.
 // DENSE X keeps the tile formulation of round 1: features in tiles of 32 (lane = feature), a dense [N][32] slab per
-//   tile, W streamed once per tile.
+//   tile, W streamed once per tile.  Every term is centred there; a feature whose values are all equal (found next to the
+//   column sums) is NaN.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cuda_fp16.h>
@@ -64,9 +74,11 @@ __global__ void ac_transpose_kernel(const XT* __restrict__ x, int64_t g0, int64_
 }
 
 // ---- column sums of a dense tile (fixed order): partial[tile][warp][lane] --------------------------------
+// pdiff[tile][warp][lane]: does any value of the warp's range differ from the feature's first value (constant features)
 template <typename XT>
 __global__ void ac_colsum_kernel(const XT* __restrict__ D, int64_t pitch, int64_t tile_stride, int64_t n,
-                                 int64_t obs_per_warp, double* __restrict__ partial, int64_t g0, int64_t n_feat) {
+                                 int64_t obs_per_warp, double* __restrict__ partial, int* __restrict__ pdiff, int64_t g0,
+                                 int64_t n_feat) {
     const int lane = threadIdx.x & 31;
     const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -76,17 +88,32 @@ __global__ void ac_colsum_kernel(const XT* __restrict__ D, int64_t pitch, int64_
     int64_t r0 = w * obs_per_warp, r1 = r0 + obs_per_warp;
     if (r1 > n) r1 = n;
     double s = 0.0;
-    if (valid)
-        for (int64_t r = r0; r < r1; ++r) s += (double)Dt[r * pitch + lane];
+    int differs = 0;
+    if (valid) {
+        const XT x0 = Dt[lane];
+        for (int64_t r = r0; r < r1; ++r) {
+            const XT x = Dt[r * pitch + lane];
+            s += (double)x;
+            differs |= x != x0;
+        }
+    }
     partial[(tl * nw + w) * TILE + lane] = s;
+    pdiff[(tl * nw + w) * TILE + lane] = differs;
 }
 
-__global__ void ac_colsum_final_kernel(const double* __restrict__ partial, int64_t nw, double* __restrict__ sums) {
+// sums[tile][lane] = column sum; varies[tile][lane] = 0 when every value of the feature is equal
+__global__ void ac_colsum_final_kernel(const double* __restrict__ partial, const int* __restrict__ pdiff, int64_t nw,
+                                       double* __restrict__ sums, int* __restrict__ varies) {
     const int lane = threadIdx.x;
     const int64_t tl = blockIdx.x;
     double s = 0.0;
-    for (int64_t w = 0; w < nw; ++w) s += partial[(tl * nw + w) * TILE + lane];
+    int d = 0;
+    for (int64_t w = 0; w < nw; ++w) {
+        s += partial[(tl * nw + w) * TILE + lane];
+        d |= pdiff[(tl * nw + w) * TILE + lane];
+    }
     sums[tl * TILE + lane] = s;
+    varies[tl * TILE + lane] = d;
 }
 
 // ---- dense SpMM-style kernel -----------------------------------------------------------------------------
@@ -151,8 +178,8 @@ __global__ void __launch_bounds__(256) ac_main_kernel(const int32_t* __restrict_
 
 template <int MODE>
 __global__ void __launch_bounds__(256) ac_final_kernel(const double* __restrict__ pnum, const double* __restrict__ pden,
-                                                       int64_t nparts, int64_t n, double s0, int64_t g0, int64_t n_feat,
-                                                       double* __restrict__ out) {
+                                                       const int* __restrict__ varies, int64_t nparts, int64_t n, double s0,
+                                                       int64_t g0, int64_t n_feat, double* __restrict__ out) {
     // 8 warps sum contiguous ranges of the per-CTA partials (lane = feature), then warp 0 combines them in order
     __shared__ double s_num[8][TILE], s_den[8][TILE];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -178,8 +205,8 @@ __global__ void __launch_bounds__(256) ac_final_kernel(const double* __restrict_
         den += s_den[k][lane];
     }
     double r;
-    if (den == 0.0) {
-        r = __longlong_as_double(0x7ff8000000000000LL);  // constant feature -> NaN (scanpy)
+    if (den == 0.0 || !varies[tl * TILE + lane]) {
+        r = __longlong_as_double(0x7ff8000000000000LL);  // constant feature -> NaN (0/0; the rounded mean need not be the value)
     } else if (MODE == 0) {
         r = (double)n / s0 * num / den;
     } else {
@@ -399,13 +426,15 @@ __device__ __forceinline__ unsigned int ac_scan_words(uint2* S, int nwords, unsi
 
 // One CTA per feature: order the (observation, value) pairs of a segment by observation (rank = number of stored
 // observations below), write them to the padded segment, pad with index -1 / value 0.  Out-of-range or repeated
-// observation indices raise the error flag.  Segment g is in_idx / in_val [in_beg[g], in_end[g]).
+// observation indices raise the error flag.  Segment g is in_idx / in_val [in_beg[g], in_end[g]).  seg_const[g] = 1 when the
+// feature is stored at every observation with every value equal.
 template <typename II, typename VT, typename XT>
 __global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __restrict__ in_beg, const int64_t* __restrict__ in_end,
                                                              const II* __restrict__ in_idx, const VT* __restrict__ in_val,
                                                              const int64_t* __restrict__ out_start,
                                                              int32_t* __restrict__ out_idx, XT* __restrict__ out_val,
-                                                             int32_t* __restrict__ seg_len, int64_t n, int64_t n_feat,
+                                                             int32_t* __restrict__ seg_len, int32_t* __restrict__ seg_const,
+                                                             int64_t n, int64_t n_feat,
                                                              int nwords, uint2* __restrict__ s_global, int* __restrict__ err) {
     extern __shared__ __align__(16) unsigned char ac_smem[];
     __shared__ unsigned int s_tmp[AC_NW + 1];
@@ -447,7 +476,15 @@ __global__ void __launch_bounds__(AC_T) ac_rank_sort_kernel(const int64_t* __res
             out_idx[os + e] = -1;
             out_val[os + e] = (XT)0;
         }
-        if (threadIdx.x == 0) seg_len[g] = len;
+        // stored at every observation with all values equal: a constant feature (0/0), whatever its rounded mean is
+        int differs = 0;
+        if (len == n)
+            for (int e = threadIdx.x; e < len; e += AC_T) differs |= sqb_cvt<XT>(in_val[rb + e]) != sqb_cvt<XT>(in_val[rb]);
+        const int varies = __syncthreads_or(differs);
+        if (threadIdx.x == 0) {
+            seg_len[g] = len;
+            seg_const[g] = len == n && !varies;
+        }
         __syncthreads();
         ac_zero_words(S, nwords);
         __syncthreads();
@@ -502,6 +539,7 @@ struct AcSparseParams {
     uint2* s_global;  // bitmap scratch in global memory (nwords per CTA) when it does not fit shared memory, else null
     const int64_t* seg_start;
     const int32_t* seg_len;
+    const int32_t* seg_const;  // 1: stored at every observation, every value equal (set by the rank sort)
     const int32_t* order;  // features by decreasing length (longest first), or null
     const int32_t* xi;
     const void* xv;
@@ -514,7 +552,8 @@ struct AcSparseParams {
     double s0;
     const int32_t* perm;  // PERM: n_perm row permutations [n_perm][n] (one feature pass serves all of them), else null
     int n_perm;           // PERM: permutations per launch; outputs go to out[b * n_feat + g]
-    double* aux;          // [5][n_feat]: mean, sum z^2 over stored, D, E, Geary column term (written by unpermuted runs)
+    double* aux;          // [5][n_feat]: mean, sum z^2 over stored, D, E, Geary column term (written by unpermuted runs; the
+                          // column term depends on the mode, so permuted runs read it only after one of their own mode)
     double* out;
     int* counter;  // dynamic feature queue
 };
@@ -568,6 +607,7 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
         const int g = p.order ? p.order[k] : k;
         const int64_t b = p.seg_start[g];
         const int len = p.seg_len[g];
+        const bool full = len == p.n;  // every observation stored: no correction term (see the header)
         const int32_t* __restrict__ xi = p.xi + b;
         const XT* __restrict__ xv = reinterpret_cast<const XT*>(p.xv) + b;
         const int len4 = (len + 3) >> 2;
@@ -642,13 +682,17 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
                     q[2] = fma(cs[t], zi, q[2]);
                     q[3] += cs[t];
                     q[4] = fma(zi, zi, q[4]);
-                    q[5] = fma(cs[t], xs[t] * xs[t], q[5]);
+                    const double xg = MODE == 1 && full ? zi : xs[t];  // Geary's shift (gs below): aux depends on the mode
+                    q[5] = fma(cs[t], xg * xg, q[5]);
                 }
             }
         } else {
             m = p.aux[g];
             __syncthreads();
         }
+        // Geary's terms are translation invariant: a feature stored everywhere is shifted by m (every term centred, nothing of
+        // size S0 * m^2 cancels); the others keep x, whose unstored values are the 0 the column-sum term assumes
+        const double gs = full ? m : 0.0;
         // ---- phase 2: walk the rows of W of the stored observations; q[0], q[1] = slot accumulators ----
         // Moran: q[0] += z_i * w z_j, q[1] += w z_j;   Geary: q[0] += w ((x_i - x_j)^2 - [j stored] x_j^2)
         // PERM: the bitmap of the feature is built once and walked once per row permutation of the batch
@@ -727,7 +771,8 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
                             q[1] += t;
                         } else {
                             const double d = rx[s] - xjd;
-                            q[0] = fma(w, d * d - xjd * xjd, q[0]);  // xj == 0 when not stored
+                            const double xg = xjd - gs;
+                            q[0] = fma(w, d * d - xg * xg, q[0]);  // xj == 0 when not stored
                         }
                     }
                 } else {
@@ -756,7 +801,8 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
                                 q[1] += t;
                             } else {
                                 const double d = rx[s] - xjd;
-                                q[0] = fma(w, d * d - xjd * xjd, q[0]);
+                                const double xg = xjd - gs;
+                                q[0] = fma(w, d * d - xg * xg, q[0]);
                             }
                         }
                     }
@@ -775,7 +821,7 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
         if (threadIdx.x == 0) {
             double D, E, Z2, CX;
             if (!PERM) {
-                D = q[2], E = q[3], Z2 = q[4], CX = q[5];
+                D = q[2], E = q[3], Z2 = p.seg_const[g] ? 0.0 : q[4], CX = q[5];  // a constant's sum z^2 is exactly 0 (aux keeps it)
                 p.aux[g] = m;
                 p.aux[p.n_feat + g] = Z2;
                 p.aux[2 * p.n_feat + g] = D;
@@ -790,9 +836,9 @@ __global__ void __launch_bounds__(AC_T, GRP == 8 ? 3 : 4) ac_sparse_kernel(const
             const double den = Z2 + (dn - (double)len) * m * m;
             double r;
             if (den == 0.0) {
-                r = __longlong_as_double(0x7ff8000000000000LL);  // constant feature -> NaN (scanpy)
+                r = __longlong_as_double(0x7ff8000000000000LL);  // constant feature -> NaN (0/0)
             } else if (MODE == 0) {
-                const double num = q[0] - m * (D - m * (p.s0 - E) - q[1]);
+                const double num = full ? q[0] : q[0] - m * (D - m * (p.s0 - E) - q[1]);
                 r = dn / p.s0 * num / den;
             } else {
                 const double num = q[0] + CX;
@@ -833,16 +879,18 @@ struct sqb_autocorr {
     int64_t n_feat = 0;
     DevBuf<uint8_t> d_x{ctx->stream};   // dense matrix or padded sparse values
     DevBuf<int64_t> d_xp{ctx->stream};  // padded segment starts (n_feat + 1)
-    DevBuf<int32_t> d_xi{ctx->stream}, d_len{ctx->stream}, d_order{ctx->stream};
+    DevBuf<int32_t> d_xi{ctx->stream}, d_len{ctx->stream}, d_const{ctx->stream}, d_order{ctx->stream};
     DevBuf<uint8_t> d_tile{ctx->stream};
     DevBuf<double> d_sums{ctx->stream}, d_partial{ctx->stream}, d_pnum{ctx->stream}, d_pden{ctx->stream}, d_out{ctx->stream}, d_aux{ctx->stream},
         d_out_perms{ctx->stream};
+    DevBuf<int> d_pdiff{ctx->stream}, d_varies{ctx->stream};  // dense path: constant-feature flags (per warp, per feature)
     DevBuf<int64_t> d_perm{ctx->stream};
     DevBuf<int32_t> d_perm32{ctx->stream};
     DevBuf<unsigned int> d_seen{ctx->stream};
     DevBuf<uint2> d_bitmap{ctx->stream};  // global-memory bitmap scratch (large n)
     DevBuf<int> d_flags{ctx->stream};     // [0] error flags, [1] feature queue counter
-    bool aux_valid = false;
+    bool aux_valid = false;  // d_aux holds the invariants of the loaded X, written by an unpermuted run of mode aux_mode
+    int aux_mode = 0;
     int tiles_per_launch = 8;  // dense path: 256 features per launch
     bool ran = false;
 };
@@ -922,6 +970,7 @@ static int ac_run_sparse(sqb_autocorr* h, int mode, const int32_t* d_perm32, dou
     p.n_feat = h->n_feat;
     p.seg_start = h->d_xp.p;
     p.seg_len = h->d_len.p;
+    p.seg_const = h->d_const.p;
     p.order = h->d_order.p;
     p.xi = h->d_xi.p;
     p.xv = h->d_x.p;
@@ -943,7 +992,10 @@ static int ac_run_sparse(sqb_autocorr* h, int mode, const int32_t* d_perm32, dou
             rc = f32 ? ac_sparse_fmt<float, 0, false>(h, p) : ac_sparse_fmt<double, 0, false>(h, p);
         else
             rc = f32 ? ac_sparse_fmt<float, 1, false>(h, p) : ac_sparse_fmt<double, 1, false>(h, p);
-        if (rc == SQB_OK) h->aux_valid = true;
+        if (rc == SQB_OK) {
+            h->aux_valid = true;
+            h->aux_mode = mode;
+        }
         return rc;
     }
     if (mode == 0) return f32 ? ac_sparse_fmt<float, 0, true>(h, p) : ac_sparse_fmt<double, 0, true>(h, p);
@@ -966,6 +1018,8 @@ static int ac_run_dense(sqb_autocorr* h, int mode, const int64_t* d_perm) {
     nw = ctas * 8;
     SQB_TRY(h->d_sums.alloc((size_t)TPL * TILE));
     SQB_TRY(h->d_partial.alloc((size_t)TPL * nw * TILE));
+    SQB_TRY(h->d_pdiff.alloc((size_t)TPL * nw * TILE));
+    SQB_TRY(h->d_varies.alloc((size_t)TPL * TILE));
     SQB_TRY(h->d_pnum.alloc((size_t)TPL * nw * TILE));
     SQB_TRY(h->d_pden.alloc((size_t)TPL * nw * TILE));
     const bool zero_copy = (h->kind == 2);
@@ -993,12 +1047,12 @@ static int ac_run_dense(sqb_autocorr* h, int mode, const int64_t* d_perm) {
         {
             SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
             dim3 grid((unsigned)ctas, (unsigned)nt);
-            ac_colsum_kernel<XT><<<grid, 256, 0, c->stream>>>(D, pitch, tile_stride, n, obs_per_warp, h->d_partial.p, g0, G);
+            ac_colsum_kernel<XT><<<grid, 256, 0, c->stream>>>(D, pitch, tile_stride, n, obs_per_warp, h->d_partial.p, h->d_pdiff.p, g0, G);
             SQB_POST_LAUNCH();
         }
         {
             SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            ac_colsum_final_kernel<<<nt, 32, 0, c->stream>>>(h->d_partial.p, nw, h->d_sums.p);
+            ac_colsum_final_kernel<<<nt, 32, 0, c->stream>>>(h->d_partial.p, h->d_pdiff.p, nw, h->d_sums.p, h->d_varies.p);
             SQB_POST_LAUNCH();
         }
         {
@@ -1017,9 +1071,9 @@ static int ac_run_dense(sqb_autocorr* h, int mode, const int64_t* d_perm) {
         {
             SqbLaunchScope scope(c, SQB_K_AUTOCORR_FINAL);
             if (mode == 0)
-                ac_final_kernel<0><<<nt, 256, 0, c->stream>>>(h->d_pnum.p, h->d_pden.p, ctas, n, h->s0, g0, G, h->d_out.p);
+                ac_final_kernel<0><<<nt, 256, 0, c->stream>>>(h->d_pnum.p, h->d_pden.p, h->d_varies.p, ctas, n, h->s0, g0, G, h->d_out.p);
             else
-                ac_final_kernel<1><<<nt, 256, 0, c->stream>>>(h->d_pnum.p, h->d_pden.p, ctas, n, h->s0, g0, G, h->d_out.p);
+                ac_final_kernel<1><<<nt, 256, 0, c->stream>>>(h->d_pnum.p, h->d_pden.p, h->d_varies.p, ctas, n, h->s0, g0, G, h->d_out.p);
             SQB_POST_LAUNCH();
         }
     }
@@ -1050,6 +1104,7 @@ static int ac_build_segments(sqb_autocorr* h, const int64_t* d_beg, const int64_
     SQB_TRY(h->d_xi.alloc((size_t)cap));
     SQB_TRY(h->d_x.alloc((size_t)cap * sizeof(XT)));
     SQB_TRY(h->d_len.alloc((size_t)n_feat));
+    SQB_TRY(h->d_const.alloc((size_t)n_feat));
     SQB_TRY(h->d_order.alloc((size_t)n_feat));
     SQB_TRY(h->d_aux.alloc((size_t)5 * n_feat));
     SQB_TRY(h->d_out.alloc((size_t)n_feat));
@@ -1060,7 +1115,7 @@ static int ac_build_segments(sqb_autocorr* h, const int64_t* d_beg, const int64_
     {
         SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
         ac_rank_sort_kernel<II, VT, XT><<<(unsigned)ctas, AC_T, geo.smem, c->stream>>>(
-            d_beg, d_end, d_idx, d_val, d_pad, h->d_xi.p, reinterpret_cast<XT*>(h->d_x.p), h->d_len.p, h->n, n_feat, geo.nwords,
+            d_beg, d_end, d_idx, d_val, d_pad, h->d_xi.p, reinterpret_cast<XT*>(h->d_x.p), h->d_len.p, h->d_const.p, h->n, n_feat, geo.nwords,
             geo.global ? h->d_bitmap.p : nullptr, h->d_flags.p);
         SQB_POST_LAUNCH();
     }
@@ -1498,9 +1553,12 @@ static int ac_upload_perms(sqb_autocorr* h, const int64_t* row_perm, int64_t cou
     return SQB_OK;
 }
 
+// the per-feature invariants a permuted sparse run reads are those of an unpermuted run of the same mode
+static bool ac_aux_ready(const sqb_autocorr* h, int mode) { return h->aux_valid && h->aux_mode == mode; }
+
 static int ac_run_one(sqb_autocorr* h, int mode, int64_t perm_index /* -1: none */, double* d_out) {
     if (h->kind == 3) {
-        if (perm_index >= 0 && !h->aux_valid) SQB_TRY(ac_run_sparse(h, mode, nullptr, h->d_out.p));
+        if (perm_index >= 0 && !ac_aux_ready(h, mode)) SQB_TRY(ac_run_sparse(h, mode, nullptr, h->d_out.p));
         return ac_run_sparse(h, mode, perm_index >= 0 ? h->d_perm32.p + perm_index * h->n : nullptr, d_out);
     }
     const int64_t* dp = perm_index >= 0 ? h->d_perm.p + perm_index * h->n : nullptr;
@@ -1550,7 +1608,7 @@ int sqb_autocorr_run_perms(sqb_autocorr* h, int mode, const int64_t* row_perms, 
         const int64_t pb = n_perms - p0 < batch ? n_perms - p0 : batch;
         SQB_TRY(ac_upload_perms(h, row_perms + p0 * h->n, pb));
         if (h->kind == 3) {  // sparse X: one launch scores the whole batch (the feature's bitmap is built once per batch)
-            if (!h->aux_valid) SQB_TRY(ac_run_sparse(h, mode, nullptr, h->d_out.p));
+            if (!ac_aux_ready(h, mode)) SQB_TRY(ac_run_sparse(h, mode, nullptr, h->d_out.p));
             SQB_TRY(ac_run_sparse(h, mode, h->d_perm32.p, h->d_out_perms.p, (int)pb));
         } else {
             for (int64_t k = 0; k < pb; ++k) SQB_TRY(ac_run_one(h, mode, k, h->d_out_perms.p + k * G));

@@ -132,3 +132,55 @@ def dense_longdouble(w: sp.spmatrix, x: np.ndarray) -> tuple[float, float]:
     z2 = (z * z).sum()
     diff = xl[:, None] - xl[None, :]
     return float(n / s0 * (z @ (wd @ z)) / z2), float((n - 1) * (wd * diff * diff).sum() / (2 * s0 * z2))
+
+
+def _longdouble_terms(w: sp.spmatrix, x: np.ndarray):
+    """W's stored entries (rows, cols, weights) and the centred feature, all in ``np.longdouble``.  The mean is kept as
+    two parts, ``mean + low`` with ``low`` the mean of the residuals: a single long double holds a mean of 1e6 only to
+    ~1e-13, which would shift every z by that much; with the second part z is accurate to its own long-double epsilon."""
+    w = sp.csr_matrix(w)
+    n = w.shape[0]
+    xl = np.asarray(x, dtype=np.longdouble).ravel()
+    mean = xl.sum() / n
+    low = (xl - mean).sum() / n
+    rows = np.repeat(np.arange(n), np.diff(w.indptr))
+    return w, rows, w.indices, w.data.astype(np.longdouble), xl, mean, (xl - mean) - low
+
+
+def sparse_longdouble(w: sp.spmatrix, x: np.ndarray) -> tuple[float, float]:
+    """(I, C) of one feature: the definition over the stored entries of ``w`` in ``np.longdouble``, never densified (N = 1M
+    takes about a second).  ``(Wz)_i`` is summed per row; Geary's numerator comes straight from the differences
+    ``x_i - x_j``.  A constant feature (every value equal, compared exactly) is the definition's 0/0: NaN."""
+    w, rows, cols, wd, xl, _, z = _longdouble_terms(w, x)
+    n = w.shape[0]
+    if xl.min() == xl.max():
+        return float("nan"), float("nan")
+    s0 = wd.sum()
+    z2 = (z * z).sum()
+    wz = np.zeros(n, dtype=np.longdouble)
+    full = np.diff(w.indptr) > 0
+    if w.nnz:
+        wz[full] = np.add.reduceat(wd * z[cols], w.indptr[:-1][full])
+    diff = xl[rows] - xl[cols]
+    return float(n / s0 * (z * wz).sum() / z2), float((n - 1) * (wd * diff * diff).sum() / (2 * s0 * z2))
+
+
+def autocorr_scale(w: sp.spmatrix, x: np.ndarray) -> tuple[float, float]:
+    """First-order error scale of a float64 evaluation of (I, C): the sum of |partial derivative| x |operand| over the
+    rounded operations, so that a careful evaluation is off by a modest multiple of eps x scale.  A test bounds
+    ``|got - ref| <= k * scale`` where I or C is near 0 and a relative bound means nothing.
+
+    I: ``(N/S0) * (sum |w_ij||z_i||z_j| + |m| * |sum_ij w_ij (z_i + z_j)|) / sum z^2``.  The first term covers the rounding of
+    every product and partial sum.  The second covers the mean: ``sum x / N`` in float64 is off by about eps * |m|, which
+    shifts every z by the same amount and moves ``z'Wz`` by that shift times ``sum_ij w_ij (z_i + z_j)``; ``sum z^2`` moves
+    only at second order.  Without it no float64 evaluation could meet the bound once |m| >> std(x).
+    C: ``(N-1) * sum |w_ij| (x_i - x_j)^2 / (2 * S0 * sum z^2)``; the differences do not involve the mean, and for
+    non-negative weights this is C itself."""
+    w, rows, cols, wd, xl, mean, z = _longdouble_terms(w, x)
+    n = w.shape[0]
+    s0 = wd.sum()
+    z2 = (z * z).sum()
+    aw = np.abs(wd)
+    si = (aw * np.abs(z[rows]) * np.abs(z[cols])).sum() + abs(mean) * abs((wd * (z[rows] + z[cols])).sum())
+    diff = xl[rows] - xl[cols]
+    return float(n / abs(s0) * si / z2), float((n - 1) * (aw * diff * diff).sum() / (2 * abs(s0) * z2))

@@ -70,6 +70,58 @@ def test_constant_feature_is_nan():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# CPU: the scalable long-double reference the GPU conditioning suite compares with
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("offset", [0.0, 1e2, 1e6, 1e12])
+def test_sparse_longdouble_vs_exact(offset):
+    """The closed-form cases, the asymmetric graphs (an empty row, an isolated source) and a feature far from 0 (the exact
+    value of the definition does not care where the mean lies; a float64 evaluation does)."""
+    cases = [(w, x) for _, w, x, _, _ in ka.CASES]
+    w, x = _random_asymmetric()
+    cases += [(w, row) for row in x] + [(w.astype(np.float64) * 0.7, x[2])]
+    for w, x in cases:
+        xo = np.asarray(x, dtype=np.float64) + offset
+        exp = ka.exact_autocorr(w, xo)
+        np.testing.assert_allclose(ka.sparse_longdouble(w, xo), exp, rtol=1e-15, atol=1e-16)
+        si, sc = ka.autocorr_scale(w, xo)
+        assert si >= abs(exp[0]) * (1 - 1e-12) and sc >= abs(exp[1]) * (1 - 1e-12)  # the scale bounds the value itself
+
+
+def test_sparse_longdouble_vs_dense_on_dummy_adata(golden_dummy):
+    from sklearn.preprocessing import normalize
+
+    g = sp.csr_matrix((golden_dummy["adj_data"], golden_dummy["adj_indices"], golden_dummy["adj_indptr"]), shape=(200, 200))
+    gn = g.astype(np.float32).copy()
+    normalize(gn, norm="l1", axis=1, copy=False)
+    X = golden_dummy["X"]
+    for w in (g, gn):
+        for k in range(X.shape[1]):
+            np.testing.assert_allclose(ka.sparse_longdouble(w, X[:, k]), ka.dense_longdouble(w, X[:, k]), rtol=1e-15, atol=1e-17)
+
+
+@pytest.mark.parametrize("value", [0.1, float(np.float32(0.1)), 1.0 / 3.0, -7.3, 0.0, 3.25])
+def test_sparse_longdouble_constant_is_nan(value):
+    w = ka.torus_grid(6)
+    assert np.isnan(ka.sparse_longdouble(w, np.full(36, value))).all()
+    x = np.full(36, value)
+    x[7] = np.nextafter(value, np.inf)  # one ulp away: no longer constant, the definition is finite
+    assert np.isfinite(ka.sparse_longdouble(w, x)).all()
+
+
+def test_sparse_longdouble_million_observations_is_fast():
+    import time
+
+    from tools import synth
+
+    g = synth.hex_graph(1000, 1000)
+    x = 1e6 + np.random.default_rng(0).normal(size=g.shape[0])
+    t = time.perf_counter()
+    i, c = ka.sparse_longdouble(g, x)
+    assert time.perf_counter() - t < 30.0
+    assert abs(i) < 0.01 and abs(c - 1.0) < 0.01  # white noise: I ~ -1/(N-1), C ~ 1
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # GPU: the CUDA kernels (dense tiles and the sparse per-feature kernel) against the same known answers
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu

@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 8
+#define SQB_ABI_VERSION 9
 
 typedef enum {
     SQB_OK = 0,
@@ -50,7 +50,8 @@ typedef enum {
     SQB_ERR_CUDA = -2,    /* CUDA runtime / launch failure */
     SQB_ERR_OOM = -3,     /* device allocation failed */
     SQB_ERR_UNSUPPORTED = -4,
-    SQB_ERR_STATE = -5 /* call sequence error (e.g. run before upload) */
+    SQB_ERR_STATE = -5, /* call sequence error (e.g. run before upload) */
+    SQB_ERR_LAYOUT = -6 /* a valid input in a layout the entry point does not take (message says which): use another path */
 } sqb_status;
 
 typedef struct sqb_ctx sqb_ctx;
@@ -256,6 +257,23 @@ int sqb_sepal_dense(const sqb_dense* x, const int32_t* sat, int64_t n_sat, const
  * sorted.  Index ranges, indptr monotonicity and duplicates are checked on the device (SQB_ERR_INVALID).   */
 int sqb_autocorr_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const int32_t* w_indptr, const int32_t* w_indices,
                         const void* w_data, int w_dtype, sqb_autocorr** out);
+/* The same from a weight matrix already in device memory (e.g. a torch sparse_csr or cupyx CSR of the caller), read in place
+ * and never on the host: indptr (n + 1 entries), indices and data (nnz) are DEVICE pointers on the context's device,
+ * indptr_bits / index_bits 32 or 64, value_code 0 = f32, 1 = f64.  Every row must be canonical (strictly increasing column
+ * indices): indptr is checked first (SQB_ERR_INVALID unless it runs from 0 to nnz without decreasing), then every index must
+ * lie in [0, n) (SQB_ERR_INVALID) and every row be canonical (SQB_ERR_LAYOUT: take the host path).  transformation != 0
+ * row-normalises W like sklearn's normalize(W, norm="l1", axis=1) in W's dtype; NaN or infinite weights, which normalize rejects,
+ * then return SQB_ERR_LAYOUT too.  data holds exactly nnz contiguous values.  The handle's W then equals, bit for bit, what
+ * sqb_autocorr_create builds from the same (normalised) host CSR.  out_moments (host, 3): s0, s1, s2 of the normalised W
+ * (_g_moments of the reference, src/squidpy/gr/_ppatterns.py:541-559) evaluated in W's dtype in scipy's operation order,
+ * converted exactly to double.  producer_stream: as in sqb_autocorr_load_csr_device.  Returns after the device has stopped
+ * reading the caller's buffers; on an error no handle is returned and the context stays usable.                             */
+int sqb_autocorr_create_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
+                               int index_bits, const void* data, int value_code, int transformation, uintptr_t producer_stream,
+                               double* out_moments, sqb_autocorr** out);
+/* How the handle's W is held: *w_format 0 packed rows of 8 slots, 1 packed rows of 16, 2 CSR walk, 3 compact rows (7 columns +
+ * one common float32 weight); *s0_branch 0 = S0 summed exactly as an integer sum in parallel, 1 = one ordered thread.          */
+int sqb_autocorr_w_info(sqb_autocorr* h, int* w_format, int* s0_branch);
 int sqb_autocorr_destroy(sqb_autocorr* h);
 int sqb_autocorr_load_dense(sqb_autocorr* h, const void* x, int x_dtype, int layout, int64_t n_features);
 int sqb_autocorr_load_csr(sqb_autocorr* h, const int64_t* x_indptr, const int32_t* x_indices, const void* x_data,

@@ -208,6 +208,26 @@ def graph_args(d: DevSparse, n_obs: int) -> DevGraph:
     return DevGraph(d, n_obs, nnz, ip_bits, ix_bits, d.format == "csc", common_stream(d))
 
 
+def _contiguous_1d(a: DevArray, size: int | None = None) -> bool:
+    return len(a.shape) == 1 and (size is None or a.shape[0] == size) and (a.shape[0] <= 1 or a.strides[0] == 1)
+
+
+def weight_graph_args(d: DevArray | DevSparse | None, n_obs: int) -> DevGraph | None:
+    """The ``DevGraph`` of a device weight matrix that ``sqb_autocorr_create_device`` reads in place: an ``n_obs x n_obs`` CSR
+    with contiguous int32 / int64 ``indptr`` (``n_obs + 1`` entries) and ``indices``, and a contiguous float32 / float64 ``data``
+    of exactly as many entries.  ``None`` for anything else (host, dense or CSC matrices, other dtypes, strided or mis-sized
+    arrays): spatial_autocorr then copies the matrix to the host as it does for every other weight matrix."""
+    if not isinstance(d, DevSparse) or d.format != "csr" or tuple(d.shape) != (n_obs, n_obs):
+        return None
+    ints = (np.dtype(np.int32), np.dtype(np.int64))
+    if d.indptr.dtype not in ints or d.indices.dtype not in ints or d.data.dtype not in (np.dtype(np.float32), np.dtype(np.float64)):
+        return None
+    nnz = d.indices.shape[0] if len(d.indices.shape) == 1 else -1
+    if not (_contiguous_1d(d.indptr, n_obs + 1) and _contiguous_1d(d.indices) and _contiguous_1d(d.data, nnz)):
+        return None
+    return graph_args(d, n_obs)
+
+
 # value dtype code of sqb_interaction_matrix_device: the autocorr codes plus bool (one byte per value)
 GRAPH_VALUE_CODES = {**DTYPE_CODES, np.dtype(np.bool_): 5}
 

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
 # phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -76,6 +76,9 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_nhood_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "sqb_nhood_bytes_per_perm": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "sqb_autocorr_create": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, c_void_pp]),
+    "sqb_autocorr_create_device": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                              C.c_int, C.c_size_t, C.c_void_p, c_void_pp]),
+    "sqb_autocorr_w_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "sqb_autocorr_destroy": (C.c_int, [C.c_void_p]),
     "sqb_autocorr_load_dense": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64]),
     "sqb_autocorr_load_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64]),

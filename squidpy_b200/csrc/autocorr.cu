@@ -44,6 +44,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <climits>
 #include <thread>
 
 #include "common.cuh"
@@ -221,7 +222,7 @@ __global__ void __launch_bounds__(256) ac_final_kernel(const double* __restrict_
 #define AC_T 256          // threads per CTA of the per-feature kernels
 #define AC_NW (AC_T / 32)
 
-enum { AC_ERR_INDEX = 1, AC_ERR_DUP = 2, AC_ERR_PERM = 8 };
+enum { AC_ERR_INDEX = 1, AC_ERR_DUP = 2, AC_ERR_PERM = 8, AC_W_NONCANON = 16, AC_W_NONFINITE = 32 };
 
 // ---- input validation / transposition (load time) ----------------------------------------------------
 // Output feature of input column c, or -1 to skip it (range errors raise *err unless err is null).  colmap == null: the shard [col_lo, col_lo + n_feat) of the columns,
@@ -869,6 +870,7 @@ struct sqb_autocorr {
     sqb_ctx* ctx;
     int64_t n = 0, nnz = 0;
     double s0 = 0.0;
+    int s0_branch = 0;  // how S0 was summed: 0 the exact integer sum of w / g (parallel), 1 one ordered thread
     int w_fmt = 2;  // 0 packed 8 lanes, 1 packed 16 lanes, 2 CSR, 3 compact (7 columns + one common weight in 32 bytes)
     DevBuf<int32_t> d_wp{ctx->stream}, d_wi{ctx->stream};
     DevBuf<double> d_wd{ctx->stream}, d_csum{ctx->stream};
@@ -1282,6 +1284,523 @@ static int ac_gather_dense(sqb_autocorr* h, const void* x, int64_t n_out, int64_
     return SQB_OK;
 }
 
+// =====================================================================================================
+// W build: one device pass serves the host upload (sqb_autocorr_create) and a caller's device CSR (sqb_autocorr_create_device).
+// Every quantity equals, bit for bit, what the host computes for the same W (tests/autocorr_w_ref.py is the specification):
+//   wd = (double)w;  S0 = the sequential float64 sum of wd in entry order;  csum[j] = the sequential float64 sum of column j in
+//   row order (a stable radix sort of the entries by column);  the packed-row format of the per-feature kernel.
+// S0 is one dependent chain.  Every weight is a multiple of g = the smallest lowest set bit among the weights; when
+// sum |w| < 2^53 g every partial sum is a representable multiple of g, so the chain is exact and equals the integer sum of w / g,
+// which is summed in parallel (a row-normalised float32 graph always qualifies).  Otherwise one thread walks the chain.
+// Device input also gets sklearn's l1 row normalisation and the moments s0, s1, s2 of _g_moments in W's dtype, in scipy's
+// operation order: numpy's pairwise summation (np.sum), np.add.reduceat per row (the first value plus the pairwise sum of the
+// rest), a sequential sum per column, and the zero-free values of W^T + W (a symmetric matrix: its canonical CSC order is the
+// row-major order of a row merge of W with its transpose).
+// =====================================================================================================
+#define AC_PW_BLOCK 128  // numpy's PW_BLOCKSIZE
+
+static inline unsigned ac_grid(const sqb_ctx* c, int64_t items, int threads = 256) { return sqb_grid_rows(c, items, threads); }
+
+// caller's column indices -> int32; an index outside [0, n) raises AC_ERR_INDEX, a row whose indices do not strictly increase
+// AC_W_NONCANON.  wp has been validated.
+template <typename II>
+__global__ void ac_w_indices_kernel(const int32_t* __restrict__ wp, const II* __restrict__ in, int64_t n, int32_t* __restrict__ out,
+                                    int* __restrict__ err) {
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+        int64_t prev = -1;
+        int f = 0;
+        for (int32_t e = wp[r]; e < wp[r + 1]; ++e) {
+            const int64_t j = (int64_t)in[e];
+            if (j < 0 || j >= n) {
+                f |= AC_ERR_INDEX;
+                out[e] = 0;
+                continue;
+            }
+            if (j <= prev) f |= AC_W_NONCANON;
+            prev = j;
+            out[e] = (int32_t)j;
+        }
+        if (f) atomicOr(err, f);
+    }
+}
+
+// sklearn's normalize(norm="l1", axis=1) of a float32 / float64 CSR (normalise = 0: a plain copy): per row a sequential float64
+// sum of |w| in entry order; a row whose sum is 0 is kept; every value becomes (T)((double)w / sum).  normalize rejects NaN and
+// infinite values: with normalise, one raises AC_W_NONFINITE.
+template <typename T>
+__global__ void ac_w_l1_kernel(const int32_t* __restrict__ wp, const T* __restrict__ in, int64_t n, int normalise, T* __restrict__ out,
+                               int* __restrict__ err) {
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t b = wp[r], e1 = wp[r + 1];
+        double s = 0.0;
+        bool finite = true;
+        if (normalise)
+            for (int32_t e = b; e < e1; ++e) {
+                finite &= isfinite((double)in[e]);
+                s = __dadd_rn(s, fabs((double)in[e]));
+            }
+        if (!finite) atomicOr(err, AC_W_NONFINITE);
+        for (int32_t e = b; e < e1; ++e) out[e] = normalise && s != 0.0 ? (T)__ddiv_rn((double)in[e], s) : in[e];
+    }
+}
+
+// exponent of the lowest set bit of a finite non-zero double
+__device__ __forceinline__ int ac_lowbit_exp(double d) {
+    int e;
+    const double m = frexp(d, &e);  // d = m 2^e, 0.5 <= |m| < 1
+    const unsigned long long sig = (unsigned long long)fabs(ldexp(m, 53));
+    return e - 53 + __ffsll((long long)sig) - 1;
+}
+
+// wd = (double)w and the statistics of W: st[0] longest row, st[1] some float32 row holds two different weights, st[2] the
+// smallest lowest-bit exponent, st[3] a non-finite weight; part[block] = sum |w| rounded upward (an upper bound)
+template <typename T>
+__global__ void __launch_bounds__(256) ac_w_stats_kernel(const int32_t* __restrict__ wp, const T* __restrict__ w, int64_t n,
+                                                         double* __restrict__ wd, int* __restrict__ st, double* __restrict__ part) {
+    __shared__ double s_sum[256];
+    double acc = 0.0;
+    int maxdeg = 0, nonuni = 0, lb = INT_MAX, nonfin = 0;
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t b = wp[r], e1 = wp[r + 1];
+        maxdeg = max(maxdeg, (int)(e1 - b));
+        for (int32_t e = b; e < e1; ++e) {
+            const T v = w[e];
+            const double d = (double)v;
+            wd[e] = d;
+            if (sizeof(T) == 4 && e > b && __float_as_uint((float)v) != __float_as_uint((float)w[b])) nonuni = 1;
+            if (!isfinite(d)) {
+                nonfin = 1;
+            } else if (d != 0.0) {
+                lb = min(lb, ac_lowbit_exp(d));
+                acc = __dadd_ru(acc, fabs(d));
+            }
+        }
+    }
+    if (maxdeg) atomicMax(&st[0], maxdeg);
+    if (nonuni) atomicOr(&st[1], 1);
+    if (lb != INT_MAX) atomicMin(&st[2], lb);
+    if (nonfin) atomicOr(&st[3], 1);
+    s_sum[threadIdx.x] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int k = 0; k < blockDim.x; ++k) t = __dadd_ru(t, s_sum[k]);
+        part[blockIdx.x] = t;
+    }
+}
+
+__global__ void ac_w_bound_kernel(const double* __restrict__ part, int np, double* __restrict__ out) {
+    double t = 0.0;
+    for (int k = 0; k < np; ++k) t = __dadd_ru(t, part[k]);
+    *out = t;
+}
+
+// S0 as the integer sum of w / 2^g (every term an integer below 2^53 in magnitude, and so is every partial sum)
+__global__ void __launch_bounds__(256) ac_w_s0_int_kernel(const double* __restrict__ wd, int64_t nnz, int g, unsigned long long* __restrict__ acc) {
+    long long loc = 0;
+    for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x)
+        loc += (long long)ldexp(wd[e], -g);
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) loc += __shfl_xor_sync(0xffffffffu, loc, d);
+    if ((threadIdx.x & 31) == 0 && loc != 0) atomicAdd(acc, (unsigned long long)loc);
+}
+
+// S0 as the host computes it: one ordered chain.  One lane adds, from shared memory, while warps 1.. stage the next tile from
+// global memory: the loop runs at the latency of the dependent additions, not of global loads.
+#define AC_SEQ_TILE 2048
+__global__ void __launch_bounds__(256) ac_w_s0_seq_kernel(const double* __restrict__ wd, int64_t nnz, double* __restrict__ out) {
+    __shared__ double buf[2][AC_SEQ_TILE];
+    const int64_t ntiles = (nnz + AC_SEQ_TILE - 1) / AC_SEQ_TILE;
+    for (int64_t i = threadIdx.x; i < AC_SEQ_TILE && i < nnz; i += blockDim.x) buf[0][i] = wd[i];
+    __syncthreads();
+    double s = 0.0;
+    for (int64_t t = 0; t < ntiles; ++t) {
+        const int64_t base = t * AC_SEQ_TILE;
+        if (threadIdx.x == 0) {
+            const double* __restrict__ b = buf[t & 1];
+            const int len = (int)(nnz - base < AC_SEQ_TILE ? nnz - base : AC_SEQ_TILE);
+            int k = 0;
+            for (; k + 8 <= len; k += 8) {
+                double v[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[j] = b[k + j];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) s = __dadd_rn(s, v[j]);
+            }
+            for (; k < len; ++k) s = __dadd_rn(s, b[k]);
+        } else if (threadIdx.x >= 32 && t + 1 < ntiles) {
+            const int64_t nb = base + AC_SEQ_TILE;
+            const int64_t len = nnz - nb < AC_SEQ_TILE ? nnz - nb : AC_SEQ_TILE;
+            for (int64_t i = threadIdx.x - 32; i < len; i += blockDim.x - 32) buf[(t + 1) & 1][i] = wd[nb + i];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *out = s;
+}
+
+__global__ void ac_iota_kernel(int32_t* __restrict__ out, int64_t m) {
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) out[k] = (int32_t)k;
+}
+
+// column ranges [cbeg[j], cend[j]) of the entries sorted by column (both zeroed first: an empty column stays empty)
+__global__ void ac_col_bounds_kernel(const int32_t* __restrict__ key, int64_t m, int32_t* __restrict__ cbeg, int32_t* __restrict__ cend) {
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t j = key[p];
+        if (p == 0 || key[p - 1] != j) cbeg[j] = (int32_t)p;
+        if (p == m - 1 || key[p + 1] != j) cend[j] = (int32_t)(p + 1);
+    }
+}
+
+// csum[j] = sequential float64 sum of column j in row order; colT (or null) the same sum in W's dtype (W.sum(0))
+template <typename T>
+__global__ void ac_col_sums_kernel(const int32_t* __restrict__ cbeg, const int32_t* __restrict__ cend, const int32_t* __restrict__ perm,
+                                   const double* __restrict__ wd, const T* __restrict__ w, int64_t n, double* __restrict__ csum,
+                                   T* __restrict__ colT) {
+    for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        double s = 0.0;
+        T t = (T)0;
+        for (int32_t p = cbeg[j]; p < cend[j]; ++p) {
+            const int32_t e = perm[p];
+            s = __dadd_rn(s, wd[e]);
+            t = t + w[e];
+        }
+        csum[j] = s;
+        if (colT) colT[j] = t;
+    }
+}
+
+// ---- numpy's pairwise summation ---------------------------------------------------------------------------
+// A block of at most 128 values: a plain loop below 8, else eight strided accumulators combined as
+// ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) and the tail added in order.  (numpy starts the short loop from -0.0 and np.sum adds the
+// result to +0.0: the sign of a zero never reaches a non-zero sum, and the caller adds +0.0 last.)
+template <typename T>
+__device__ T ac_pw_leaf(const T* __restrict__ a, int64_t n) {
+    if (n < 8) {
+        T r = (T)0;
+        for (int64_t i = 0; i < n; ++i) r = r + a[i];
+        return r;
+    }
+    T r[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = a[j];
+    int64_t i = 8;
+    for (; i < n - (n % 8); i += 8)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] = r[j] + a[i + j];
+    T res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+    for (; i < n; ++i) res = res + a[i];
+    return res;
+}
+
+// a whole pairwise tree on one thread (rows of W)
+template <typename T>
+__device__ T ac_pw_seq(const T* __restrict__ a, int64_t n) {
+    if (n <= AC_PW_BLOCK) return ac_pw_leaf(a, n);
+    int64_t h = n / 2;
+    h -= h % 8;
+    return ac_pw_seq(a, h) + ac_pw_seq(a + h, n - h);
+}
+
+// node p of level L of the tree over n values (left = 0 bit, most significant first): false when the path ends in a leaf above L
+// and p is not the first index under it
+__device__ __forceinline__ bool ac_pw_node(int64_t n, int L, int64_t p, int64_t* off, int64_t* len) {
+    int64_t o = 0;
+    for (int l = 0; l < L; ++l) {
+        if (n <= AC_PW_BLOCK) {
+            *off = o, *len = n;
+            return (p & ((1LL << (L - l)) - 1)) == 0;
+        }
+        int64_t h = n / 2;
+        h -= h % 8;
+        if ((p >> (L - 1 - l)) & 1) {
+            o += h;
+            n -= h;
+        } else {
+            n = h;
+        }
+    }
+    *off = o, *len = n;
+    return true;
+}
+
+template <typename T>
+__global__ void ac_pw_leaves_kernel(const T* __restrict__ a, int64_t n, int depth, T* __restrict__ res) {
+    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < (1LL << depth); t += (int64_t)gridDim.x * blockDim.x) {
+        int64_t off, len;
+        if (ac_pw_node(n, depth, t, &off, &len)) res[t] = ac_pw_leaf(a + off, len);
+    }
+}
+
+// level L: every inner node = its left subtree's sum + its right subtree's (kept at the first index under each node)
+template <typename T>
+__global__ void ac_pw_level_kernel(int64_t n, int depth, int L, T* __restrict__ res) {
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < (1LL << L); p += (int64_t)gridDim.x * blockDim.x) {
+        int64_t off, len;
+        if (ac_pw_node(n, L, p, &off, &len) && len > AC_PW_BLOCK)
+            res[p << (depth - L)] = res[(2 * p) << (depth - L - 1)] + res[(2 * p + 1) << (depth - L - 1)];
+    }
+}
+
+static int ac_pw_depth(int64_t n) {  // the right half is never the shorter one: its path is the deepest
+    int d = 0;
+    while (n > AC_PW_BLOCK) {
+        int64_t h = n / 2;
+        h -= h % 8;
+        n -= h;
+        ++d;
+    }
+    return d;
+}
+
+// *out (device) = pairwise sum of a[0, n) in T, leaves in parallel, then one launch per level of the tree
+template <typename T>
+static int ac_pairwise(sqb_ctx* c, const T* a, int64_t n, T* out) {
+    if (n == 0) {
+        SQB_CUDA(cudaMemsetAsync(out, 0, sizeof(T), c->stream));
+        return SQB_OK;
+    }
+    const int depth = ac_pw_depth(n);
+    DevBuf<T> res(c->stream);
+    SQB_TRY(res.alloc((size_t)1 << depth));
+    {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_pw_leaves_kernel<T><<<ac_grid(c, (int64_t)1 << depth), 256, 0, c->stream>>>(a, n, depth, res.p);
+        SQB_POST_LAUNCH();
+    }
+    for (int L = depth - 1; L >= 0; --L) {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_pw_level_kernel<T><<<ac_grid(c, (int64_t)1 << L), 256, 0, c->stream>>>(n, depth, L, res.p);
+        SQB_POST_LAUNCH();
+    }
+    SQB_CUDA(cudaMemcpyAsync(out, res.p, sizeof(T), cudaMemcpyDeviceToDevice, c->stream));
+    return SQB_OK;
+}
+
+// (W.sum(1) + W.sum(0).T)^2 per row: the row sum is np.add.reduceat's (first value + the pairwise sum of the rest; 0 if empty)
+template <typename T>
+__global__ void ac_w_rowcol_sq_kernel(const int32_t* __restrict__ wp, const T* __restrict__ w, const T* __restrict__ colT, int64_t n,
+                                      int32_t* __restrict__ rowof, T* __restrict__ out) {
+    for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t b = wp[r], e1 = wp[r + 1];
+        T rs = (T)0;
+        if (e1 > b) rs = e1 - b > 1 ? w[b] + ac_pw_seq(w + b + 1, (int64_t)(e1 - b - 1)) : w[b];
+        const T v = rs + colT[r];
+        out[r] = v * v;
+        for (int32_t e = b; e < e1; ++e) rowof[e] = (int32_t)r;
+    }
+}
+
+// row i of W^T + W: merge of row i of W (ascending columns) with column i of W (ascending rows, the sorted entries); the squares
+// of the non-zero sums that are themselves non-zero (scipy drops zeros from both the sum and the product).  cnt: count pass
+// (out null) or write pass at out + off[i].
+template <typename T>
+__global__ void ac_w_sym_kernel(const int32_t* __restrict__ wp, const int32_t* __restrict__ wi, const T* __restrict__ w,
+                                const int32_t* __restrict__ cbeg, const int32_t* __restrict__ cend, const int32_t* __restrict__ perm,
+                                const int32_t* __restrict__ rowof, int64_t n, unsigned long long* __restrict__ cnt,
+                                const unsigned long long* __restrict__ off, T* __restrict__ out) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        int32_t a = wp[i];
+        const int32_t ae = wp[i + 1];
+        int32_t b = cbeg[i];
+        const int32_t be = cend[i];
+        unsigned long long k = 0, o = out ? off[i] : 0;
+        while (a < ae || b < be) {
+            const int32_t ja = a < ae ? wi[a] : INT_MAX;
+            const int32_t jb = b < be ? rowof[perm[b]] : INT_MAX;
+            T t;
+            if (ja == jb) {
+                t = w[a++] + w[perm[b++]];
+            } else if (ja < jb) {
+                t = w[a++];
+            } else {
+                t = w[perm[b++]];
+            }
+            if (t == (T)0) continue;
+            const T sq = t * t;
+            if (sq == (T)0) continue;
+            if (out) out[o + k] = sq;
+            ++k;
+        }
+        if (!out) cnt[i] = k;
+    }
+}
+
+// The rest of a handle's W once h->d_wp / h->d_wi hold a validated CSR (n, nnz set) and w its values (float or double, already
+// normalised): d_wd, S0, d_csum, the packed rows; with moments (3 doubles, host) s0, s1, s2 of _g_moments in T.  Synchronises.
+template <typename T>
+static int ac_build_w(sqb_autocorr* h, const T* w, double* moments) {
+    sqb_ctx* c = h->ctx;
+    const int64_t n = h->n, nnz = h->nnz;
+    const unsigned gs = (unsigned)c->sm_count * 4;
+    SQB_TRY(h->d_wd.alloc(nnz > 0 ? nnz : 1));
+    SQB_TRY(h->d_csum.alloc(n));
+    DevBuf<int> st(c->stream);
+    DevBuf<double> part(c->stream), bound(c->stream);
+    SQB_TRY(st.alloc(4));
+    SQB_TRY(part.alloc(gs));
+    SQB_TRY(bound.alloc(1));
+    const int st0[4] = {0, 0, INT_MAX, 0};
+    SQB_CUDA(cudaMemcpyAsync(st.p, st0, sizeof(st0), cudaMemcpyHostToDevice, c->stream));
+    {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_w_stats_kernel<T><<<gs, 256, 0, c->stream>>>(h->d_wp.p, w, n, h->d_wd.p, st.p, part.p);
+        SQB_POST_LAUNCH();
+    }
+    {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_w_bound_kernel<<<1, 1, 0, c->stream>>>(part.p, (int)gs, bound.p);
+        SQB_POST_LAUNCH();
+    }
+    int sth[4];
+    double bnd = 0.0;
+    SQB_CUDA(cudaMemcpyAsync(sth, st.p, sizeof(sth), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaMemcpyAsync(&bnd, bound.p, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    const int maxdeg = sth[0], g = sth[2];
+    const bool exact = !sth[3] && (g == INT_MAX || bnd < ldexp(1.0, 53 + g));
+    h->s0_branch = exact ? 0 : 1;
+    DevBuf<unsigned long long> acc(c->stream);
+    DevBuf<double> d_s0(c->stream);
+    if (exact) {
+        SQB_TRY(acc.alloc(1));
+        SQB_CUDA(cudaMemsetAsync(acc.p, 0, sizeof(unsigned long long), c->stream));
+        if (g != INT_MAX) {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_w_s0_int_kernel<<<ac_grid(c, nnz), 256, 0, c->stream>>>(h->d_wd.p, nnz, g, acc.p);
+            SQB_POST_LAUNCH();
+        }
+    } else {
+        SQB_TRY(d_s0.alloc(1));
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_w_s0_seq_kernel<<<1, 256, 0, c->stream>>>(h->d_wd.p, nnz, d_s0.p);
+        SQB_POST_LAUNCH();
+    }
+    // stable transpose: the entries sorted by column keep their row order
+    DevBuf<int32_t> keys(c->stream), iota(c->stream), perm(c->stream), cbeg(c->stream), cend(c->stream), rowof(c->stream);
+    DevBuf<T> colT(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(cbeg.alloc(n));
+    SQB_TRY(cend.alloc(n));
+    SQB_TRY(perm.alloc(nnz > 0 ? nnz : 1));
+    if (moments) SQB_TRY(colT.alloc(n));
+    SQB_CUDA(cudaMemsetAsync(cbeg.p, 0, n * sizeof(int32_t), c->stream));
+    SQB_CUDA(cudaMemsetAsync(cend.p, 0, n * sizeof(int32_t), c->stream));
+    if (nnz > 0) {
+        SQB_TRY(keys.alloc(nnz));
+        SQB_TRY(iota.alloc(nnz));
+        {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_iota_kernel<<<ac_grid(c, nnz), 256, 0, c->stream>>>(iota.p, nnz);
+            SQB_POST_LAUNCH();
+        }
+        int bits = 1;
+        while (bits < 31 && ((uint64_t)(n - 1) >> bits) != 0) ++bits;
+        size_t bytes = 0;
+        SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, h->d_wi.p, keys.p, iota.p, perm.p, (int)nnz, 0, bits, c->stream));
+        SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
+        SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, h->d_wi.p, keys.p, iota.p, perm.p, (int)nnz, 0, bits, c->stream));
+        c->launches += 1;
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_col_bounds_kernel<<<ac_grid(c, nnz), 256, 0, c->stream>>>(keys.p, nnz, cbeg.p, cend.p);
+        SQB_POST_LAUNCH();
+    }
+    {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_col_sums_kernel<T><<<ac_grid(c, n), 256, 0, c->stream>>>(cbeg.p, cend.p, perm.p, h->d_wd.p, w, n, h->d_csum.p,
+                                                                     moments ? colT.p : nullptr);
+        SQB_POST_LAUNCH();
+    }
+    // rows of at most 7 entries that all carry the same float32 weight (a row-normalised binary graph) take the compact format;
+    // packed rows hold float32 weights: only for float32 W (lossless); float64 W walks the CSR
+    const bool f32 = sizeof(T) == 4;
+    const bool uniform7 = f32 && maxdeg <= 7 && nnz > 0 && !sth[1];
+    h->w_fmt = uniform7 ? 3 : (f32 && maxdeg <= 8) ? 0 : (f32 && maxdeg <= 16) ? 1 : 2;
+    if (h->w_fmt != 2) {
+        const int lpr = h->w_fmt == 3 ? 4 : h->w_fmt == 0 ? 8 : 16;  // uint2 units per row
+        SQB_TRY(h->d_rows.alloc((size_t)n * lpr));
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        if (h->w_fmt == 3)
+            ac_pack_rows32_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, reinterpret_cast<uint32_t*>(h->d_rows.p));
+        else if (h->w_fmt == 0)
+            ac_pack_rows_kernel<8><<<c->sm_count * 4, 256, 0, c->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, h->d_rows.p);
+        else
+            ac_pack_rows_kernel<16><<<c->sm_count * 4, 256, 0, c->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, h->d_rows.p);
+        SQB_POST_LAUNCH();
+    }
+    DevBuf<T> mom(c->stream), sq_rc(c->stream), sq_sym(c->stream);
+    DevBuf<unsigned long long> scnt(c->stream), soff(c->stream);
+    if (moments) {
+        SQB_TRY(mom.alloc(3));
+        SQB_TRY(sq_rc.alloc(n));
+        SQB_TRY(rowof.alloc(nnz > 0 ? nnz : 1));
+        SQB_TRY(scnt.alloc(n + 1));
+        SQB_TRY(soff.alloc(n + 1));
+        SQB_TRY(ac_pairwise<T>(c, w, nnz, mom.p));  // s0 = W.sum() = np.sum(W.data)
+        {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_w_rowcol_sq_kernel<T><<<ac_grid(c, n), 256, 0, c->stream>>>(h->d_wp.p, w, colT.p, n, rowof.p, sq_rc.p);
+            SQB_POST_LAUNCH();
+        }
+        SQB_TRY(ac_pairwise<T>(c, sq_rc.p, n, mom.p + 2));  // s2
+        SQB_CUDA(cudaMemsetAsync(scnt.p + n, 0, sizeof(unsigned long long), c->stream));
+        {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_w_sym_kernel<T><<<ac_grid(c, n), 256, 0, c->stream>>>(h->d_wp.p, h->d_wi.p, w, cbeg.p, cend.p, perm.p, rowof.p, n, scnt.p,
+                                                                     nullptr, nullptr);
+            SQB_POST_LAUNCH();
+        }
+        size_t bytes = 0;
+        SQB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, scnt.p, soff.p, (int)(n + 1), c->stream));
+        SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
+        SQB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, scnt.p, soff.p, (int)(n + 1), c->stream));
+        c->launches += 1;
+        unsigned long long m = 0;
+        SQB_CUDA(cudaMemcpyAsync(&m, soff.p + n, sizeof(m), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        SQB_TRY(sq_sym.alloc(m > 0 ? m : 1));
+        {
+            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+            ac_w_sym_kernel<T><<<ac_grid(c, n), 256, 0, c->stream>>>(h->d_wp.p, h->d_wi.p, w, cbeg.p, cend.p, perm.p, rowof.p, n, nullptr,
+                                                                     soff.p, sq_sym.p);
+            SQB_POST_LAUNCH();
+        }
+        SQB_TRY(ac_pairwise<T>(c, sq_sym.p, (int64_t)m, mom.p + 1));  // s1 = (W^T + W).multiply(W^T + W).sum() / 2
+    }
+    unsigned long long s0_int = 0;
+    T mh[3] = {(T)0, (T)0, (T)0};
+    if (exact) SQB_CUDA(cudaMemcpyAsync(&s0_int, acc.p, sizeof(s0_int), cudaMemcpyDeviceToHost, c->stream));
+    else SQB_CUDA(cudaMemcpyAsync(&h->s0, d_s0.p, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (moments) SQB_CUDA(cudaMemcpyAsync(mh, mom.p, sizeof(mh), cudaMemcpyDeviceToHost, c->stream));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    if (exact) h->s0 = g == INT_MAX ? 0.0 : ldexp((double)(long long)s0_int, g);
+    if (moments) {  // np.sum adds the pairwise sum to +0.0; s1 is halved in T
+        moments[0] = (double)((T)0 + mh[0]);
+        moments[1] = (double)(((T)0 + mh[1]) / (T)2);
+        moments[2] = (double)((T)0 + mh[2]);
+    }
+    return SQB_OK;
+}
+
+// W's values from the caller's device array into the handle's build: normalised (or copied) into a buffer of W's own dtype
+template <typename T>
+static int ac_create_from_device(sqb_autocorr* h, const void* data, int transformation, double* moments) {
+    sqb_ctx* c = h->ctx;
+    DevBuf<T> w(c->stream);
+    SQB_TRY(w.alloc(h->nnz > 0 ? h->nnz : 1));
+    {
+        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
+        ac_w_l1_kernel<T><<<ac_grid(c, h->n), 256, 0, c->stream>>>(h->d_wp.p, (const T*)data, h->n, transformation, w.p, h->d_flags.p);
+        SQB_POST_LAUNCH();
+    }
+    if (transformation) {  // sklearn's normalize raises on NaN / infinite weights: the host path reports it
+        int f = 0;
+        SQB_CUDA(cudaMemcpyAsync(&f, h->d_flags.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        SQB_CUDA(cudaStreamSynchronize(c->stream));
+        SQB_CHECK(!(f & AC_W_NONFINITE), SQB_ERR_LAYOUT, "sqb_autocorr_create_device: W holds NaN or infinite weights to normalise");
+    }
+    return ac_build_w<T>(h, w.p, moments);
+}
+
 extern "C" {
 
 int sqb_autocorr_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const int32_t* w_indptr, const int32_t* w_indices,
@@ -1292,66 +1811,82 @@ int sqb_autocorr_create(sqb_ctx* ctx, int64_t n, int64_t nnz, const int32_t* w_i
     SQB_CHECK(w_dtype == 0 || w_dtype == 1, SQB_ERR_INVALID, "sqb_autocorr_create: w_dtype must be 0 (f32) or 1 (f64)");
     SQB_CHECK(w_indptr[0] == 0 && (int64_t)w_indptr[n] == nnz, SQB_ERR_INVALID, "sqb_autocorr_create: inconsistent indptr");
     SQB_CHECK(nnz == 0 || (w_indices && w_data), SQB_ERR_INVALID, "sqb_autocorr_create: null W arrays");
-    // one host pass over W (it is small next to X): validation, float64 weights (scanpy casts W.data to float64), S0 =
-    // sum(W.data), column sums in CSR order (deterministic), longest row
-    int64_t maxdeg = 0;
+    // host validation (messages of the host path); the build itself is the device pass sqb_autocorr_create_device runs
     for (int64_t r = 0; r < n; ++r) {
         const int64_t d = (int64_t)w_indptr[r + 1] - (int64_t)w_indptr[r];
         SQB_CHECK(d >= 0 && w_indptr[r + 1] <= nnz, SQB_ERR_INVALID, "sqb_autocorr_create: indptr decreases at row %lld", (long long)r);
-        if (d > maxdeg) maxdeg = d;
     }
-    std::vector<double> wd((size_t)(nnz > 0 ? nnz : 1)), csum((size_t)n, 0.0);
-    double s0 = 0.0;
     for (int64_t e = 0; e < nnz; ++e) {
         const int32_t j = w_indices[e];
         SQB_CHECK(j >= 0 && j < n, SQB_ERR_INVALID, "sqb_autocorr_create: column index %d out of range at entry %lld", j, (long long)e);
-        wd[e] = w_dtype == 0 ? (double)((const float*)w_data)[e] : ((const double*)w_data)[e];
-        s0 += wd[e];
-        csum[j] += wd[e];
-    }
-    // rows of at most 7 entries that all carry the same float32 weight (a row-normalised binary graph) take the compact format
-    bool uniform7 = (w_dtype == 0 && maxdeg <= 7 && nnz > 0);
-    if (uniform7) {
-        const uint32_t* wb = reinterpret_cast<const uint32_t*>(w_data);
-        for (int64_t r = 0; r < n && uniform7; ++r)
-            for (int64_t e = (int64_t)w_indptr[r] + 1; e < (int64_t)w_indptr[r + 1]; ++e)
-                if (wb[e] != wb[w_indptr[r]]) {
-                    uniform7 = false;
-                    break;
-                }
     }
     SQB_CUDA(cudaSetDevice(ctx->device));
     std::unique_ptr<sqb_autocorr> h(new sqb_autocorr(ctx));
     h->n = n;
     h->nnz = nnz;
-    h->s0 = s0;
-    // packed rows hold float32 weights: only for float32 W (lossless); float64 W walks the CSR
-    h->w_fmt = uniform7 ? 3 : (w_dtype == 0 && maxdeg <= 8) ? 0 : (w_dtype == 0 && maxdeg <= 16) ? 1 : 2;
-    const int lpr = h->w_fmt == 3 ? 4 : h->w_fmt == 0 ? 8 : 16;  // uint2 units per row
     SQB_TRY(h->d_wp.alloc(n + 1));
     SQB_TRY(h->d_wi.alloc(nnz > 0 ? nnz : 1));
-    SQB_TRY(h->d_wd.alloc(nnz > 0 ? nnz : 1));
-    SQB_TRY(h->d_csum.alloc(n));
     SQB_TRY(h->d_flags.alloc(2));
-    if (h->w_fmt != 2) SQB_TRY(h->d_rows.alloc((size_t)n * lpr));
+    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), ctx->stream));
+    const size_t vbytes = (size_t)nnz * (w_dtype == 0 ? sizeof(float) : sizeof(double));
+    DevBuf<uint8_t> wv(ctx->stream);
+    SQB_TRY(wv.alloc(vbytes > 0 ? vbytes : 1));
     SQB_CUDA(cudaMemcpyAsync(h->d_wp.p, w_indptr, (n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
     if (nnz > 0) SQB_CUDA(cudaMemcpyAsync(h->d_wi.p, w_indices, nnz * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    if (nnz > 0) SQB_CUDA(cudaMemcpyAsync(h->d_wd.p, wd.data(), nnz * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    SQB_CUDA(cudaMemcpyAsync(h->d_csum.p, csum.data(), n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), ctx->stream));
-    if (h->w_fmt != 2) {
-        ctx->launches += 1;
-        if (h->w_fmt == 3)
-            ac_pack_rows32_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n,
-                                                                             reinterpret_cast<uint32_t*>(h->d_rows.p));
-        else if (h->w_fmt == 0)
-            ac_pack_rows_kernel<8><<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, h->d_rows.p);
-        else
-            ac_pack_rows_kernel<16><<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(h->d_wp.p, h->d_wi.p, h->d_wd.p, n, h->d_rows.p);
-        SQB_POST_LAUNCH();
-    }
-    SQB_CUDA(cudaStreamSynchronize(ctx->stream));  // wd / csum are host temporaries
+    if (nnz > 0) SQB_CUDA(cudaMemcpyAsync(wv.p, w_data, vbytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (w_dtype == 0)
+        SQB_TRY(ac_build_w<float>(h.get(), reinterpret_cast<const float*>(wv.p), nullptr));
+    else
+        SQB_TRY(ac_build_w<double>(h.get(), reinterpret_cast<const double*>(wv.p), nullptr));
     *out = h.release();
+    return SQB_OK;
+}
+
+int sqb_autocorr_create_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                               const void* data, int value_code, int transformation, uintptr_t producer_stream, double* out_moments,
+                               sqb_autocorr** out) {
+    static const char* where = "sqb_autocorr_create_device";
+    SQB_CHECK(ctx && out && indptr && out_moments, SQB_ERR_INVALID, "%s: null argument", where);
+    SQB_CHECK(n >= 2 && n < 2147483647LL, SQB_ERR_INVALID, "%s: n=%lld out of range", where, (long long)n);
+    SQB_CHECK(nnz >= 0 && nnz < 2147483647LL, SQB_ERR_INVALID, "%s: nnz=%lld does not fit int32", where, (long long)nnz);
+    SQB_CHECK(value_code == 0 || value_code == 1, SQB_ERR_INVALID, "%s: value_code must be 0 (f32) or 1 (f64)", where);
+    SQB_CHECK(nnz == 0 || (indices && data), SQB_ERR_INVALID, "%s: null W arrays", where);
+    SQB_CUDA(cudaSetDevice(ctx->device));
+    std::unique_ptr<sqb_autocorr> h(new sqb_autocorr(ctx));
+    h->n = n;
+    h->nnz = nnz;
+    SQB_TRY(h->d_wp.alloc(n + 1));
+    SQB_TRY(h->d_wi.alloc(nnz > 0 ? nnz : 1));
+    SQB_TRY(h->d_flags.alloc(2));
+    SQB_CUDA(cudaMemsetAsync(h->d_flags.p, 0, 2 * sizeof(int), ctx->stream));
+    SQB_TRY(sqb_read_caller_buffers(ctx, producer_stream, [&]() -> int {
+        return sqb_dispatch_index(indptr_bits, index_bits, where, [&](auto ipt, auto ixt) -> int {
+            using IP = typename decltype(ipt)::type;
+            using II = typename decltype(ixt)::type;
+            // indptr first (one synchronisation): nothing follows it before it is known to run from 0 to nnz
+            SQB_TRY(sqb_check_indptr(ctx, SQB_K_AUTOCORR_PREP, (const IP*)indptr, n, nnz, reinterpret_cast<uint32_t*>(h->d_wp.p), where));
+            {
+                SqbLaunchScope scope(ctx, SQB_K_AUTOCORR_PREP);
+                ac_w_indices_kernel<II><<<ac_grid(ctx, n), 256, 0, ctx->stream>>>(h->d_wp.p, (const II*)indices, n, h->d_wi.p, h->d_flags.p);
+                SQB_POST_LAUNCH();
+            }
+            int f = 0;
+            SQB_CUDA(cudaMemcpyAsync(&f, h->d_flags.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            SQB_CUDA(cudaStreamSynchronize(ctx->stream));
+            SQB_CHECK(!(f & AC_ERR_INDEX), SQB_ERR_INVALID, "%s: %s", where, ac_err_text(AC_ERR_INDEX));
+            SQB_CHECK(!(f & AC_W_NONCANON), SQB_ERR_LAYOUT, "%s: the column indices of a row are not strictly increasing", where);
+            return value_code == 0 ? ac_create_from_device<float>(h.get(), data, transformation, out_moments)
+                                   : ac_create_from_device<double>(h.get(), data, transformation, out_moments);
+        });
+    }));
+    *out = h.release();
+    return SQB_OK;
+}
+
+int sqb_autocorr_w_info(sqb_autocorr* h, int* w_format, int* s0_branch) {
+    SQB_CHECK(h && w_format && s0_branch, SQB_ERR_INVALID, "sqb_autocorr_w_info: null argument");
+    *w_format = h->w_fmt;
+    *s0_branch = h->s0_branch;
     return SQB_OK;
 }
 

@@ -15,7 +15,7 @@ import ctypes as C
 import time
 import warnings
 from collections.abc import Sequence
-from typing import Any, Literal
+from typing import Any, Literal, NamedTuple
 
 import numpy as np
 import pandas as pd
@@ -23,8 +23,8 @@ from scipy import stats
 from scipy.sparse import issparse, spmatrix
 
 from .._constants import Key, SpatialAutocorr
-from .._device import (DevArray, DevSparse, array_device, common_stream, device_matrix, dtype_code, feature_map, index_bits, on_host,
-                       to_host_matrix)
+from .._device import (DevArray, DevGraph, DevSparse, array_device, common_stream, device_matrix, dtype_code, feature_map, index_bits,
+                       on_host, to_host_matrix, weight_graph_args)
 from .._dist import all_gather_rows, all_reduce_sum, shard_range, shared_seed, world
 from .._lib import Context, check, default_context, load, pointer_device
 from .._rng import spawn_generators
@@ -42,6 +42,20 @@ __all__ = ["spatial_autocorr", "co_occurrence", "AutocorrPlan", "cooc_counts"]
 
 fp = np.float32
 ip = np.int32
+SQB_ERR_LAYOUT = -6  # sqb_autocorr_create_device: a row of the device W is not canonical
+
+
+class WeightMoments(NamedTuple):
+    """s0, s1, s2 of the weight matrix (``_g_moments``) and its number of rows."""
+
+    s0: Any
+    s1: Any
+    s2: Any
+    n: int
+
+
+def _weight_moments(w: Any) -> WeightMoments:
+    return w if isinstance(w, WeightMoments) else WeightMoments(*_g_moments(w), w.shape[0])
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -68,6 +82,49 @@ class AutocorrPlan:
         check(self._lib.sqb_autocorr_create(self.ctx.handle, self.n, wi.size, wp.ctypes.data, wi.ctypes.data, wd.ctypes.data, wdt, C.byref(h)))
         self._h = h
         self.n_features = 0
+
+    @classmethod
+    def from_device(cls, graph: DevGraph, transformation: bool, ctx: Context | None = None) -> "AutocorrPlan | None":
+        """Plan over a weight matrix already in GPU memory (``weight_graph_args`` of a torch ``sparse_csr`` or cupyx-style CSR with
+        float32 / float64 values and canonical rows), read in place and never on the host or modified.  ``transformation``
+        row-normalises W on the device like ``normalize(W, norm="l1", axis=1)``.  ``moments`` holds s0, s1, s2 of
+        ``_g_moments`` of the normalised W, as numpy scalars of W's dtype.  Returns ``None`` when a row's column indices do
+        not strictly increase, or when W holds NaN / infinite weights and ``transformation`` is set (sklearn rejects those):
+        the caller then takes the host copy.  An index out of range or a bad indptr raise."""
+        if graph.transposed:
+            raise ValueError("Expected a CSR weight matrix.")
+        code = {np.dtype(np.float32): 0, np.dtype(np.float64): 1}.get(graph.sparse.data.dtype)
+        if code is None:
+            raise TypeError(f"Device weight matrices of dtype `{graph.sparse.data.dtype}` are read on the host; use float32 or float64.")
+        data = graph.sparse.data
+        if len(data.shape) != 1 or data.shape[0] != graph.nnz or (graph.nnz > 1 and data.strides[0] != 1):
+            raise ValueError(f"The weight matrix's values must be a contiguous 1-D array of `{graph.nnz}` entries.")
+        self = cls.__new__(cls)
+        self._h = None
+        self._lib = load()
+        self.ctx = ctx or default_context()
+        self.n = graph.n
+        self.n_features = 0
+        h = C.c_void_p()
+        mom = np.zeros(3, dtype=np.float64)
+        rc = self._lib.sqb_autocorr_create_device(self.ctx.handle, graph.n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None,
+                                                  graph.index_bits, graph.sparse.data.ptr or None, code, int(bool(transformation)),
+                                                  graph.stream, mom.ctypes.data, C.byref(h))
+        if rc == SQB_ERR_LAYOUT:
+            return None
+        check(rc)
+        self._h = h
+        t = graph.sparse.data.dtype.type
+        self.moments = WeightMoments(t(mom[0]), t(mom[1]), t(mom[2]), graph.n)
+        return self
+
+    @property
+    def w_info(self) -> tuple[int, int]:
+        """``(format, s0_branch)`` of the plan's W: format 0 packed rows of 8 slots, 1 of 16, 2 CSR walk, 3 compact rows;
+        s0_branch 0 = S0 summed exactly in parallel, 1 = on one ordered thread."""
+        f, b = C.c_int(), C.c_int()
+        check(self._lib.sqb_autocorr_w_info(self._h, C.byref(f), C.byref(b)))
+        return f.value, b.value
 
     @staticmethod
     def _dt(a: np.ndarray) -> tuple[np.ndarray, int]:
@@ -228,7 +285,12 @@ def spatial_autocorr(
     ``adata.X`` / ``layers[layer]`` / ``raw.X`` / ``obsm[layer]`` may be resident in device memory (cupy / cupyx.scipy.sparse,
     torch CUDA tensors, anything exposing ``__cuda_array_interface__``): the features are then selected and scored on the
     array's own device (``device`` must match it), and the matrix is never copied to the host.  A device-resident
-    ``obsp[connectivity_key]`` is copied to the host once (it is small; its moments and row normalisation are computed there)."""
+    ``obsp[connectivity_key]`` in CSR layout with float32 / float64 values and canonical rows (strictly increasing column
+    indices: what ``spatial_neighbors_*`` export) is read in place on its own device: its row normalisation, S0, column sums
+    and the moments of the p-values are computed there, equal bit for bit to the host computation, and the caller's graph is
+    neither modified nor copied to the host.  ``device`` must match that device, and a device X must live on it too.  Any
+    other device graph (CSC, integer / bool / float16 values, strided or mis-sized arrays, unsorted or repeated column
+    indices, NaN / infinite weights to normalise, dense) is copied to the host once and handled as a host graph."""
     adata = extract_adata_if_sdata(adata, table_key=table_key)
     assert_connectivity_key(adata, connectivity_key)
 
@@ -302,27 +364,51 @@ def spatial_autocorr(
     else:
         params.update(stat="C", expected=1.0, ascending=True)
 
-    g = adata.obsp[connectivity_key]
-    g = g.copy() if device_matrix(g) is None else to_host_matrix(g)
-    if transformation:  # row-normalise in place, dtype preserved (float32 stays float32), :212-214
-        from sklearn.preprocessing import normalize
+    g_src = adata.obsp[connectivity_key]
+    w_dev = device_matrix(g_src)
+    # a device CSR with float values in contiguous arrays is read where it lives; everything else is copied to the host (sklearn /
+    # scipy there)
+    w_graph = weight_graph_args(w_dev, adata.shape[0])
 
-        normalize(g, norm="l1", axis=1, copy=False)
+    def host_w():
+        g = g_src.copy() if w_dev is None else to_host_matrix(g_src)
+        if transformation:  # row-normalise in place, dtype preserved (float32 stays float32), :212-214
+            from sklearn.preprocessing import normalize
+
+            normalize(g, norm="l1", axis=1, copy=False)
+        return g
+
+    g = None if w_graph is not None else host_w()
 
     start = time.perf_counter()
     n_feat = mat.shape[1] if src is None else len(positions)
     rank, ws = world()
     lo, hi = shard_range(n_feat, rank, ws)
     expand = None  # device input: scores of the shard = loaded scores[expand] (duplicate features are loaded once)
+    if w_graph is not None:  # the plan lives on W's device
+        on_w = array_device(w_dev, pointer_device)
+        if device is not None and int(device) != on_w:
+            raise ValueError(f"`device={device}` does not match the device of the weight matrix, cuda:{on_w}.")
+        device = on_w
     if src is not None:
         on = array_device(device_matrix(src), pointer_device)
+        if w_graph is not None and on != device:
+            raise ValueError(f"The feature matrix lives on cuda:{on}, but the weight matrix on cuda:{device}.")
         if device is not None and int(device) != on:
             raise ValueError(f"`device={device}` does not match the device of the feature matrix, cuda:{on}.")
         device = on
     ctx = default_context(device)
     logg.info("Calculating %s's statistic for `%s` permutations on cuda:%d (rank %d/%d, features %d..%d)", mode, n_perms, ctx.device, rank, ws, lo, hi)
     with ctx.lock:
-        plan = AutocorrPlan(g, ctx)
+        plan = None
+        if w_graph is not None:
+            plan = AutocorrPlan.from_device(w_graph, transformation, ctx)
+            if plan is None:  # a row that is not canonical, or non-finite weights to normalise: the host copy handles it as before
+                g = host_w()
+        if plan is None:
+            plan = AutocorrPlan(g, ctx)
+        weights = plan.moments if g is None else g
+        n_obs = plan.n
         try:
             if hi > lo and src is not None:
                 col_map, _, expand = feature_map(src.shape[1], positions, lo, hi)
@@ -339,11 +425,11 @@ def spatial_autocorr(
                 assert_positive(n_perms, name="n_perms")
                 generators = spawn_generators(shared_seed(seed), int(n_perms))
                 sp_local = np.empty((int(n_perms), hi - lo), dtype=np.float64)
-                batch = max(1, min(32, (256 << 20) // (8 * g.shape[0])))  # <= 256 MB of int64 permutations per device call
+                batch = max(1, min(32, (256 << 20) // (8 * n_obs)))  # <= 256 MB of int64 permutations per device call
                 from concurrent.futures import ThreadPoolExecutor
 
                 def draw(p0):  # idx_shuffle of _score_helper (:258-280) for one batch; numpy releases the GIL while it shuffles
-                    return np.stack([generators[p].permutation(g.shape[0]) for p in range(p0, min(p0 + batch, int(n_perms)))])
+                    return np.stack([generators[p].permutation(n_obs) for p in range(p0, min(p0 + batch, int(n_perms)))])
 
                 starts = list(range(0, int(n_perms), batch))
                 with ThreadPoolExecutor(max_workers=1) as pool:  # the next batch is drawn while the device scores this one
@@ -360,7 +446,7 @@ def spatial_autocorr(
             plan.close()
 
     with np.errstate(divide="ignore", invalid="ignore"):
-        pval_results = _p_value_calc(score, score_perms, g, params)
+        pval_results = _p_value_calc(score, score_perms, weights, params)
 
     df = pd.DataFrame({str(params["stat"]): score, **pval_results}, index=index)
     if corr_method is not None:
@@ -412,7 +498,7 @@ def _multipletests(pvals: np.ndarray, method: str) -> np.ndarray:
 
 def _p_value_calc(score: np.ndarray, sims: np.ndarray | None, weights: Any, params: dict[str, Any]) -> dict[str, Any]:
     """p-values of the autocorrelation scores (``_ppatterns.py:443-498``): analytic (normality) and, with
-    permutations, simulation based."""
+    permutations, simulation based.  ``weights``: the weight matrix, or its ``WeightMoments``."""
     p_norm, var_norm = _analytic_pval(score, weights, params)
     results = {"pval_norm": p_norm, "var_norm": var_norm}
     if sims is None:
@@ -436,9 +522,9 @@ def _p_value_calc(score: np.ndarray, sims: np.ndarray | None, weights: Any, para
 
 
 def _analytic_pval(score: np.ndarray, g: Any, params: dict[str, Any]) -> tuple[np.ndarray, float]:
-    """Normality-assumption variance and p-value (Cliff & Ord 1981; ``_ppatterns.py:501-538``)."""
-    s0, s1, s2 = _g_moments(g)
-    n = g.shape[0]
+    """Normality-assumption variance and p-value (Cliff & Ord 1981; ``_ppatterns.py:501-538``).  ``g``: the weight matrix,
+    or its ``WeightMoments``."""
+    s0, s1, s2, n = _weight_moments(g)
     s02 = s0 * s0
     if params["mode"] == SpatialAutocorr.GEARY.s:
         v_score = ((2 * s1 + s2) * (n - 1) - 4 * s02) / (2 * (n + 1) * s02)

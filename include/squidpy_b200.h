@@ -28,6 +28,7 @@
  *   sqb_ligrec_counts_dense    <- _score_permutations on a gathered device matrix  src/squidpy/gr/_ligrec.py:616-676
  *   sqb_sepal_dense            <- _diffusion on a gathered device matrix  src/squidpy/gr/_sepal.py:186-233
  *   sqb_nn_dist_hist_f64       <- NearestNeighbors(...).fit(ref).kneighbors(qry) + np.histogram  src/squidpy/gr/_ripley.py:140-150,160-169,206-209
+ *   sqb_nn_min_dist_f64        <- KDTree(anchor_coord, metric=...).query(batch_coord)  src/squidpy/tl/_var_by_distance.py:129-134
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
  *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
@@ -42,7 +43,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 9
+#define SQB_ABI_VERSION 10
 
 typedef enum {
     SQB_OK = 0,
@@ -348,6 +349,18 @@ int sqb_pair_counts_f64(sqb_ctx* ctx, const double* pts, const int64_t* group_pt
  * block % shard_count == shard_index (multi-GPU sharding; pass 0,1 for everything); partial results add up across shards. */
 int sqb_nn_dist_hist_f64(sqb_ctx* ctx, const double* pts, int64_t n_pts, const int64_t* tasks, int64_t n_tasks,
                          const double* support, int S, int n_rows, int shard_index, int shard_count, int64_t* out);
+
+/* ---- tl.var_by_distance ----------------------------------------------------------------------------------------------
+ * Distance from every query point to its nearest reference point (src/squidpy/tl/_var_by_distance.py:129-134: KDTree of the
+ * anchor coordinates, queried with every observation).  pts: n_pts x 2 float64 point pool (interleaved x,y), n_pts < 2^31, all
+ * finite.  tasks: n_tasks x 5 int64 {ref_begin, ref_end, qry_begin, qry_end, out_begin}, ranges into the pool:
+ * out[out_begin + (q - qry_begin)] = min over r in [ref_begin, ref_end) of dist(pts[q], pts[r]) for q in [qry_begin, qry_end)
+ * (no point excluded: a query that is also a reference point gets 0).  metric 0 euclidean sqrt(dx*dx + dy*dy) without
+ * contraction, 1 manhattan |dx| + |dy|, 2 chebyshev max(|dx|, |dy|): bit-identical to scikit-learn's KDTree.query.  Reference
+ * ranges must be non-empty; output ranges must lie in [0, n_out) and not overlap.  out: n_out float64; positions no task
+ * writes are NaN.                                                                                                         */
+int sqb_nn_min_dist_f64(sqb_ctx* ctx, const double* pts, int64_t n_pts, const int64_t* tasks, int64_t n_tasks, int metric,
+                        int64_t n_out, double* out);
 
 /* ---- sepal ---------------------------------------------------------------------------------------------------------
  * `_diffusion` for every gene (src/squidpy/gr/_sepal.py:186-289): vals = n_genes x n float64 (one row per gene), sat / unsat =

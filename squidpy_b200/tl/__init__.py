@@ -1,0 +1,5 @@
+"""``squidpy_b200.tl`` — ``squidpy.tl`` tools whose cost is a spatial search, on an H100."""
+
+from ._var_by_distance import nn_min_dist, var_by_distance
+
+__all__ = ["var_by_distance", "nn_min_dist"]

@@ -19,7 +19,7 @@
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out) src/squidpy/gr/_nhood.py:401,412-429
  *   sqb_autocorr_*             <- scanpy.metrics.morans_i / gearys_c call     src/squidpy/gr/_ppatterns.py:216,267-272
  *   sqb_cooc_counts            <- _occur_count(x, y, thresholds, labs, n,k,l) src/squidpy/gr/_ppatterns.py:283-310
- *   sqb_pair_counts_f64        <- KDTree.two_point_correlation(points, r)     src/squidpy/gr/_ripley.py:218-223
+ *   sqb_pair_counts_f64        <- KDTree(points, metric=...).two_point_correlation(points, r)  src/squidpy/gr/_ripley.py:218-223
  *   sqb_ligrec_counts          <- _score_permutations(data, clustering, generators, ...)  src/squidpy/gr/_ligrec.py:616-676
  *   sqb_sepal                  <- _diffusion(conc, use_hex, n_iter, sat, sat_idx, unsat, unsat_idx, dt, thresh)  src/squidpy/gr/_sepal.py:186-233
  *   sqb_dense_gather_device    <- X.toarray() / np.asarray(X) + DataFrame.fillna(0.0) + column selection  src/squidpy/gr/_ligrec.py:203-218,
@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 10
+#define SQB_ABI_VERSION 11
 
 typedef enum {
     SQB_OK = 0,
@@ -332,10 +332,14 @@ int sqb_cooc_counts(sqb_ctx* ctx, const float* x, const float* y, int64_t n, con
 
 /* ---- ripley L -------------------------------------------------------------------------------------------
  * For every group g (points group_ptr[g]..group_ptr[g+1] of pts, interleaved x,y float64):
- * out[g*S + s] = #{ordered (i,j) in group g, INCLUDING i == j : sqrt(dx*dx + dy*dy) <= support[s]}  (int64),
- * i.e. sklearn KDTree.two_point_correlation(points_g, support).  support ascending.                        */
+ * out[g*S + s] = #{ordered (i,j) in group g, INCLUDING i == j : dist(i, j) <= support[s]}  (int64),
+ * i.e. sklearn KDTree(points_g, metric=...).two_point_correlation(points_g, support).  support ascending, no NaN;
+ * a negative radius counts nothing.  metric (the codes of sqb_nn_min_dist_f64) 0 euclidean sqrt(dx*dx + dy*dy) without
+ * contraction, 1 manhattan |dx| + |dy|, 2 chebyshev max(|dx|, |dy|), in float64; any other code is SQB_ERR_INVALID.
+ * Tiles t with t % shard_count == shard_index are evaluated, and shard 0 adds the self pairs (multi-GPU sharding;
+ * pass 0,1 for everything); partial results add up across shards.                                           */
 int sqb_pair_counts_f64(sqb_ctx* ctx, const double* pts, const int64_t* group_ptr, int n_groups,
-                        const double* support, int S, int shard_index, int shard_count, int64_t* out);
+                        const double* support, int S, int metric, int shard_index, int shard_count, int64_t* out);
 
 /* ---- ripley F / G ----------------------------------------------------------------------------------------
  * Histograms of nearest-neighbour distances (src/squidpy/gr/_ripley.py:140-150,160-169: kneighbors of a query set against a

@@ -4,7 +4,7 @@
 // Replaces  _occur_count                      src/squidpy/gr/_ppatterns.py:283-310   (float32, ordered pairs i != j,
 //                                             cumulative in r, per (label_i, label_j))
 //      and  KDTree.two_point_correlation      src/squidpy/gr/_ripley.py:218-223       (float64, ordered pairs incl. i == j,
-//                                             cumulative in r, per cluster)
+//                                             cumulative in r, per cluster; euclidean, manhattan or chebyshev)
 // Points are grouped by label on the host (stable counting sort), so every tile of the pair matrix belongs to
 // ONE (label_a, label_b) cell and only an L-bin radial histogram is needed per tile.  Each warp keeps a
 // lane-private histogram column in shared memory (bank == lane: no conflicts, no atomics); a pair is binned
@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <cmath>
 #include <limits>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -57,14 +58,31 @@ __device__ __forceinline__ double sqb_d2<double, 1>(double dx, double dy) {
     return __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
 }
 
+// Ripley-L pair distance in the kernel's compare space (float64 only).  METRIC 0: squared euclidean, compared with squared
+// thresholds; 1 manhattan |dx| + |dy| and 2 chebyshev max(|dx|, |dy|), compared with the radii themselves.  These are
+// scikit-learn's EuclideanDistance / ManhattanDistance / ChebyshevDistance in float64 (0 + |dx| + |dy| == |dx| + |dy|, and
+// max(0, |dx|, |dy|) == max(|dx|, |dy|)).  All are exactly symmetric in (i, j): |a - b| == |b - a| in round-to-nearest.
+template <typename FT, int FMA, int METRIC>
+__device__ __forceinline__ FT sqb_pair_dist(FT dx, FT dy) {
+    static_assert(METRIC == 0 || std::is_same<FT, double>::value, "manhattan / chebyshev pair counts are float64 only");
+    if constexpr (METRIC == 0)
+        return sqb_d2<FT, FMA>(dx, dy);
+    else if constexpr (METRIC == 1)
+        return __dadd_rn(fabs(dx), fabs(dy));
+    else
+        return fmax(fabs(dx), fabs(dy));
+}
+
 #define PAIRS_THREADS 256
 #define PAIRS_IPT 4
 #define PAIRS_JCHUNK 1024
 #define PAIRS_NC 1024
 
-// LANEPRIV: hist[warp][bin][lane] (conflict-free, plain read-modify-write); else hist[warp][bin] with atomics
-template <typename FT, int FMA, bool LANEPRIV>
-__global__ void __launch_bounds__(PAIRS_THREADS) pairs_kernel(const typename Vec2<FT>::type* __restrict__ pts,
+// LANEPRIV: hist[warp][bin][lane] (conflict-free, plain read-modify-write); else hist[warp][bin] with atomics.
+// Launch bounds: a minimum of 1 block per SM lets ptxas give the manhattan / chebyshev kernels the 64-72 registers they
+// need without spilling; 0 (no minimum) leaves the euclidean and co-occurrence kernels as ptxas allocates them by default.
+template <typename FT, int FMA, int METRIC, bool LANEPRIV>
+__global__ void __launch_bounds__(PAIRS_THREADS, METRIC == 0 ? 0 : 1) pairs_kernel(const typename Vec2<FT>::type* __restrict__ pts,
                                                               const PairTile* __restrict__ tiles, int64_t ntiles,
                                                               int shard_index, int shard_count, const FT* __restrict__ thr,
                                                               int L, const int* __restrict__ lut, FT lut_scale,
@@ -103,7 +121,9 @@ __global__ void __launch_bounds__(PAIRS_THREADS) pairs_kernel(const typename Vec
                 yi[q] = p.y;
             } else {
                 gi[q] = -1;
-                xi[q] = (FT)NAN;  // NaN never satisfies d2 <= thr
+                // NaN never satisfies d2 <= thr.  Both coordinates must stay NaN: fmax (METRIC 2) returns its non-NaN
+                // operand, so one finite axis would give a padded lane a real distance.
+                xi[q] = (FT)NAN;
                 yi[q] = (FT)NAN;
             }
         }
@@ -117,7 +137,7 @@ __global__ void __launch_bounds__(PAIRS_THREADS) pairs_kernel(const typename Vec
                 const int gj = jb + jj;
 #pragma unroll
                 for (int q = 0; q < PAIRS_IPT; ++q) {
-                    const FT d2 = sqb_d2<FT, FMA>(xi[q] - pj.x, yi[q] - pj.y);
+                    const FT d2 = sqb_pair_dist<FT, FMA, METRIC>(xi[q] - pj.x, yi[q] - pj.y);
                     if (d2 <= thr_max && !(tile.diag && gj == gi[q])) {
                         int cell = (int)(d2 * lut_scale) - 1;
                         cell = max(0, min(cell, PAIRS_NC - 1));
@@ -153,7 +173,7 @@ __global__ void __launch_bounds__(PAIRS_THREADS) pairs_kernel(const typename Vec
 // ------------------------------------------------------------------------------------------------
 template <typename FT>
 static int pairs_run(sqb_ctx* c, const FT* xy /* interleaved, grouped */, int64_t n, const std::vector<int64_t>& gptr,
-                     bool cross_groups, const FT* thr, int L, int use_fma, int shard_index, int shard_count,
+                     bool cross_groups, const FT* thr, int L, int use_fma, int metric, int shard_index, int shard_count,
                      std::vector<unsigned long long>& hout /* nslots*L */, int nslots_k) {
     typedef typename Vec2<FT>::type V2;
     const int k = (int)gptr.size() - 1;
@@ -243,23 +263,38 @@ static int pairs_run(sqb_ctx* c, const FT* xy /* interleaved, grouped */, int64_
     int64_t grid = std::min<int64_t>((int64_t)c->sm_count * ctas_per_sm, std::max<int64_t>(my_tiles, 1));
     {
         SqbLaunchScope scope(c, SQB_K_PAIRS);
-#define PAIRS_LAUNCH(FMAV, LP)                                                                                        \
+#define PAIRS_LAUNCH(FMAV, METRIC, LP)                                                                                \
     do {                                                                                                              \
-        auto kern = pairs_kernel<FT, FMAV, LP>;                                                                       \
+        auto kern = pairs_kernel<FT, FMAV, METRIC, LP>;                                                               \
         SQB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                \
         kern<<<(unsigned)grid, PAIRS_THREADS, smem, c->stream>>>(d_pts.p, d_tiles.p, ntiles, shard_index, shard_count, \
                                                                  d_thr.p, L, d_lut.p, scale, d_out.p);                \
     } while (0)
-        if (use_fma) {
-            if (lanepriv)
-                PAIRS_LAUNCH(1, true);
-            else
-                PAIRS_LAUNCH(1, false);
-        } else {
-            if (lanepriv)
-                PAIRS_LAUNCH(0, true);
-            else
-                PAIRS_LAUNCH(0, false);
+        if constexpr (std::is_same<FT, double>::value) {
+            if (metric == 1) {
+                if (lanepriv)
+                    PAIRS_LAUNCH(0, 1, true);
+                else
+                    PAIRS_LAUNCH(0, 1, false);
+            } else if (metric == 2) {
+                if (lanepriv)
+                    PAIRS_LAUNCH(0, 2, true);
+                else
+                    PAIRS_LAUNCH(0, 2, false);
+            }
+        }
+        if (metric == 0) {
+            if (use_fma) {
+                if (lanepriv)
+                    PAIRS_LAUNCH(1, 0, true);
+                else
+                    PAIRS_LAUNCH(1, 0, false);
+            } else {
+                if (lanepriv)
+                    PAIRS_LAUNCH(0, 0, true);
+                else
+                    PAIRS_LAUNCH(0, 0, false);
+            }
         }
 #undef PAIRS_LAUNCH
         SQB_POST_LAUNCH();
@@ -301,7 +336,7 @@ int sqb_cooc_counts(sqb_ctx* ctx, const float* x, const float* y, int64_t n, con
         }
     }
     std::vector<unsigned long long> h;
-    SQB_TRY(pairs_run<float>(ctx, xy.data(), n, gptr, true, thr, L, use_fma, shard_index, shard_count, h, k));
+    SQB_TRY(pairs_run<float>(ctx, xy.data(), n, gptr, true, thr, L, use_fma, 0, shard_index, shard_count, h, k));
     // first-bin histogram -> cumulative counts, mirrored to both (a,b) and (b,a)
     for (int a = 0; a < k; ++a) {
         for (int b = a; b < k; ++b) {
@@ -317,10 +352,12 @@ int sqb_cooc_counts(sqb_ctx* ctx, const float* x, const float* y, int64_t n, con
 }
 
 int sqb_pair_counts_f64(sqb_ctx* ctx, const double* pts, const int64_t* group_ptr, int n_groups, const double* support, int S,
-                        int shard_index, int shard_count, int64_t* out) {
+                        int metric, int shard_index, int shard_count, int64_t* out) {
     SQB_CHECK(ctx && pts && group_ptr && support && out, SQB_ERR_INVALID, "sqb_pair_counts_f64: null argument");
     SQB_CHECK(n_groups >= 1 && n_groups <= 1000000, SQB_ERR_INVALID, "sqb_pair_counts_f64: n_groups=%d out of range", n_groups);
     SQB_CHECK(S >= 1 && S <= 4096, SQB_ERR_INVALID, "sqb_pair_counts_f64: S=%d out of range [1,4096]", S);
+    SQB_CHECK(metric >= 0 && metric <= 2, SQB_ERR_INVALID, "sqb_pair_counts_f64: metric=%d is not 0 (euclidean), 1 (manhattan) or 2 (chebyshev)",
+              metric);
     SQB_CHECK(shard_count >= 1 && shard_index >= 0 && shard_index < shard_count, SQB_ERR_INVALID, "sqb_pair_counts_f64: bad shard %d/%d",
               shard_index, shard_count);
     SQB_CHECK(group_ptr[0] == 0, SQB_ERR_INVALID, "sqb_pair_counts_f64: group_ptr[0] must be 0");
@@ -329,13 +366,17 @@ int sqb_pair_counts_f64(sqb_ctx* ctx, const double* pts, const int64_t* group_pt
         SQB_CHECK(gptr[g + 1] >= gptr[g], SQB_ERR_INVALID, "sqb_pair_counts_f64: group_ptr must be non-decreasing");
     const int64_t n = gptr[n_groups];
     SQB_CHECK(n < 2147483647LL, SQB_ERR_INVALID, "sqb_pair_counts_f64: too many points");
-    // thresholds in d2 space: T_s = max{ t : sqrt(t) <= r_s }  (sqrt is monotone and correctly rounded), so that
-    // (sqrt(d2) <= r_s)  <=>  (d2 <= T_s) exactly.
+    // euclidean thresholds in d2 space: T_s = max{ t : sqrt(t) <= r_s }  (sqrt is monotone and correctly rounded), so that
+    // (sqrt(d2) <= r_s)  <=>  (d2 <= T_s) exactly.  Manhattan and chebyshev compare the distance itself: T_s = r_s.
     std::vector<double> T(S);
     for (int s = 0; s < S; ++s) {
         const double r = support[s];
         SQB_CHECK(!(r != r), SQB_ERR_INVALID, "sqb_pair_counts_f64: support[%d] is NaN", s);
         SQB_CHECK(s == 0 || r >= support[s - 1], SQB_ERR_INVALID, "sqb_pair_counts_f64: support must be ascending (support[%d])", s);
+        if (metric != 0) {
+            T[s] = r;  // a negative radius counts nothing: every distance is >= 0
+            continue;
+        }
         if (r < 0.0) {
             T[s] = -1.0;  // nothing satisfies sqrt(d2) <= negative
             continue;
@@ -357,7 +398,7 @@ int sqb_pair_counts_f64(sqb_ctx* ctx, const double* pts, const int64_t* group_pt
     }
     SQB_CUDA(cudaSetDevice(ctx->device));
     std::vector<unsigned long long> h;
-    SQB_TRY(pairs_run<double>(ctx, pts, n, gptr, false, T.data(), S, 0, shard_index, shard_count, h, n_groups));
+    SQB_TRY(pairs_run<double>(ctx, pts, n, gptr, false, T.data(), S, 0, metric, shard_index, shard_count, h, n_groups));
     for (int g = 0; g < n_groups; ++g) {
         unsigned long long run = 0;
         const int64_t m = gptr[g + 1] - gptr[g];

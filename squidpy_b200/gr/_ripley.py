@@ -2,8 +2,10 @@
 
 Mode ``L``: the expensive step — cumulative ordered-pair counts per cluster, ``KDTree.two_point_correlation`` in the
 reference (:218-223) — runs on the H100 (``sqb_pair_counts_f64``: float64, bit-identical counts), for the observed
-clusters and for all Poisson-point-process simulations in ONE launch.  Modes ``F``/``G``: the nearest-neighbour searches
-(:140-150, :160-169) and the histogram of their distances (:206-209) run on the H100 too (``sqb_nn_dist_hist_f64``: float64,
+clusters and for all Poisson-point-process simulations in ONE launch.  This holds for all nine metric names ``KDTree``
+takes: each resolves to scikit-learn's euclidean, manhattan or chebyshev distance, and the kernel computes all three in
+float64 exactly as scikit-learn does.  Modes ``F``/``G``: the nearest-neighbour searches (:140-150, :160-169) and the
+histogram of their distances (:206-209) run on the H100 too (``sqb_nn_dist_hist_f64``: float64,
 bit-identical bin counts) for the euclidean metric, again in ONE call for the observed clusters and every simulation.  G is
 the heavy one: its observed statistic queries every point outside a cluster against the cluster, and every simulation
 queries all N points.  A reference set goes to the device only when scikit-learn would search it with its kd_tree (whose
@@ -24,6 +26,7 @@ from .._constants import Key, RipleyStat
 from .._device import on_host
 from .._dist import all_reduce_sum, world, shared_seed
 from .._lib import Context, check, default_context, load
+from .._metrics import metric_code
 from .._rng import spawn_generators
 from .._validators import assert_categorical_obs, assert_spatial_basis, extract_adata_if_sdata
 from ._utils import _save_data, logg
@@ -35,9 +38,12 @@ _EUCLIDEAN = ("euclidean", "l2", "minkowski")
 _NN_MAX_K = 64  # largest k of the kernel
 
 
-def pair_counts(groups: list[np.ndarray], support: np.ndarray, *, ctx: Context | None = None, shard: tuple[int, int] = (0, 1)) -> np.ndarray:
-    """For every point set in ``groups`` (each (m, 2) float64): int64 (len(groups), S) counts of ordered pairs,
-    self pairs included, with ``sqrt(dx^2 + dy^2) <= support[s]`` — i.e. ``KDTree(p).two_point_correlation(p, support)``."""
+def pair_counts(groups: list[np.ndarray], support: np.ndarray, *, metric: int = 0, ctx: Context | None = None,
+                shard: tuple[int, int] = (0, 1)) -> np.ndarray:
+    """For every point set in ``groups`` (each (m, 2) float64): int64 (len(groups), S) counts of ordered pairs, self pairs
+    included, with ``d(p, q) <= support[s]`` — i.e. ``KDTree(p, metric=m).two_point_correlation(p, support)``.  ``metric``
+    (see :func:`squidpy_b200._metrics.metric_code`): 0 euclidean ``sqrt(dx^2 + dy^2)``, 1 manhattan ``|dx| + |dy|``, 2 chebyshev
+    ``max(|dx|, |dy|)``.  ``shard=(r, n)``: this device's share of the pair tiles (the shares add up to the whole)."""
     lib = load()
     ctx = ctx or default_context()
     support = np.ascontiguousarray(support, dtype=np.float64)
@@ -46,7 +52,7 @@ def pair_counts(groups: list[np.ndarray], support: np.ndarray, *, ctx: Context |
     pts = np.ascontiguousarray(np.concatenate([np.asarray(g, dtype=np.float64).reshape(-1, 2) for g in groups], axis=0)) if ptr[-1] else np.zeros((1, 2))
     out = np.empty((len(groups), support.size), dtype=np.int64)
     check(lib.sqb_pair_counts_f64(ctx.handle, pts.ctypes.data, ptr.ctypes.data, len(groups), support.ctypes.data, support.size,
-                                  int(shard[0]), int(shard[1]), out.ctypes.data))
+                                  int(metric), int(shard[0]), int(shard[1]), out.ctypes.data))
     return out
 
 
@@ -121,7 +127,7 @@ def ripley(
     bins = support
 
     if mode == RipleyStat.L:
-        _check_l_metric(metric)
+        code = _check_l_metric(metric)
         # all simulations first (host RNG stream identical to the reference: one generator per simulation), then ONE
         # GPU launch counts pairs for the observed clusters and every simulated pattern
         groups = [coordinates[cluster_idx == i, :].astype(np.float64, copy=False) for i in range(int(np.max(cluster_idx)) + 1)]
@@ -130,7 +136,7 @@ def ripley(
         deln = Delaunay(hull.points[hull.vertices])  # one triangulation of the hull for all simulations
         sims_pts = [_ppp(hull, 1, n_observations, rng=sim_rngs[i], deln=deln).reshape(-1, 2) for i in range(n_simulations)]
         rank, ws = world()
-        counts = pair_counts(groups + sims_pts, support, ctx=default_context(device), shard=(rank, ws))
+        counts = pair_counts(groups + sims_pts, support, metric=code, ctx=default_context(device), shard=(rank, ws))
         counts = all_reduce_sum(counts)
         sizes = np.array([len(g) for g in groups + sims_pts], dtype=np.int64)
         l_all = _l_from_counts(counts, sizes, N, area)
@@ -161,13 +167,13 @@ def ripley(
     return None
 
 
-def _check_l_metric(metric: str) -> None:
+def _check_l_metric(metric: str) -> int:
+    """The kernel code of an L metric; names ``KDTree`` does not take raise the reference's error."""
     from sklearn.neighbors import KDTree
 
     if metric not in KDTree.valid_metrics:  # same check and message as _ripley.py:213-214
         raise ValueError(f"Unsupported metric '{metric}'. Ripley's L supports {KDTree.valid_metrics}")
-    if metric not in ("euclidean", "l2", "minkowski", "p"):
-        raise NotImplementedError(f"Ripley's L on the GPU implements the euclidean metric only, found `{metric}`.")
+    return metric_code(metric)
 
 
 def _l_from_counts(counts: np.ndarray, sizes: np.ndarray, n: int, area: float) -> np.ndarray:

@@ -19,25 +19,10 @@ import pandas as pd
 
 from .._device import on_host
 from .._lib import Context, check, default_context, load
+from .._metrics import metric_code
 from ..gr._utils import _save_data, logg
 
 __all__ = ["var_by_distance", "nn_min_dist", "metric_code"]
-
-_METRIC_CODES = {"EuclideanDistance": 0, "ManhattanDistance": 1, "ChebyshevDistance": 2}
-
-
-def metric_code(metric: str) -> int:
-    """Kernel code of a metric name: 0 euclidean, 1 manhattan, 2 chebyshev, the classes ``DistanceMetric.get_metric`` resolves
-    every ``KDTree`` metric name to.  Names it rejects raise its error; metrics ``KDTree`` does not take raise KDTree's."""
-    from sklearn.metrics import DistanceMetric
-    from sklearn.neighbors import KDTree
-
-    dm = DistanceMetric.get_metric(metric)
-    name = type(dm).__name__.rstrip("0123456789")
-    if name not in _METRIC_CODES:
-        KDTree(np.zeros((1, 2)), metric=dm)  # ValueError: not valid for KDTree
-        raise NotImplementedError(f"var_by_distance on the GPU has no kernel for the metric `{metric}`.")
-    return _METRIC_CODES[name]
 
 
 def nn_min_dist(points: np.ndarray, tasks: np.ndarray, metric: int, n_out: int, *, ctx: Context | None = None) -> np.ndarray:

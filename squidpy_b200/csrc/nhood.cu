@@ -1342,7 +1342,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) nhood_apply_part_kernel(LT* __r
     constexpr int L = SQB_PART_L;
     constexpr uint32_t full_mask = 0xFFFFFFFFu;  // (SQB_CONVERGE)
     constexpr int HS = 2 * NT;   // slots per window = hash slots per table
-    constexpr int NWB = 2 * HS;  // filter words (16 buckets of 2 bits each)
+    constexpr int NWB = 4 * HS;  // filter words (16 buckets of 2 bits each: 64 buckets per slot, see part_tables_bytes)
     constexpr int LOG_HS = (HS == 1024 ? 10 : HS == 2048 ? 11 : 12);
     static_assert(HS == (1 << LOG_HS), "HS must be a power of two");
     static_assert(HS <= (1 << SQB_PART_IDB), "slot ids must fit a table entry");
@@ -2617,11 +2617,11 @@ static int part_max_blocks(const sqb_nhood* h) {
 }
 
 // shared memory of nhood_apply_part_kernel besides the slab:
-// [tabT, tabO u32 x HS][bits u32 x 2 HS][top int x HS][bpref, bslot int x bwords][wsum int x 32][next u16 x HS]
+// [tabT, tabO u32 x HS][bits u32 x 4 HS][top int x HS][bpref, bslot int x bwords][wsum int x 32][next u16 x HS]
 // [gath u32 x HS][otop LT x HS]
 static size_t part_tables_bytes(int nt, int lt_bytes, int nbmax) {
     const size_t HS = 2 * (size_t)nt;
-    return 2 * HS * 4 + 2 * HS * 4 + HS * 4 + 2 * (size_t)sqb_part_bwords(nbmax) * 4 + 32 * 4 + HS * 2 + HS * 4 + HS * lt_bytes;
+    return 2 * HS * 4 + 4 * HS * 4 + HS * 4 + 2 * (size_t)sqb_part_bwords(nbmax) * 4 + 32 * 4 + HS * 2 + HS * 4 + HS * lt_bytes;
 }
 
 // positions per region of shuffle_algo 9 with nt threads and per_sm resident CTAs per SM (a multiple of 16; 0 = not even 16
@@ -2657,14 +2657,16 @@ static int part_apply_attributes(size_t smem) {
 // runs when asked for (shuffle_algo 9) and in auto mode for many permutations of arrays of >= 512 K elements, provided that
 // every segment fits SQB_PART_RMAX regions; otherwise the list replay (algo 7) runs.  Its 32 warps spend much of a window
 // waiting at the window's three block barriers, so the first choice is two resident 512-thread CTAs per SM, each with half
-// of the SM's shared memory (1M u8 labels: 12 regions of 83 344 positions; 1M u16 labels: 25 regions; u8 arrays up to about
-// 2.5M elements).  When a segment does not fit that or two such CTAs do not fit an SM, one 1024-thread CTA per SM takes a
-// block's opt-in limit (1M u8 labels: 6 regions).  shuffle_threads = 1024 with shuffle_algo 9 asks for the latter.
+// of the SM's shared memory (1M u8 labels: 14 regions of 75 776 positions; 1M u16 labels: 27 regions; u8 arrays up to about
+// 2.25M elements).  When a segment does not fit that or two such CTAs do not fit an SM, one 1024-thread CTA per SM takes a
+// block's opt-in limit (1M u8 labels: 7 regions).  shuffle_threads = 1024 with shuffle_algo 9 asks for the latter.
 // Measured on an H100 80GB HBM3 (700 W power limit), tools/apply_time.py, 1M spots x 1000 permutations, before the window
 // loop stopped waiting on global memory: the apply took 18.4-18.5 ms with two CTAs per SM against 19.8-19.9 ms with one
 // 1024-thread CTA per SM, and 30.9 ms with 13 regions but one 512-thread CTA per SM.  Four 256-thread CTAs per SM (26
 // regions of ~39 K positions, 512-slot windows) do not pay: 15.0 ms against 14.47 ms for two 512-thread CTAs with the same
-// 32-bit tables (same card, DESIGN.md §3.1), because a half-size window no longer hides its J loads.  At 300 K cells x 10 000
+// 32-bit tables (same card, DESIGN.md §3.1), because a half-size window no longer hides its J loads.  Four slots per thread
+// (2048-slot windows, two 512-thread CTAs per SM, 18 regions) do not pay either: 14.79-14.82 ms against 12.53-12.57 ms (H100
+// 80GB HBM3, 700 W power limit), since the barrier waits grow with the window instead of staying fixed.  At 300 K cells x 10 000
 // permutations (tools/apply_time.py cfg5, H100 80GB HBM3, 400 W power limit) algo 9 takes 92.5 ms against 84.2 ms for auto
 // (list replay): its apply now ties (46.2 against 46.0 ms) but its target generation costs 9 ms more, so auto keeps the list
 // replay below 512 K elements (DESIGN.md §3.1).

@@ -32,6 +32,8 @@
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
  *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
+ *   sqb_centrality_scores      <- _build_graph + rx.group_degree_centrality / rx.group_closeness_centrality + _local_clustering
+ *                                 src/squidpy/gr/_nhood.py:305-317,432-491
  */
 #ifndef SQUIDPY_B200_H
 #define SQUIDPY_B200_H
@@ -43,7 +45,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 11
+#define SQB_ABI_VERSION 12
 
 typedef enum {
     SQB_OK = 0,
@@ -196,6 +198,26 @@ int sqb_interaction_matrix(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t*
 int sqb_interaction_matrix_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
                                   int index_bits, const void* data, int data_dtype, const int32_t* codes, int n_cls,
                                   double* out_weighted, int64_t* out_counts, uintptr_t producer_stream);
+
+/* ---- centrality_scores -------------------------------------------------------------------------------------
+ * The integer parts of the three group measures of centrality_scores (src/squidpy/gr/_nhood.py:245-346), over the graph
+ * _build_graph makes (:432-454): A + Aᵀ with values summed in A's dtype, diagonal and zero sums dropped (an explicit zero or a
+ * cancelling +w / -w pair removes the edge, a NaN sum keeps it).  The caller's CSR is taken as given, from the host
+ * (device_input = 0: host pointers, uploaded) or from device memory (device_input = 1: DEVICE pointers on the context's
+ * device, read in place; producer_stream as in sqb_autocorr_load_csr_device).  indptr_bits / index_bits 32 or 64;
+ * data_dtype 0 = f32, 1 = f64, 3 = int32, 4 = int64, 5 = bool (one byte); an integer sum wraps at int_bits (8, 16, 32 or 64:
+ * the width of the caller's dtype, whose values may arrive widened to int32 / int64).  nnz < 2^30; data may be NULL when nnz = 0.
+ * codes[v] in [0, n_cls) is the cluster of observation v, -1 none (it is a node but in no group).  measures: a mask of
+ *   1: out_reach1[k] = |N(S_k) \ S_k|                              (rx.group_degree_centrality numerator, :311-312)
+ *   2: out_dist[k]   = sum over v not in S_k reachable from S_k of the hop distance d(S_k, v)
+ *                      (rx.group_closeness_centrality denominator, :309-310); *out_levels = deepest BFS level reached
+ *   4: out_cc[v]     = 2 T(v) / (k_v (k_v - 1)) in float64, 0 when k_v < 2  (_local_clustering, :457-491)
+ * The divisions by n - |S_k| and the per-group means are the caller's.  Column indices outside [0, n) or an indptr not
+ * running from 0 to nnz return SQB_ERR_INVALID.  Returns after the device has stopped reading the caller's buffers.          */
+int sqb_centrality_scores(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
+                          int index_bits, const void* data, int data_dtype, int int_bits, int device_input, const int32_t* codes,
+                          int n_cls, int measures, int64_t* out_reach1, int64_t* out_dist, double* out_cc, int64_t* out_levels,
+                          uintptr_t producer_stream);
 
 /* ---- ligrec permutation test ------------------------------------------------------------------------------
  * _score_permutations of the reference (src/squidpy/gr/_ligrec.py:616-676) for a handle whose base labels are the cells'

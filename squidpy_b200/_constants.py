@@ -1,7 +1,7 @@
 """Key strings and mode enums of the hot path (contract with AnnData and ``sq.pl``).
 
 Mirrors ``src/squidpy/_constants/_pkg_constants.py:65-121,198-213`` (``Key``) and
-``src/squidpy/_constants/_constants.py:93-110`` (``SpatialAutocorr``, ``RipleyStat``) of the reference, including the
+``src/squidpy/_constants/_constants.py:74-77,93-110`` (``Centrality``, ``SpatialAutocorr``, ``RipleyStat``) of the reference, including the
 error text of an invalid enum value (``_constants/_utils.py:30-40``).
 """
 
@@ -88,6 +88,13 @@ class RipleyStat(ModeEnum):
     L = "L"
 
 
+@unique
+class Centrality(ModeEnum):
+    DEGREE = "degree_centrality"
+    CLUSTERING = "average_clustering"
+    CLOSENESS = "closeness_centrality"
+
+
 class Key:
     class obsm:
         spatial = "spatial"
@@ -129,6 +136,10 @@ class Key:
         @classmethod
         def ripley(cls, cluster: str, mode) -> str:
             return f"{cluster}_ripley_{mode}"
+
+        @classmethod
+        def centrality_scores(cls, cluster: str) -> str:
+            return f"{cluster}_centrality_scores"
 
         @classmethod
         def interaction_matrix(cls, cluster: str) -> str:

@@ -3,7 +3,7 @@
 from ._build import (GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, knn_2d, radius_2d, spatial_neighbors_grid,
                      spatial_neighbors_knn, spatial_neighbors_radius)
 from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
-from ._nhood import NhoodEnrichmentResult, NhoodPlan, interaction_matrix, nhood_enrichment
+from ._nhood import NhoodEnrichmentResult, NhoodPlan, centrality_counts, centrality_scores, interaction_matrix, nhood_enrichment
 from ._ppatterns import AutocorrPlan, co_occurrence, cooc_counts, spatial_autocorr
 from ._ripley import nn_distance_hist, pair_counts, ripley
 from ._sepal import sepal, sepal_scores
@@ -25,6 +25,8 @@ __all__ = [
     "ligrec_analysis_device",
     "nhood_enrichment",
     "interaction_matrix",
+    "centrality_scores",
+    "centrality_counts",
     "spatial_autocorr",
     "co_occurrence",
     "ripley",

@@ -1,5 +1,6 @@
 """``nhood_enrichment`` — drop-in for ``squidpy.gr.nhood_enrichment`` (``src/squidpy/gr/_nhood.py:146-242``) running the
-permutation test on an H100 through ``libsquidpy_b200.so``.
+permutation test on an H100 through ``libsquidpy_b200.so``; ``interaction_matrix`` and ``centrality_scores`` over the same
+neighbour graph.
 
 Same signature, same ``adata.uns`` keys, same exceptions.  ``numba_parallel``, ``n_jobs``, ``backend`` and
 ``show_progress_bar`` are accepted for compatibility and ignored (the joblib fan-out over permutations is replaced by
@@ -17,7 +18,7 @@ from typing import Any, NamedTuple
 
 import numpy as np
 
-from .._constants import Key
+from .._constants import Centrality, Key
 from .._device import DevGraph, DevSparse, array_device, device_graph, graph_args, graph_value_code
 from .._dist import nccl_cuda, sequential_stats, shard_range, shared_seed, stats_device, world
 from .._lib import Context, check, default_context, load, pointer_device
@@ -25,7 +26,7 @@ from .._rng import spawn_states
 from .._validators import assert_categorical_obs, assert_connectivity_key, assert_positive, extract_adata_if_sdata
 from ._utils import _save_data, as_csr, category_codes, logg
 
-__all__ = ["nhood_enrichment", "NhoodEnrichmentResult", "NhoodPlan"]
+__all__ = ["nhood_enrichment", "NhoodEnrichmentResult", "NhoodPlan", "centrality_scores", "centrality_counts"]
 
 
 class NhoodEnrichmentResult(NamedTuple):
@@ -314,6 +315,148 @@ def nhood_enrichment(
         return NhoodEnrichmentResult(zscore=zscore, counts=count)
     _save_data(adata, attr="uns", key=Key.uns.nhood_enrichment(cluster_key), data={"zscore": zscore, "count": count},
                time_start=start)
+    return None
+
+
+class CentralityCounts(NamedTuple):
+    """The integer parts of the group measures (``sqb_centrality_scores``); fields not requested are ``None``."""
+
+    reach1: np.ndarray | None  # int64[C]: |N(S) \ S|
+    dist: np.ndarray | None  # int64[C]: sum of hop distances from S over the nodes it reaches
+    cc: np.ndarray | None  # float64[n]: local clustering coefficient
+    levels: int  # BFS levels that reached a node (-1 without closeness)
+
+
+# value dtype of a host graph -> (dtype it is uploaded as, ABI value code, bits at which its integer sum wraps)
+_HOST_VALUES = {
+    np.dtype(np.bool_): (np.bool_, 5, 64), np.dtype(np.float32): (np.float32, 0, 64), np.dtype(np.float64): (np.float64, 1, 64),
+    np.dtype(np.int8): (np.int32, 3, 8), np.dtype(np.uint8): (np.int32, 3, 8), np.dtype(np.int16): (np.int32, 3, 16),
+    np.dtype(np.uint16): (np.int32, 3, 16), np.dtype(np.int32): (np.int32, 3, 32), np.dtype(np.uint32): (np.int64, 4, 32),
+    np.dtype(np.int64): (np.int64, 4, 64), np.dtype(np.uint64): (np.int64, 4, 64),
+}
+_MEASURE_BITS = {Centrality.DEGREE: 1, Centrality.CLOSENESS: 2, Centrality.CLUSTERING: 4}
+
+
+def centrality_counts(conn: Any, codes: np.ndarray, n_cls: int, measures: int, *, device: int | None = None) -> CentralityCounts:
+    """Run ``sqb_centrality_scores`` on the neighbour graph ``conn``: a scipy / numpy matrix on the host, or a CSR / CSC
+    in GPU memory (as ``nhood_enrichment`` takes it).  ``codes``: int32[n] cluster codes, -1 for none.  ``measures``: a
+    mask of 1 (degree), 2 (closeness), 4 (clustering).  A CSC matrix is read as the CSR of its transpose, which is the
+    same undirected graph."""
+    import scipy.sparse as sp
+
+    codes = np.ascontiguousarray(codes, dtype=np.int32)
+    n = codes.size
+    dev = device_graph(conn)
+    if dev is None:
+        g = conn if sp.issparse(conn) and conn.format in ("csr", "csc") else as_csr(conn)
+        if g.shape != (n, n):
+            raise ValueError(f"Expected the connectivity graph to be of shape `{(n, n)}`, found `{g.shape}`.")
+        spec = _HOST_VALUES.get(g.dtype)
+        if spec is None:
+            raise TypeError(f"Graph values of dtype `{g.dtype}` are not supported.")
+        dtype, code, int_bits = spec
+        indptr, indices = (np.ascontiguousarray(a) if a.dtype in (np.int32, np.int64) else np.ascontiguousarray(a, np.int64)
+                           for a in (g.indptr, g.indices))
+        data = g.data.view(np.int64) if g.dtype == np.uint64 else g.data
+        data = np.ascontiguousarray(data, dtype=dtype)
+        args = (n, indices.size, indptr.ctypes.data, 8 * indptr.itemsize, indices.ctypes.data, 8 * indices.itemsize, data.ctypes.data,
+                code, int_bits, 0)
+        stream = 0
+    else:
+        graph = graph_args(dev, n)
+        device = _graph_device(dev, device)
+        code = graph_value_code(dev.data, graph.nnz)
+        if code == 2:
+            raise TypeError("Device graph values of dtype `float16` are not supported; use float32, float64, int32, int64 or bool.")
+        args = (n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None, graph.index_bits, dev.data.ptr or None, code,
+                32 if code == 3 else 64, 1)
+        stream = graph.stream
+    reach1 = np.zeros(n_cls, dtype=np.int64) if measures & 1 else None
+    dist = np.zeros(n_cls, dtype=np.int64) if measures & 2 else None
+    cc = np.empty(n, dtype=np.float64) if measures & 4 else None
+    levels = C.c_int64(-1)
+    ctx = default_context(device)
+    with ctx.lock:
+        check(load().sqb_centrality_scores(ctx.handle, *args, codes.ctypes.data, int(n_cls), int(measures),
+                                           None if reach1 is None else reach1.ctypes.data, None if dist is None else dist.ctypes.data,
+                                           None if cc is None else cc.ctypes.data, C.byref(levels), stream))
+    return CentralityCounts(reach1, dist, cc, int(levels.value))
+
+
+def centrality_scores(
+    adata: Any,
+    cluster_key: str,
+    score: str | Centrality | None = None,
+    connectivity_key: str | None = None,
+    copy: bool = False,
+    n_jobs: int | None = None,
+    backend: str = "loky",
+    show_progress_bar: bool = False,
+    *,
+    table_key: str | None = None,
+    device: int | None = None,
+):
+    """Centrality scores of every cluster (reference ``gr/_nhood.py:245-346``) over the undirected neighbour graph
+    ``obsp[connectivity_key] + obsp[connectivity_key].T`` without self loops, entries whose sum is zero dropped.  For the
+    group S of each category (``cat.categories`` in order, unused ones included; observations with a NaN label are nodes of
+    the graph but in no group) and n observations:
+
+    - ``degree_centrality``: ``|N(S) \\ S| / (n - |S|)``;
+    - ``average_clustering``: the mean over S of the local clustering coefficient, 0.0 for an empty group;
+    - ``closeness_centrality``: ``(n - |S|) / sum of d(S, v)`` over the nodes v outside S reachable from S in hops, 0.0
+      when that sum is 0.
+
+    Where the measure is undefined the value is NaN: closeness of an empty category and degree of a category holding every
+    observation.  The counts are computed on the GPU (``centrality_counts``), the divisions on the host in float64, so the
+    values are those of networkx's ``group_degree_centrality`` / ``group_closeness_centrality`` / ``average_clustering``.
+
+    ``score``: one name (``str`` or :class:`Centrality`) or ``None`` for all three, in that order: degree, clustering,
+    closeness.  ``n_jobs``, ``backend`` and ``show_progress_bar`` are accepted and ignored.  Under a process group every
+    rank computes the whole result on its own device.  Returns the float64 frame if ``copy=True``, otherwise writes
+    ``adata.uns[f'{cluster_key}_centrality_scores']``."""
+    import pandas as pd
+
+    adata = extract_adata_if_sdata(adata, table_key=table_key)
+    connectivity_key = Key.obsp.spatial_conn(connectivity_key)
+    assert_categorical_obs(adata, cluster_key)
+    assert_connectivity_key(adata, connectivity_key)
+    if isinstance(score, str | Centrality):
+        centrality = [score]
+    elif score is None:
+        centrality = [c.s for c in Centrality]
+    else:  # the reference leaves `centrality` unbound here (:293-298)
+        raise UnboundLocalError("cannot access local variable 'centrality' where it is not associated with a value")
+    centralities = [Centrality(c) for c in centrality]
+
+    start = time.perf_counter()
+    cats = adata.obs[cluster_key]
+    cat = cats.cat.categories.values
+    n_cls = len(cat)
+    codes = np.asarray(cats.array.codes, dtype=np.int32)
+    n = codes.size
+    measures = 0
+    for c in centralities:
+        measures |= _MEASURE_BITS[c]
+    counts = centrality_counts(adata.obsp[connectivity_key], codes, n_cls, measures, device=device)
+    logg.info("Calculating centralities `%s` on the GPU (%d BFS levels)", centralities, counts.levels)
+
+    size = np.bincount(codes[codes >= 0], minlength=n_cls)
+    columns = {}
+    for c in centralities:
+        if c == Centrality.DEGREE:  # networkx: len(N(S) - S) / (len(G) - len(S)), Python int division
+            vals = [int(r) / (n - int(s)) if n != s else np.nan for r, s in zip(counts.reach1, size)]
+        elif c == Centrality.CLOSENESS:
+            vals = [np.nan if s == 0 else ((n - int(s)) / int(d) if d else 0.0) for d, s in zip(counts.dist, size)]
+        else:  # float(cc[idx].mean()) per group (:316): the group's coefficients in index order, numpy's pairwise mean
+            order = np.argsort(codes, kind="stable")[n - int(size.sum()):]
+            groups = np.split(counts.cc[order], np.cumsum(size)[:-1])
+            vals = [float(g.mean()) if g.size else 0.0 for g in groups]
+        columns[c.s] = pd.DataFrame(vals, columns=[c.s], index=cat)
+    df = pd.concat(list(columns.values()), axis=1)
+
+    if copy:
+        return df
+    _save_data(adata, attr="uns", key=Key.uns.centrality_scores(cluster_key), data=df, time_start=start)
     return None
 
 

@@ -29,6 +29,7 @@
  *   sqb_sepal_dense            <- _diffusion on a gathered device matrix  src/squidpy/gr/_sepal.py:186-233
  *   sqb_nn_dist_hist_f64       <- NearestNeighbors(...).fit(ref).kneighbors(qry) + np.histogram  src/squidpy/gr/_ripley.py:140-150,160-169,206-209
  *   sqb_nn_min_dist_f64        <- KDTree(anchor_coord, metric=...).query(batch_coord)  src/squidpy/tl/_var_by_distance.py:129-134
+ *   sqb_window_ranges          <- the per-window coordinate masks of sliding_window  src/squidpy/tl/_sliding_window.py:130-158
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
  *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
@@ -45,7 +46,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 12
+#define SQB_ABI_VERSION 13
 
 typedef enum {
     SQB_OK = 0,
@@ -387,6 +388,20 @@ int sqb_nn_dist_hist_f64(sqb_ctx* ctx, const double* pts, int64_t n_pts, const i
  * writes are NaN.                                                                                                         */
 int sqb_nn_min_dist_f64(sqb_ctx* ctx, const double* pts, int64_t n_pts, const int64_t* tasks, int64_t n_tasks, int metric,
                         int64_t n_out, double* out);
+
+/* ---- tl.sliding_window -------------------------------------------------------------------------------------------------
+ * The windows that contain each observation (src/squidpy/tl/_sliding_window.py:130-158: one mask
+ * x_start <= x <= x_end & y_start <= y <= y_end over the library's observations per window; the windows of a library are the
+ * product of its x and y windows, :224-242).  xy: n x 2 coordinates (interleaved x,y), n < 2^31, in the dtype the comparisons
+ * are made in: xy_dtype 0 float64, 1 int64; starts / ends hold the edges in the same dtype.  lib[i] in [-1, n_libs) is the
+ * library of observation i, -1 none.  edge_off (2 n_libs + 1 entries, edge_off[0] = 0): the x edges of library l are
+ * starts / ends [edge_off[2l], edge_off[2l+1]), its y edges [edge_off[2l+1], edge_off[2l+2]); within one such range both starts
+ * and ends must be non-decreasing and not NaN (SQB_ERR_INVALID otherwise).  out: n x 4 int32 {lo_x, hi_x, lo_y, hi_y}, where
+ * hi = the last window index whose start <= v and lo = the first whose end >= v: observation i lies in window (ix, iy) of its
+ * library iff lo_x <= ix <= hi_x and lo_y <= iy <= hi_y.  An axis with lo > hi, a NaN coordinate or lib[i] = -1 (written as
+ * {0, -1, 0, -1}) puts the observation in no window.                                                                       */
+int sqb_window_ranges(sqb_ctx* ctx, const void* xy, int xy_dtype, int64_t n, const int32_t* lib, int n_libs, const int64_t* edge_off,
+                      const void* starts, const void* ends, int32_t* out);
 
 /* ---- sepal ---------------------------------------------------------------------------------------------------------
  * `_diffusion` for every gene (src/squidpy/gr/_sepal.py:186-289): vals = n_genes x n float64 (one row per gene), sat / unsat =

@@ -665,6 +665,49 @@ __host__ __device__ __forceinline__ void sqb_part_magic(int B, uint32_t& M, int&
 }
 __device__ __forceinline__ int part_idx(int t) { return t + (t >> 6); }
 
+// Clocks build only (SQB_PART_CLOCKS, tools/jgen_phases.py): clock64() cycles of nhood_jgen_kernel<Q, true> as lane 0 of every
+// warp sees them, summed over the warps: each generator's waits for a free block buffer and its whole run, each partition
+// warp's waits for a full block buffer, its four phases per block and its whole run, and the number of blocks partitioned.
+enum SqbJgenClk {
+    SQB_JCLK_GEN_WAIT,   // generator: waits on the empty barriers
+    SQB_JCLK_GEN_RUN,    // generator: whole run
+    SQB_JCLK_PART_WAIT,  // partition warp: waits on the full barriers
+    SQB_JCLK_COUNT,      // partition warp: region counts (with the table clear)
+    SQB_JCLK_SCAN,       // partition warp: slot scan and count row
+    SQB_JCLK_SCATTER,    // partition warp: scatter into the output block
+    SQB_JCLK_STREAM,     // partition warp: stream-out to J
+    SQB_JCLK_PART_RUN,   // partition warp: whole run
+    SQB_JCLK_BLOCKS,     // count
+    SQB_JCLK_N
+};
+#ifdef SQB_PART_CLOCKS
+__device__ unsigned long long g_jgen_clk[SQB_JCLK_N];
+#define SQB_JCLK_START()                             \
+    unsigned long long jclk[SQB_JCLK_N] = {};        \
+    long long jclk_t = clock64();                    \
+    const long long jclk_0 = jclk_t
+#define SQB_JCLK_SKIP() jclk_t = clock64()
+#define SQB_JCLK(ph)                                           \
+    do {                                                       \
+        const long long t_ = clock64();                        \
+        jclk[ph] += (unsigned long long)(t_ - jclk_t);         \
+        jclk_t = t_;                                           \
+    } while (0)
+#define SQB_JCLK_COUNT(ph) ++jclk[ph]
+#define SQB_JCLK_END(ph)                                                                     \
+    do {                                                                                     \
+        jclk[ph] = (unsigned long long)(clock64() - jclk_0);                                 \
+        if (lane == 0)                                                                       \
+            for (int k_ = 0; k_ < SQB_JCLK_N; ++k_) atomicAdd(&g_jgen_clk[k_], jclk[k_]);    \
+    } while (0)
+#else
+#define SQB_JCLK_START()
+#define SQB_JCLK_SKIP()
+#define SQB_JCLK(ph)
+#define SQB_JCLK_COUNT(ph)
+#define SQB_JCLK_END(ph)
+#endif
+
 __device__ __forceinline__ void mbar_init(uint64_t* b, unsigned count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(b)), "r"(count) : "memory");
 }
@@ -686,6 +729,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* b, unsigned parity) {
 // Partition warp of nhood_jgen_kernel<Q, true>: block seq of its generator arrives in buffer seq & 1 (use seq >> 1 of it).
 // NW = packed words of the region scan: 8 when no segment has more than 16 regions, else 16.  The partition warp shares the
 // SM's issue slots with the generators, so the narrow scan is kept for the inputs that fit it.
+// NW = 8 keeps the table as 32-bit words (16 regions x 32 lanes, the same 2 KB), so that one shared-memory atomic counts a step
+// and one hands out its slot, with four steps' input loads issued ahead of them.  With the 16-bit table's load, add and store
+// every step waited for the previous step's store, and the partition warp, not the generator, set the pace of a pair
+// (tools/jgen_phases.py).  Counts kept in registers break that chain too but issue more instructions, and the SM's issue rate
+// bounds the pairs (DESIGN.md §3.1).  32 regions of 32-bit words would take 4 KB, so NW = 16 keeps the 16-bit table.
 template <int NW>
 __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uint32_t* __restrict__ J, int64_t stride,
                                                 int64_t perm0, int64_t n_perms, int64_t warps_total, int nseg,
@@ -695,7 +743,9 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
     uint64_t* bar = reinterpret_cast<uint64_t*>(pair);  // full[0], full[1], empty[0], empty[1]
     uint32_t* __restrict__ out = pair + 8 + 2 * SQB_PART_LP;
     uint16_t* __restrict__ tab = reinterpret_cast<uint16_t*>(out + L);  // tab[r * 32 + lane]: this lane's entries of region r, then its next slot
+    uint32_t* __restrict__ tab32 = reinterpret_cast<uint32_t*>(tab);   // NW = 8: the same as 32-bit words
     unsigned seq = 0;
+    SQB_JCLK_START();
     for (int64_t perm = perm0; perm < n_perms; perm += warps_total) {
         int64_t row = perm * nb_total;  // count row of the current block's segment, block 0
         for (int seg = 0; seg < nseg; ++seg) {
@@ -705,20 +755,47 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
                 uint32_t M;
                 sqb_part_regions(m, region_cap, R, B);
                 sqb_part_magic(B, M, sh);
+                const uint32_t nB = 0u - (uint32_t)B;
                 uint32_t* __restrict__ Jseg = J + perm * stride + seg_start[seg];
                 for (int blk = (m - 1) / L; blk >= 0; --blk, ++seq) {
                     const int bL = blk * L, t0 = blk == 0 ? 1 : 0, t1 = min(L, m - bL);
                     const int s0 = max(t0 - 64 * lane, 0), s1 = min(t1 - 64 * lane, 64);  // this lane's steps t = 64 lane + s
                     const uint32_t* __restrict__ in = pair + 8 + (seq & 1) * SQB_PART_LP + 65 * lane;
 #pragma unroll
-                    for (int r = 0; r < 2 * NW; ++r) tab[r * 32 + lane] = 0;
+                    for (int r = 0; r < 2 * NW; ++r) {
+                        if (NW == 8)
+                            tab32[r * 32 + lane] = 0;
+                        else
+                            tab[r * 32 + lane] = 0;
+                    }
+                    SQB_JCLK(SQB_JCLK_COUNT);
                     mbar_wait(&bar[seq & 1], (seq >> 1) & 1);
+                    SQB_JCLK(SQB_JCLK_PART_WAIT);
+                    if (NW == 8) {
+                        int s = s0;
+                        for (; s + 4 <= s1; s += 4) {
+                            uint32_t j[4];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) j[q] = in[s + q];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) atomicAdd(&tab32[(__umulhi(j[q], M) >> sh) * 32 + lane], 1u);
+                        }
+                        for (; s < s1; ++s) atomicAdd(&tab32[(__umulhi(in[s], M) >> sh) * 32 + lane], 1u);
+                    } else {
 #pragma unroll 4
-                    for (int s = s0; s < s1; ++s) ++tab[(__umulhi(in[s], M) >> sh) * 32 + lane];
+                        for (int s = s0; s < s1; ++s) ++tab[(__umulhi(in[s], M) >> sh) * 32 + lane];
+                    }
+                    SQB_JCLK(SQB_JCLK_COUNT);
                     // slots: region base + entries of the same region on higher lanes (earlier steps); 16-bit fields, 2 regions a word
                     uint32_t w[NW], x[NW];
 #pragma unroll
-                    for (int k = 0; k < NW; ++k) x[k] = w[k] = (uint32_t)tab[2 * k * 32 + lane] | ((uint32_t)tab[(2 * k + 1) * 32 + lane] << 16);
+                    for (int k = 0; k < NW; ++k) {
+                        if (NW == 8)
+                            w[k] = tab32[2 * k * 32 + lane] | (tab32[(2 * k + 1) * 32 + lane] << 16);
+                        else
+                            w[k] = (uint32_t)tab[2 * k * 32 + lane] | ((uint32_t)tab[(2 * k + 1) * 32 + lane] << 16);
+                        x[k] = w[k];
+                    }
 #pragma unroll
                     for (int d = 1; d < 32; d <<= 1)
 #pragma unroll
@@ -733,32 +810,72 @@ __device__ __forceinline__ void nhood_part_warp(uint32_t* __restrict__ pair, uin
                         const uint32_t lo = tot[k] & 0xFFFFu;
                         const uint32_t slot = (run | ((run + lo) << 16)) + x[k] - w[k];
                         run += lo + (tot[k] >> 16);
-                        tab[2 * k * 32 + lane] = (uint16_t)(slot & 0xFFFFu);
-                        tab[(2 * k + 1) * 32 + lane] = (uint16_t)(slot >> 16);
+                        if (NW == 8) {
+                            tab32[2 * k * 32 + lane] = slot & 0xFFFFu;
+                            tab32[(2 * k + 1) * 32 + lane] = slot >> 16;
+                        } else {
+                            tab[2 * k * 32 + lane] = (uint16_t)(slot & 0xFFFFu);
+                            tab[(2 * k + 1) * 32 + lane] = (uint16_t)(slot >> 16);
+                        }
                     }
                     if (lane == 0) {  // the count row: u16 counts of regions 0 .. 2 NW - 1, little-endian pairs = tot[]
                         uint4* crow = reinterpret_cast<uint4*>(cnt + (row + blk) * SQB_PART_RMAX);
 #pragma unroll
                         for (int q = 0; q < NW / 4; ++q) crow[q] = make_uint4(tot[4 * q], tot[4 * q + 1], tot[4 * q + 2], tot[4 * q + 3]);
                     }
+                    SQB_JCLK(SQB_JCLK_SCAN);
                     __syncwarp();  // every lane has streamed the previous output block out
+                    if (NW == 8) {  // in step order; entry = (t << 18) | (j - r B) = (t << 18) + j - r B, as j - r B < B <= 2^18
+                        int s = s1 - 1;
+                        for (; s - 3 >= s0; s -= 4) {
+                            uint32_t j[4], r[4], slot[4];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) j[q] = in[s - q];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) {
+                                r[q] = __umulhi(j[q], M) >> sh;
+                                slot[q] = atomicAdd(&tab32[r[q] * 32 + lane], 1u);
+                            }
+                            const uint32_t ts = (uint32_t)(64 * lane + s) << 18;
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) out[slot[q]] = r[q] * nB + (j[q] + ts - ((uint32_t)q << 18));
+                        }
+                        for (; s >= s0; --s) {
+                            const uint32_t j = in[s], r = __umulhi(j, M) >> sh;
+                            out[atomicAdd(&tab32[r * 32 + lane], 1u)] = r * nB + (j + ((uint32_t)(64 * lane + s) << 18));
+                        }
+                    } else {
 #pragma unroll 4
-                    for (int s = s1 - 1; s >= s0; --s) {  // in step order
-                        const uint32_t j = in[s];
-                        const uint32_t r = __umulhi(j, M) >> sh;
-                        const uint32_t slot = tab[r * 32 + lane];
-                        tab[r * 32 + lane] = (uint16_t)(slot + 1);
-                        out[slot] = ((uint32_t)(64 * lane + s) << 18) | (j - r * (uint32_t)B);
+                        for (int s = s1 - 1; s >= s0; --s) {  // in step order
+                            const uint32_t j = in[s];
+                            const uint32_t r = __umulhi(j, M) >> sh;
+                            const uint32_t slot = tab[r * 32 + lane];
+                            tab[r * 32 + lane] = (uint16_t)(slot + 1);
+                            out[slot] = ((uint32_t)(64 * lane + s) << 18) | (j - r * (uint32_t)B);
+                        }
                     }
                     mbar_arrive(&bar[2 + (seq & 1)]);  // the buffer is free for the generator
+                    SQB_JCLK(SQB_JCLK_SCATTER);
                     __syncwarp();
+                    // whole 16-byte vectors when the block starts 16-byte aligned in J (out always does); a library segment
+                    // may start anywhere
                     uint32_t* __restrict__ Jblk = Jseg + bL;
-                    for (int k = lane; k < t1 - t0; k += 32) __stcs(Jblk + k, out[k]);
+                    const int n = t1 - t0;
+                    int k = lane;
+                    if ((reinterpret_cast<uintptr_t>(Jblk) & 15u) == 0) {
+                        const uint4* __restrict__ out4 = reinterpret_cast<const uint4*>(out);
+                        for (; k < n >> 2; k += 32) __stcs(reinterpret_cast<uint4*>(Jblk) + k, out4[k]);
+                        k = (n & ~3) + lane;
+                    }
+                    for (; k < n; k += 32) __stcs(Jblk + k, out[k]);
+                    SQB_JCLK(SQB_JCLK_STREAM);
+                    SQB_JCLK_COUNT(SQB_JCLK_BLOCKS);
                 }
             }
             row += (m + L - 1) / L;
         }
     }
+    SQB_JCLK_END(SQB_JCLK_PART_RUN);
 }
 
 // J[top - c] = u when u <= i (an accepted value), streamed (evict-first): one multiply-add from the window's base address
@@ -812,6 +929,7 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
         }
     }
     unsigned seq = 0;  // PART: blocks handed to the partition warp so far
+    SQB_JCLK_START();
     const uint32_t lt_mask = (1u << lane) - 1u;
     // Q independent LCG chains per lane (output q*32 + lane of every batch has its own state, advanced by 32*Q per batch)
     // instead of one chain stepped Q times: the 128-bit multiply-adds of a batch no longer depend on each other
@@ -838,7 +956,11 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
             const int m = (int)seg_len[seg];
             int i_cur = m - 1;
             int blk = i_cur / L;  // PART: block of step i_cur
-            if (PART && i_cur >= 1) mbar_wait(&bar[2 + (seq & 1)], ((seq >> 1) & 1) ^ 1);  // its buffer is free
+            if (PART && i_cur >= 1) {
+                SQB_JCLK_SKIP();
+                mbar_wait(&bar[2 + (seq & 1)], ((seq >> 1) & 1) ^ 1);  // its buffer is free
+                SQB_JCLK(SQB_JCLK_GEN_WAIT);
+            }
             while (i_cur >= 1) {
                 if (pos >= RAW) {
 #pragma unroll
@@ -854,11 +976,12 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
                 const int i_lo = (int)(mask >> 1) + 1;
                 const int n_ph = i_cur - i_lo + 1;
                 // The common window, tested once per window with warp-uniform conditions: the whole fresh batch (pos = 0,
-                // K = RAW), no candidate whose acceptance depends on its rank (below), the phase goes on past the window
-                // (every accepted value is the target of a step of this phase) and, PART, the window stays inside block blk
-                // without completing it.  Only u and the ranks are live here; the acceptance flag of a value is u <= i_cur,
-                // re-tested where it is needed, and the stores are predicated on it.  Every other window (refills in
-                // mid-batch, ends of a phase or of a block, the small-i end where K = i/4) takes the general path below.
+                // K = RAW), no candidate whose acceptance depends on its rank (below) and the phase goes on past the window
+                // (every accepted value is the target of a step of this phase).  PART: a window that completes block blk
+                // hands it over and stores its lower steps into block blk - 1's buffer, as the general path does.  Only u
+                // and the ranks are live here; the acceptance flag of a value is u <= i_cur, re-tested where it is needed,
+                // and the stores are predicated on it.  Every other window (refills in mid-batch, ends of a phase, the
+                // small-i end where K = i/4) takes the general path below.
                 if (pos == 0 && (i_cur >> 2) >= RAW) {
                     uint32_t u[2 * Q];
                     bool uncertain = false;
@@ -878,17 +1001,34 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
                             run += __popc(blo) + __popc(bhi);
                         }
                         const int bL = blk * L;
-                        if (run < n_ph && (!PART || i_cur - run >= max(bL, 1))) {
+                        // run < n_ph keeps i_cur - run >= i_lo >= 1: the window never ends the segment
+                        if (run < n_ph) {
                             if (!PART) {
                                 uint32_t* __restrict__ Jtop = Jp + base + i_cur;
 #pragma unroll
                                 for (int k = 0; k < 2 * Q; ++k) st_cs_target(Jtop, c[k], u[k], i_cur);
-                            } else {
+                            } else if (i_cur - run >= bL) {  // inside block blk
                                 uint32_t* stage = pair + 8 + (seq & 1) * SQB_PART_LP;
                                 const int t = i_cur - bL;
 #pragma unroll
                                 for (int k = 0; k < 2 * Q; ++k)
                                     if (u[k] <= (uint32_t)i_cur) stage[part_idx(t - c[k])] = u[k];
+                            } else {  // completes block blk (bL >= 1 here) and opens block blk - 1 in the other buffer
+                                uint32_t* stage = pair + 8 + (seq & 1) * SQB_PART_LP;
+                                const int t = i_cur - bL;
+#pragma unroll
+                                for (int k = 0; k < 2 * Q; ++k)
+                                    if (u[k] <= (uint32_t)i_cur && c[k] <= t) stage[part_idx(t - c[k])] = u[k];
+                                mbar_arrive(&bar[seq & 1]);
+                                ++seq;
+                                --blk;
+                                SQB_JCLK_SKIP();
+                                mbar_wait(&bar[2 + (seq & 1)], ((seq >> 1) & 1) ^ 1);
+                                SQB_JCLK(SQB_JCLK_GEN_WAIT);
+                                stage = pair + 8 + (seq & 1) * SQB_PART_LP;
+#pragma unroll
+                                for (int k = 0; k < 2 * Q; ++k)
+                                    if (u[k] <= (uint32_t)i_cur && c[k] > t) stage[part_idx(t - c[k] + L)] = u[k];
                             }
                             i_cur -= run;
                             pos = RAW;
@@ -971,7 +1111,9 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
                         mbar_arrive(&bar[seq & 1]);
                         ++seq;
                         if (--blk >= 0) {  // the window's lower steps open block blk - 1 in the other buffer
+                            SQB_JCLK_SKIP();
                             mbar_wait(&bar[2 + (seq & 1)], ((seq >> 1) & 1) ^ 1);
+                            SQB_JCLK(SQB_JCLK_GEN_WAIT);
                             stage = pair + 8 + (seq & 1) * SQB_PART_LP;
 #pragma unroll
                             for (int k = 0; k < 2 * Q; ++k)
@@ -984,6 +1126,7 @@ __global__ void __launch_bounds__(PART ? 256 : 128, PART ? 2 : 1) nhood_jgen_ker
             }
         }
     }
+    if (PART) SQB_JCLK_END(SQB_JCLK_GEN_RUN);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3665,6 +3808,15 @@ int sqb_test_part_clocks(unsigned long long* out, int reset) {
     if (reset) {
         const unsigned long long zero[SQB_PCLK_N] = {};
         SQB_CUDA(cudaMemcpyToSymbol(g_part_clk, zero, sizeof(g_part_clk)));
+    }
+    return SQB_OK;
+}
+// clocks build only: the same for the SQB_JCLK_N clock totals of nhood_jgen_kernel<Q, true>
+int sqb_test_jgen_clocks(unsigned long long* out, int reset) {
+    if (out) SQB_CUDA(cudaMemcpyFromSymbol(out, g_jgen_clk, sizeof(g_jgen_clk)));
+    if (reset) {
+        const unsigned long long zero[SQB_JCLK_N] = {};
+        SQB_CUDA(cudaMemcpyToSymbol(g_jgen_clk, zero, sizeof(g_jgen_clk)));
     }
     return SQB_OK;
 }

@@ -35,6 +35,10 @@
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
  *   sqb_centrality_scores      <- _build_graph + rx.group_degree_centrality / rx.group_closeness_centrality + _local_clustering
  *                                 src/squidpy/gr/_nhood.py:305-317,432-491
+ *   sqb_niche_profile          <- _NhoodProfileEmbedder: _calculate_neighborhood_profile + the hop loop of get_embedding
+ *                                 src/squidpy/gr/_niche.py:1117-1169,1176-1214
+ *   sqb_niche_aggregate        <- normalize(A, "l1") @ X of _UtagEmbedder (:1259-1260); _setdiag, _hop, _normalize, _aggregate
+ *                                 and hstack(...).toarray() of _CellcharterEmbedder (:1002-1054,1336-1355)
  */
 #ifndef SQUIDPY_B200_H
 #define SQUIDPY_B200_H
@@ -46,7 +50,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 13
+#define SQB_ABI_VERSION 14
 
 typedef enum {
     SQB_OK = 0,
@@ -452,6 +456,45 @@ int sqb_graph_build_device(sqb_ctx* ctx, const void* xy, int xy_dtype, int64_t n
 int sqb_graph_export(sqb_graph* g, int32_t* adj_indptr, int32_t* adj_indices, float* adj_data, int32_t* dst_indptr,
                      int32_t* dst_indices, void* dst_data, uintptr_t consumer_stream);
 int sqb_graph_free(sqb_graph* g);
+
+/* ---- calculate_niche embeddings -----------------------------------------------------------------------------------
+ * The graph (both entry points): an n x n CSR (csc = 0) or CSC (csc = 1) from the host (device_input = 0) or from device memory
+ * (device_input = 1: DEVICE pointers on the context's device, read in place after producer_stream, as in
+ * sqb_autocorr_load_csr_device).  indptr_bits / index_bits 32 or 64; data_dtype 0 f32, 1 f64, 3 i32, 4 i64 (boolean graphs are
+ * refused: scipy combines them with logical and / or); nnz < 2^31; data may be NULL when nnz = 0.  Integer values are taken as
+ * their float64 values, exact while the reference's integer sums do not overflow the graph's dtype.  Duplicates are summed
+ * (in float32 for a float32 graph) where the reference's scipy calls sum them.  Both return once the device has stopped
+ * reading the caller's buffers.
+ *
+ * sqb_niche_profile: the neighbourhood-profile embedding (src/squidpy/gr/_niche.py:1117-1214).  codes[v] in [-1, n_cls): the
+ * category of observation v (-1: NaN, a row that counts towards no column).  P_1 = A Y (Y the one-hot codes), P_k = A P_{k-1},
+ * summed in float64 over ascending columns.  Per hop p_k = P_k (abs_nhood) or P_k / (row total), NaN (a zero total) -> 0.
+ * out (HOST, n x n_cls float64 row-major) = p_1 when distance = 1, else w_0 p_1 + w_1 p_2 + ... (weights: distance entries,
+ * already extended), divided by weight_sum (the sum of every weight given) unless abs_nhood.
+ * Exactness: bit for bit with the reference for integer-valued graphs whose path sums stay below 2^24; for other weights within
+ * float32 rounding of it, and bit for bit with this float64 statement.
+ *
+ * sqb_niche_aggregate: X is n x m, dense row-major contiguous (x_format 0) or CSR (x_format 1: x = values, x_indptr / x_indices
+ * of x_indptr_bits / x_index_bits), float32 (x_f32 = 1) or float64 values, on the host (x_device = 0) or the device (x_device = 1,
+ * after x_stream).  Duplicate X entries add up.  out (HOST, row-major) is float32 (out_f32) or float64: the dtype numpy's upcast gives.
+ *   mode 0, UTAG (:1259-1260): normalize(A, "l1", axis=1) in the graph's storage order (a CSC transposed as scipy's tocsr
+ *     does it): row sum of |a| in float64, a / sum rounded once to the value type, a zero row unchanged; out (n x m) = N X
+ *     accumulated over each row's entries in that order, in float32 when N and X are float32, else float64.  Bit for bit.
+ *   modes 1 (mean) / 2 (variance), CellCharter (:1336-1355): from the canonical A, hop_1 = A without diagonal and zeros,
+ *     visited = A with diagonal 1, hop_k = (hop_{k-1} A) > visited compared on path sums in the value type, visited += hop_k.
+ *     out (n x (distance + 1) m) = [X, agg_1, ..., agg_distance] where agg_k = N_k X (mean) or N_k (X∘X) - (N_k X)² (variance),
+ *     N_1 = diag(1 / deg) hop_1 in the value type (deg: numpy's pairwise row sum) taken in reverse column order as scipy's SpGEMM
+ *     stores it, N_k (k >= 2) = 1 / |row| over the hop set in ascending columns, in float64.  out_hop_nnz[k - 1] = nnz of hop_k.
+ *     hop_1's aggregate is bit for bit; hop sets are identical; hop >= 2 aggregates are bit for bit with this statement (the
+ *     reference's own order, fixed by scipy's non-canonical sparse binops, differs within 1e-12 relative).                  */
+int sqb_niche_profile(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                      const void* data, int data_dtype, int csc, int device_input, uintptr_t producer_stream, const int32_t* codes,
+                      int n_cls, int distance, const double* weights, double weight_sum, int abs_nhood, double* out);
+int sqb_niche_aggregate(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                        const void* data, int data_dtype, int csc, int device_input, uintptr_t producer_stream, const void* x,
+                        const void* x_indptr, const void* x_indices, int64_t x_nnz, int x_format, int x_indptr_bits, int x_index_bits,
+                        int x_f32, int64_t m, int x_device, uintptr_t x_stream, int mode, int distance, int out_f32, void* out,
+                        int64_t* out_hop_nnz);
 
 #ifdef __cplusplus
 }

@@ -57,10 +57,13 @@ class AnnDataLite:
     def copy(self) -> "AnnDataLite":
         import copy as _copy
 
+        def dup(v):
+            return v.clone() if hasattr(v, "clone") and not hasattr(v, "copy") else v.copy()  # torch tensors clone
+
         return AnnDataLite(
-            X=None if self.X is None else self.X.copy(), obs=self.obs.copy(), var=self.var.copy(),
-            obsm={k: v.copy() for k, v in self.obsm.items()}, obsp={k: v.copy() for k, v in self.obsp.items()},
-            uns=_copy.deepcopy(self.uns), layers={k: v.copy() for k, v in self.layers.items()}, raw=self.raw,
+            X=None if self.X is None else dup(self.X), obs=self.obs.copy(), var=self.var.copy(),
+            obsm={k: dup(v) for k, v in self.obsm.items()}, obsp={k: dup(v) for k, v in self.obsp.items()},
+            uns=_copy.deepcopy(self.uns), layers={k: dup(v) for k, v in self.layers.items()}, raw=self.raw,
             shape=self._shape,
         )
 
@@ -80,9 +83,39 @@ class AnnDataLite:
             raise KeyError(f"Values {missing} are not valid var names or indices.")
         return ix
 
+    def _obs_indexer(self, sel: Any) -> np.ndarray:
+        if isinstance(sel, slice):
+            return np.arange(self.n_obs)[sel]
+        if isinstance(sel, (pd.Series, pd.Index)):
+            sel = sel.to_numpy()
+        sel = np.asarray(sel)
+        if sel.dtype == bool:
+            return np.flatnonzero(sel)
+        if sel.dtype.kind in "iu":
+            return sel.astype(np.int64)
+        ix = self.obs.index.get_indexer(np.atleast_1d(sel))
+        if (ix < 0).any():
+            missing = [str(s) for s, i in zip(np.atleast_1d(sel), ix) if i < 0]
+            raise KeyError(f"Values {missing} are not valid obs names or indices.")
+        return ix
+
+    def _obs_subset(self, sel: Any) -> "AnnDataLite":
+        """``adata[obs]`` / ``adata[obs, :]``: the rows of X, obs, obsm, layers and an AnnDataLite ``raw``, the rows and columns of
+        obsp.  Integer selections are positions, as in AnnData; obs names select by label."""
+        ri = self._obs_indexer(sel)
+        return AnnDataLite(X=None if self.X is None else _take(self.X, ri), obs=self.obs.iloc[ri], var=self.var,
+                           obsm={k: _take(v, ri) for k, v in self.obsm.items()}, obsp={k: _take(v, ri, both=True) for k, v in self.obsp.items()},
+                           uns=self.uns, layers={k: _take(v, ri) for k, v in self.layers.items()},
+                           raw=self.raw[ri] if isinstance(self.raw, AnnDataLite) else self.raw, shape=(len(ri), self.n_vars))
+
     def __getitem__(self, index):
-        if not isinstance(index, tuple) or len(index) != 2:
-            raise NotImplementedError("AnnDataLite only supports `adata[:, vars]` / `adata[obs, vars]` indexing")
+        if not isinstance(index, tuple):
+            return self._obs_subset(index)
+        if len(index) == 2 and isinstance(index[1], slice) and index[1] == slice(None) and not (
+                isinstance(index[0], slice) and index[0] == slice(None)):
+            return self._obs_subset(index[0])
+        if len(index) != 2:
+            raise NotImplementedError("AnnDataLite only supports `adata[obs]`, `adata[:, vars]` and `adata[obs, vars]` indexing")
         rows, cols = index
         ci = self._var_indexer(cols)
         ri = slice(None) if (isinstance(rows, slice) and rows == slice(None)) else rows
@@ -92,3 +125,26 @@ class AnnDataLite:
         return AnnDataLite(X=X, obs=obs, var=self.var.iloc[ci], obsm=self.obsm if isinstance(ri, slice) else {},
                            obsp=self.obsp if isinstance(ri, slice) else {}, uns=self.uns, layers=layers,
                            shape=(len(obs), len(ci)))
+
+
+def _take(a: Any, ri: np.ndarray, both: bool = False) -> Any:
+    """Rows ``ri`` of ``a`` (and the same columns when ``both``): numpy, scipy, pandas, or a torch tensor, sparse ones included,
+    which stay on their device and keep their layout."""
+    if hasattr(a, "iloc"):
+        return a.iloc[ri, ri] if both else a.iloc[ri]
+    import sys
+
+    torch = sys.modules.get("torch")
+    if torch is not None and isinstance(a, torch.Tensor):
+        idx = torch.as_tensor(ri, dtype=torch.int64, device=a.device)
+        if a.layout == torch.strided:
+            out = a.index_select(0, idx)
+            return out.index_select(1, idx) if both else out
+        layout = a.layout
+        out = a.to_sparse_coo().index_select(0, idx)
+        if both:
+            out = out.index_select(1, idx)
+        out = out.coalesce()
+        return out.to_sparse_csr() if layout == torch.sparse_csr else out.to_sparse_csc() if layout == torch.sparse_csc else out
+    return a[ri][:, ri] if both else a[ri]
+

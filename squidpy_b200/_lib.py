@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
 # phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -133,6 +133,11 @@ _SIGNATURES: dict[str, tuple] = {
                                         C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sqb_window_ranges": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p]),
+    "sqb_niche_profile": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                    C.c_int, C.c_size_t, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_double, C.c_int, C.c_void_p]),
+    "sqb_niche_aggregate": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                      C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int64, C.c_int, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -3,6 +3,8 @@
 from ._build import (GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, knn_2d, radius_2d, spatial_neighbors_grid,
                      spatial_neighbors_knn, spatial_neighbors_radius)
 from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
+from ._niche import (calculate_niche, calculate_niche_cellcharter, calculate_niche_neighborhood, calculate_niche_spatialleiden,
+                     calculate_niche_utag, niche_aggregate, niche_profile)
 from ._nhood import NhoodEnrichmentResult, NhoodPlan, centrality_counts, centrality_scores, interaction_matrix, nhood_enrichment
 from ._ppatterns import AutocorrPlan, co_occurrence, cooc_counts, spatial_autocorr
 from ._ripley import nn_distance_hist, pair_counts, ripley
@@ -27,6 +29,13 @@ __all__ = [
     "interaction_matrix",
     "centrality_scores",
     "centrality_counts",
+    "calculate_niche",
+    "calculate_niche_neighborhood",
+    "calculate_niche_utag",
+    "calculate_niche_cellcharter",
+    "calculate_niche_spatialleiden",
+    "niche_profile",
+    "niche_aggregate",
     "spatial_autocorr",
     "co_occurrence",
     "ripley",

@@ -31,6 +31,7 @@
  *   sqb_nn_min_dist_f64        <- KDTree(anchor_coord, metric=...).query(batch_coord)  src/squidpy/tl/_var_by_distance.py:129-134
  *   sqb_window_ranges          <- the per-window coordinate masks of sliding_window  src/squidpy/tl/_sliding_window.py:130-158
  *   sqb_knn_2d / sqb_radius_2d <- NearestNeighbors.kneighbors / radius_neighbors src/squidpy/gr/neighbors.py:192-209,253-270,395-419
+ *   sqb_delaunay_2d            <- scipy.spatial.Delaunay(coords).vertex_neighbor_vertices  src/squidpy/gr/neighbors.py:318-332
  *   sqb_graph_*                <- GraphBuilder.build + GraphBuilderCSR.combine  src/squidpy/gr/neighbors.py:80-156,192-209,253-270,365-477
  *   sqb_interaction_matrix     <- _interaction_matrix(data, indices, indptr, cats, out)  src/squidpy/gr/_nhood.py:412-429
  *   sqb_centrality_scores      <- _build_graph + rx.group_degree_centrality / rx.group_closeness_centrality + _local_clustering
@@ -50,7 +51,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 14
+#define SQB_ABI_VERSION 15
 
 typedef enum {
     SQB_OK = 0,
@@ -429,6 +430,15 @@ int sqb_knn_2d(sqb_ctx* ctx, const double* xy, int64_t n, int k, int32_t* out_id
 int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int64_t* out_indptr, int32_t* out_idx,
                   double* out_dist, int64_t capacity, int64_t* nnz_out);
 
+/* The Delaunay graph of n points (DelaunayBuilder.build_graph, neighbors.py:318-332): row i lists the Delaunay neighbours of
+ * observation i in ascending order.  Exact predicates; exactly cocircular points are resolved by a symbolic perturbation of
+ * x^2 + y^2 by index (one fixed triangulation); exact duplicates are collapsed to the lowest index of their group, the other
+ * copies get empty rows.  Two calls as sqb_radius_2d (out_idx == NULL: out_indptr and *nnz_out only; nnz < 6n always, so one
+ * call with capacity 6n suffices).  Fewer than three distinct points or all distinct points collinear: SQB_ERR_INVALID with a
+ * message starting "QhullError".  out_pass_counts: NULL or int64[2], the points finished by pass 1 and by pass 2.          */
+int sqb_delaunay_2d(sqb_ctx* ctx, const double* xy, int64_t n, int64_t* out_indptr, int32_t* out_idx, int64_t capacity,
+                    int64_t* nnz_out, int64_t* out_pass_counts);
+
 /* ---- spatial neighbour graphs from coordinates in GPU memory, kept there ---------------------------------------------
  * The whole builder on the device: search, cut, ring expansion, diagonals, interval / percentile pruning, eliminate_zeros,
  * transform and the library block diagonal of KNNBuilder / GridBuilder / RadiusBuilder.build and GraphBuilderCSR.combine
@@ -437,7 +447,9 @@ int sqb_radius_2d(sqb_ctx* ctx, const double* xy, int64_t n, double radius, int6
  *   xy: DEVICE pointer on the context's device to n x 2 coordinates, xy_dtype 0 float32 / 1 float64, element strides
  *   stride_row / stride_col (any); never read on the host.  producer_stream: as in sqb_autocorr_load_csr_device.
  *   kind 0 kNN (n_neighbors in [1, 64]), 1 grid (n_neighbors, n_rings >= 1, 1.3 x median cut), 2 radius (radius; interval != 0
- *   prunes to [radius_min, radius_max] like a tuple radius).  set_diag as the builders'.  percentile: NaN for none (kNN /
+ *   prunes to [radius_min, radius_max] like a tuple radius), 3 Delaunay (as sqb_delaunay_2d; interval as for radius; the
+ *   distances are computed in the coordinates' dtype, so float32 coordinates give float32 distances, and the interval bounds
+ *   and the percentile follow numpy's float32 arithmetic).  set_diag as the builders'.  percentile: NaN for none (kNN /
  *   radius).  transform 0 none, 1 spectral, 2 cosine.
  *   lib_ptr / lib_rows (HOST, or NULL with n_libs = 0): library b is the ascending rows lib_rows[lib_ptr[b] .. lib_ptr[b+1]) of
  *   the coordinates; each is built as its own block, the blocks are combined in the order of the rows.

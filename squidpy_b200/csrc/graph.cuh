@@ -15,6 +15,43 @@ struct PointGrid {
     DevBuf<int32_t> d_idx_sorted, d_cell_start;
 };
 
+__device__ __forceinline__ int grid_cell_coord(double v, double v0, double inv, int g) {
+    int c = (int)floor((v - v0) * inv);
+    return c < 0 ? 0 : (c >= g ? g - 1 : c);
+}
+
+// Lower bound on the squared distance from q to every point of the grid outside the visited square of cells
+// [cx - r, cx + r] x [cy - r, cy + r]: the minimum over the square's sides that still have cells beyond them of (separation
+// along that axis)^2 + (distance from q to the grid box along the other axis)^2.  It holds for queries outside the box too
+// (their cell is clamped to the box), where r cells alone would be a loose bound.  Both terms are shrunk by a slack
+// proportional to the box's coordinates: the cell assignment of a point is a rounded computation.  Returns -1 when no cell
+// is left (the walk is complete).
+__device__ __forceinline__ double grid_unvisited_bound(const GridGeom gm, double2 q, int cx, int cy, int r) {
+    const double bx1 = gm.x0 + gm.gx * gm.cell, by1 = gm.y0 + gm.gy * gm.cell;
+    const double slack = 1e-12 * (fabs(gm.x0) + fabs(gm.y0) + fabs(bx1) + fabs(by1));
+    const double ox = fmax(fmax(gm.x0 - q.x, q.x - bx1) - slack, 0.0), oy = fmax(fmax(gm.y0 - q.y, q.y - by1) - slack, 0.0);
+    const double oy2 = __dmul_rn(oy, oy), ox2 = __dmul_rn(ox, ox);
+    double lb = INFINITY;
+    bool left = false;
+    if (cx + r + 1 < gm.gx) {
+        const double s = fmax(gm.x0 + (cx + r + 1) * gm.cell - q.x - slack, 0.0);
+        lb = fmin(lb, s * s + oy2), left = true;
+    }
+    if (cx - r - 1 >= 0) {
+        const double s = fmax(q.x - (gm.x0 + (cx - r) * gm.cell) - slack, 0.0);
+        lb = fmin(lb, s * s + oy2), left = true;
+    }
+    if (cy + r + 1 < gm.gy) {
+        const double s = fmax(gm.y0 + (cy + r + 1) * gm.cell - q.y - slack, 0.0);
+        lb = fmin(lb, s * s + ox2), left = true;
+    }
+    if (cy - r - 1 >= 0) {
+        const double s = fmax(q.y - (gm.y0 + (cy - r) * gm.cell) - slack, 0.0);
+        lb = fmin(lb, s * s + ox2), left = true;
+    }
+    return left ? lb : -1.0;
+}
+
 // Grid geometry from the bounding box of n points: square cells of edge `cell_hint` (or sized for `pts_per_cell` points per
 // cell when the hint is 0), coarsened until the grid has at most ~4n + 16 cells.
 GridGeom grid_geometry(double x0, double y0, double x1, double y1, int64_t n, double cell_hint, double pts_per_cell);

@@ -7,6 +7,7 @@
 //   GraphBuilder.build -> _filter_by_radius_interval /       :80-135, :423-452             (interval and percentile pruning,
 //     _apply_percentile / _apply_transform                   :455-477                       eliminate_zeros, spectral / cosine)
 //   GraphBuilderCSR.combine                                  :138-156                       (library_key block diagonal)
+//   DelaunayBuilder.build_graph                              :318-332                       (Delaunay graph, delaunay.cu)
 // Every value equals the host path's bit for bit (squidpy_b200/gr/_build.py; DESIGN.md §3.4 has the argument per step):
 //  * entries are those of the host's CSR after eliminate_zeros: the host's explicit zeros (setdiag, pruning) only matter to
 //    the percentile, whose order statistics include them here too (the n diagonal zeros lead the sorted distances);
@@ -25,9 +26,9 @@
 
 #include <vector>
 
-#include "graph.cuh"
+#include "delaunay.cuh"
 
-enum { GD_KNN = 0, GD_GRID = 1, GD_RADIUS = 2 };
+enum { GD_KNN = 0, GD_GRID = 1, GD_RADIUS = 2, GD_DELAUNAY = 3 };
 enum { GD_NONE = 0, GD_SPECTRAL = 1, GD_COSINE = 2 };
 enum { DST_DIST = 0, DST_ADJ = 1, DST_VAL = 2 };  // distances value: the distance (f64), the connectivity (f32), the table value (f32)
 
@@ -122,6 +123,24 @@ int percentile_linear(double q_pct, int64_t m, double* thr, int (*get)(void*, in
     double r = a + diff * gamma;
     if (gamma >= 0.5) r = b - diff * (1.0 - gamma);
     *thr = r;
+    return SQB_OK;
+}
+
+// The same for float32 values, in numpy's float32 arithmetic (NEP 50: the Python-float percentile and the Python-int counts
+// are cast to float32): q = float32(p) / 100, the virtual index (m - 1) * q, its fraction and the interpolation all in float32.
+int percentile_linear_f32(double q_pct, int64_t m, double* thr, int (*get)(void*, int64_t, double*), void* env) {
+    const float q = (float)q_pct / 100.0f;
+    const float vi = (float)(m - 1) * q;
+    int64_t ip = (int64_t)floorf(vi), in = ip + 1;
+    float gamma = vi - (float)ip;
+    if (vi >= (float)(m - 1)) ip = in = m - 1, gamma = (float)((double)vi + 1.0);  // numpy's index -1
+    double a, b;
+    SQB_TRY(get(env, ip, &a));
+    SQB_TRY(get(env, in, &b));
+    const float fa = (float)a, fb = (float)b, diff = fb - fa;
+    float r = fa + diff * gamma;
+    if (gamma >= 0.5f) r = fb - diff * (1.0f - gamma);
+    *thr = (double)r;
     return SQB_OK;
 }
 
@@ -547,8 +566,11 @@ int pct_get(void* env, int64_t i, double* v) {
 // One graph (or one library's block), before its transform, from the rows `rows` (device, or null: all n) of the caller's
 // coordinates.  Its temporaries are freed when it returns.
 int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64_t n, const Params& P, Csr* adj, Csr* dst) {
-    const bool knn = P.kind != GD_RADIUS;
-    if (knn) {  // the checks and messages of sqb_knn_2d / sqb_radius_2d, in their order
+    const bool knn = P.kind == GD_KNN || P.kind == GD_GRID;
+    if (P.kind == GD_DELAUNAY) {
+        SQB_CHECK(n >= 3, SQB_ERR_INVALID,
+                  "QhullError: the Delaunay triangulation needs at least three distinct points that are not all collinear");
+    } else if (knn) {  // the checks and messages of sqb_knn_2d / sqb_radius_2d, in their order
         SQB_CHECK(n >= 2 && n < 2147483647LL, SQB_ERR_INVALID, "sqb_knn_2d: n=%lld out of range", (long long)n);
         SQB_CHECK(P.k >= 1 && P.k <= 64, SQB_ERR_UNSUPPORTED, "sqb_knn_2d: n_neighbors=%d outside [1, 64]", P.k);
         SQB_CHECK(P.k < n, SQB_ERR_INVALID, "Expected n_neighbors <= n_samples_fit, but n_neighbors = %d, n_samples_fit = %lld, n_samples = %lld",
@@ -584,13 +606,18 @@ int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64
         first_bad = hbad[b] < first_bad ? hbad[b] : first_bad;
     }
     SQB_CHECK(first_bad == LLONG_MAX, SQB_ERR_INVALID, "coordinates of observation %lld are not finite", first_bad);
-    g.gm = knn ? grid_geometry(x0, y0, x1, y1, n, 0.0, knn_pts_per_cell(P.k))
-               : grid_geometry(x0, y0, x1, y1, n, P.radius > 0.0 ? P.radius : 0.0, 2.5);
+    g.gm = P.kind == GD_DELAUNAY ? grid_geometry(x0, y0, x1, y1, n, 0.0, DT_PTS_PER_CELL)
+           : knn                 ? grid_geometry(x0, y0, x1, y1, n, 0.0, knn_pts_per_cell(P.k))
+                                 : grid_geometry(x0, y0, x1, y1, n, P.radius > 0.0 ? P.radius : 0.0, 2.5);
     SQB_TRY(grid_bucket(c, n, &g));
     // the neighbour table as rows of ascending columns: bptr / idx / dist
     int64_t m;
     SQB_TRY(bptr.alloc(n + 1));
-    if (knn) {
+    if (P.kind == GD_DELAUNAY) {
+        SQB_TRY(delaunay_csr(c, g, n, bptr, idx, &m, nullptr));
+        SQB_TRY(dist.alloc(m));
+        if (m > 0) SQB_TRY(delaunay_dist(c, g.d_xy.p, bptr.p, idx.p, n, xy.dtype == 0, dist.p));
+    } else if (knn) {
         m = n * P.k;
         SQB_TRY(idx.alloc(m));
         SQB_TRY(dist.alloc(m));
@@ -638,11 +665,15 @@ int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64
     ap.diag = P.set_diag || P.interval || !isnan(P.percentile);  // _Builder._diagonals
     ap.diag_adj = P.set_diag ? 1.0f : 0.0f;
     ap.interval = P.interval, ap.lo = P.lo, ap.hi = P.hi, ap.dst_mode = DST_DIST;
+    // float32 Delaunay distances are compared with the bounds cast to float32, as numpy compares a float32 array with a
+    // Python float; the float32 values themselves are exact in float64
+    const bool f32 = P.kind == GD_DELAUNAY && xy.dtype == 0;
+    if (f32) ap.lo = (double)(float)P.lo, ap.hi = (double)(float)P.hi;
     if (!isnan(P.percentile)) {
         SQB_TRY(bval.alloc(m));
         SQB_TRY(sorted.alloc(m));
         if (m > 0) {
-            GD_LAUNCH(gd_masked_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(dist.p, m, P.interval, P.lo, P.hi, bval.p));
+            GD_LAUNCH(gd_masked_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(dist.p, m, P.interval, ap.lo, ap.hi, bval.p));
             size_t bytes = 0;
             SQB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
             SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
@@ -650,9 +681,9 @@ int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64
             c->launches += 1;
         }
         PctEnv env{c, sorted.p, n};
-        SQB_TRY(percentile_linear(P.percentile, m + n, &ap.thr, pct_get, &env));
+        SQB_TRY((f32 ? percentile_linear_f32 : percentile_linear)(P.percentile, m + n, &ap.thr, pct_get, &env));
     }
-    return assemble(c, bptr.p, idx.p, dist.p, n, ap, true, adj, dst);
+    return assemble(c, bptr.p, idx.p, dist.p, n, ap, !f32, adj, dst);
 }
 
 // One graph (or one library's block) with its transform
@@ -714,13 +745,13 @@ int sqb_graph_build_device(sqb_ctx* c, const void* xy, int xy_dtype, int64_t n, 
     SQB_CHECK(xy || n == 0, SQB_ERR_INVALID, "%s: null coordinates", where);
     SQB_CHECK(xy_dtype == 0 || xy_dtype == 1, SQB_ERR_INVALID, "%s: xy_dtype must be 0 (float32) or 1 (float64)", where);
     SQB_CHECK(n >= 0 && n < 2147483647LL, SQB_ERR_INVALID, "%s: n=%lld out of range", where, (long long)n);
-    SQB_CHECK(kind >= GD_KNN && kind <= GD_RADIUS, SQB_ERR_INVALID, "%s: kind must be 0 (kNN), 1 (grid) or 2 (radius)", where);
+    SQB_CHECK(kind >= GD_KNN && kind <= GD_DELAUNAY, SQB_ERR_INVALID, "%s: kind must be 0 (kNN), 1 (grid), 2 (radius) or 3 (Delaunay)", where);
     SQB_CHECK(transform >= GD_NONE && transform <= GD_COSINE, SQB_ERR_INVALID, "%s: transform must be 0 (none), 1 (spectral) or 2 (cosine)", where);
     SQB_CHECK(kind != GD_GRID || n_rings >= 1, SQB_ERR_INVALID, "%s: n_rings must be positive", where);
     SQB_CHECK(kind != GD_RADIUS || (radius >= 0.0 && isfinite(radius)), SQB_ERR_INVALID, "sqb_radius_2d: radius must be finite and non-negative");
     SQB_CHECK(isnan(percentile) || (percentile >= 0.0 && percentile <= 100.0), SQB_ERR_INVALID, "Percentiles must be in the range [0, 100]");
     SQB_CHECK(n_libs >= 0 && (n_libs == 0 || (lib_ptr && lib_rows)), SQB_ERR_INVALID, "%s: library index lists missing", where);
-    Params P{kind, n_neighbors, n_rings, set_diag ? 1 : 0, kind == GD_RADIUS && interval ? 1 : 0, transform, radius, radius_min, radius_max,
+    Params P{kind, n_neighbors, n_rings, set_diag ? 1 : 0, (kind == GD_RADIUS || kind == GD_DELAUNAY) && interval ? 1 : 0, transform, radius, radius_min, radius_max,
              kind == GD_GRID ? NAN : percentile};
     // libraries: ascending, distinct rows of [0, n); output row = rank among all listed rows (the host's argsort of the blocks)
     std::vector<int32_t> rank;

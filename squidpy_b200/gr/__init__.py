@@ -1,7 +1,8 @@
 """``squidpy_b200.gr`` — the spatial-statistics hot path of ``squidpy.gr`` on an H100."""
 
-from ._build import (GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, knn_2d, radius_2d, spatial_neighbors_grid,
-                     spatial_neighbors_knn, spatial_neighbors_radius)
+from ._build import (DelaunayBuilder, GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, delaunay_2d, knn_2d, radius_2d,
+                     spatial_neighbors_delaunay, spatial_neighbors_from_builder, spatial_neighbors_grid, spatial_neighbors_knn,
+                     spatial_neighbors_radius)
 from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
 from ._niche import (calculate_niche, calculate_niche_cellcharter, calculate_niche_neighborhood, calculate_niche_spatialleiden,
                      calculate_niche_utag, niche_aggregate, niche_profile)
@@ -14,7 +15,11 @@ __all__ = [
     "spatial_neighbors_knn",
     "spatial_neighbors_grid",
     "spatial_neighbors_radius",
+    "spatial_neighbors_delaunay",
+    "spatial_neighbors_from_builder",
     "SpatialNeighborsResult",
+    "DelaunayBuilder",
+    "delaunay_2d",
     "KNNBuilder",
     "GridBuilder",
     "RadiusBuilder",

@@ -1,14 +1,17 @@
 """Spatial neighbour graphs on the GPU — drop-ins for ``squidpy.gr.spatial_neighbors_knn / _grid / _radius``
 (``src/squidpy/gr/_build.py:484-549, 553-620, 701-786``) and the builder classes behind them
-(``src/squidpy/gr/neighbors.py``: ``KNNBuilder`` :157-209, ``RadiusBuilder`` :212-270, ``GridBuilder`` :335-419).
+(``src/squidpy/gr/neighbors.py``: ``KNNBuilder`` :157-209, ``RadiusBuilder`` :212-270, ``GridBuilder`` :335-419), plus
+``spatial_neighbors_delaunay`` / ``DelaunayBuilder`` (``_build.py:625-697``, ``neighbors.py:272-332``) and the public bridge
+``spatial_neighbors_from_builder`` (``_build.py:388-460``).
 
 This is the step right before every hot-path call (SURVEY.md 8f-1): at 1M spots the scikit-learn KD-tree query costs
 seconds where the statistics now cost milliseconds.  The neighbour search runs on the H100 (``sqb_knn_2d`` /
 ``sqb_radius_2d``: exact, float64, scikit-learn's arithmetic, rows in CSR order); the cheap O(nnz) post-processing
 (percentile / interval pruning, spectral / cosine transform, ring expansion, library block-diagonal) follows the
 reference's scipy code on the host.  Output contract as in the reference: ``obsp['{key}_connectivities']`` CSR float32,
-``obsp['{key}_distances']`` CSR, ``uns['{key}_neighbors']`` with the parameters.  Delaunay-based graphs are not offered
-(Qhull has no counterpart here); they raise ``NotImplementedError``.
+``obsp['{key}_distances']`` CSR, ``uns['{key}_neighbors']`` with the parameters.  The Delaunay graph is triangulated on the GPU
+with exact predicates (``sqb_delaunay_2d``, DESIGN.md §3.10); ``GridBuilder(delaunay=True)`` still raises
+``NotImplementedError``.
 
 Coordinates already in GPU memory (a torch CUDA tensor or any ``__cuda_array_interface__`` exporter of shape (n, 2), float32
 or float64, any strides) take the device path instead (``sqb_graph_build_device``): search AND post-processing run on the
@@ -31,8 +34,9 @@ from .._lib import Context, check, default_context, load, pointer_device
 from .._validators import assert_categorical_obs, assert_positive, assert_spatial_basis, extract_adata_if_sdata
 from ._utils import _save_data, logg
 
-__all__ = ["spatial_neighbors_knn", "spatial_neighbors_grid", "spatial_neighbors_radius", "SpatialNeighborsResult",
-           "KNNBuilder", "GridBuilder", "RadiusBuilder", "knn_2d", "radius_2d"]
+__all__ = ["spatial_neighbors_knn", "spatial_neighbors_grid", "spatial_neighbors_radius", "spatial_neighbors_delaunay",
+           "spatial_neighbors_from_builder", "SpatialNeighborsResult", "KNNBuilder", "GridBuilder", "RadiusBuilder", "DelaunayBuilder",
+           "knn_2d", "radius_2d", "delaunay_2d"]
 
 
 class SpatialNeighborsResult(NamedTuple):
@@ -81,6 +85,34 @@ def radius_2d(coords, radius: float, *, ctx: Context | None = None):
         dist = np.empty(max(nnz.value, 1), dtype=np.float64)
         check(lib.sqb_radius_2d(ctx.handle, xy.ctypes.data, n, float(radius), indptr.ctypes.data, idx.ctypes.data, dist.ctypes.data, idx.size, C.byref(nnz)))
     return indptr, idx[: nnz.value], dist[: nnz.value]
+
+
+def delaunay_2d(coords, *, ctx: Context | None = None, pass_counts: bool = False):
+    """``scipy.spatial.Delaunay(coords).vertex_neighbor_vertices`` on the GPU: ``(indptr int64[n+1], idx int32[nnz])`` with every
+    row in ascending column order (and the points finished by pass 1 and pass 2 if ``pass_counts``).  Exact duplicates are
+    collapsed to the lowest index of their group; the other copies get empty rows.  Raises ``scipy.spatial.QhullError`` for
+    fewer than three distinct points or all of them collinear."""
+    from scipy.spatial import QhullError
+
+    xy = _coords2d(coords)
+    if not np.isfinite(xy).all():
+        raise ValueError("Points cannot contain NaN")
+    n = xy.shape[0]
+    if n >= 2**31 - 1:
+        raise ValueError(f"Delaunay graphs take fewer than 2^31 - 1 points, found {n}.")
+    ctx = ctx or default_context()
+    indptr = np.empty(n + 1, dtype=np.int64)
+    idx = np.empty(max(6 * n, 1), dtype=np.int32)  # a planar graph has fewer than 3n edges
+    nnz, counts = C.c_int64(0), np.zeros(2, dtype=np.int64)
+    with ctx.lock:
+        try:
+            check(load().sqb_delaunay_2d(ctx.handle, xy.ctypes.data, n, indptr.ctypes.data, idx.ctypes.data, idx.size, C.byref(nnz), counts.ctypes.data))
+        except ValueError as e:
+            if str(e).startswith("QhullError"):
+                raise QhullError(str(e)) from None
+            raise
+    out = (indptr, idx[: nnz.value].copy())
+    return (*out, counts) if pass_counts else out
 
 
 def _device_coords(coords) -> DevArray | None:
@@ -356,6 +388,49 @@ class GridBuilder(_Builder):
         return adj, dst
 
 
+class DelaunayBuilder(_Builder):
+    """Delaunay graph (``neighbors.py:272-332``): the edges of the Delaunay triangulation, float32 ones and euclidean distances
+    in the coordinates' dtype.  ``radius`` only prunes: a scalar ``r`` keeps edges of length in ``(0.0, r)``, a tuple is sorted
+    and used as the interval, ``None`` keeps every edge."""
+
+    def __init__(self, radius=None, transform=None, set_diag: bool = False, percentile: float | None = None, ctx: Context | None = None):
+        if isinstance(radius, int | float):
+            radius = (0.0, float(radius))
+        super().__init__(transform, set_diag, percentile, ctx)
+        self.radius = list(radius) if isinstance(radius, tuple) else radius
+
+    def _interval(self):
+        return None if self.radius is None else tuple(sorted(self.radius))
+
+    def uns_params(self) -> dict[str, Any]:
+        return {"coord_type": CoordType.GENERIC.v, "radius": self.radius, "transform": self.transform.v}
+
+    def _device_args(self):
+        return 3, 0, 1, 0.0, self._interval()
+
+    def build_device(self, d: DevArray, device: int | None = None, libraries: tuple[np.ndarray, np.ndarray] | None = None):
+        from scipy.spatial import QhullError
+
+        try:
+            return super().build_device(d, device, libraries)
+        except ValueError as e:
+            if str(e).startswith("QhullError"):
+                raise QhullError(str(e)) from None
+            raise
+
+    def build_graph(self, coords):
+        coords = np.asarray(coords)
+        n = coords.shape[0]
+        indptr, idx = delaunay_2d(coords, ctx=self.ctx)
+        ip = indptr.astype(np.int32)
+        adj = csr_matrix((np.ones(idx.size, dtype=np.float32), idx, ip), shape=(n, n))
+        rows = np.repeat(np.arange(n), np.diff(indptr))
+        dst = csr_matrix((np.linalg.norm(coords[rows] - coords[idx], axis=1), idx.copy(), ip.copy()), shape=(n, n))
+        adj.has_sorted_indices = dst.has_sorted_indices = True
+        self._diagonals(adj, dst)
+        return adj, dst
+
+
 # ---------------------------------------------------------------------------------------------------------
 # public functions
 # ---------------------------------------------------------------------------------------------------------
@@ -453,3 +528,30 @@ def spatial_neighbors_grid(data: Any, *, spatial_key: str = Key.obsm.spatial, el
                           ctx=_host_context(adata, spatial_key, device))
     return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy,
                 device=device)
+
+
+def spatial_neighbors_delaunay(data: Any, *, spatial_key: str = Key.obsm.spatial, elements_to_coordinate_systems: dict[str, str] | None = None,
+                               table_key: str | None = None, library_key: str | None = None, radius: float | tuple[float, float] | None = None,
+                               percentile: float | None = None, transform=None, set_diag: bool = False, key_added: str = "spatial",
+                               copy: bool = False, n_jobs: int = 1, device: int | None = None) -> SpatialNeighborsResult | None:
+    """Delaunay graph from spatial coordinates (``_build.py:625-697``); ``n_jobs`` is accepted and ignored."""
+    adata = _prepare(data, spatial_key, table_key)
+    builder = DelaunayBuilder(radius=radius, percentile=percentile, transform=transform, set_diag=set_diag, ctx=_host_context(adata, spatial_key, device))
+    return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy, device=device)
+
+
+def spatial_neighbors_from_builder(data: Any, builder: _Builder, *, spatial_key: str = Key.obsm.spatial,
+                                   elements_to_coordinate_systems: dict[str, str] | None = None, table_key: str | None = None,
+                                   library_key: str | None = None, key_added: str = "spatial", copy: bool = False, n_jobs: int = 1,
+                                   device: int | None = None) -> SpatialNeighborsResult | None:
+    """Spatial graph from a builder the caller constructed (``_build.py:388-460``): any of ``KNNBuilder``, ``RadiusBuilder``,
+    ``GridBuilder`` and ``DelaunayBuilder``."""
+    if not isinstance(builder, _Builder):
+        raise TypeError(f"Expected a graph builder, found `{type(builder).__name__}`.")
+    adata = _prepare(data, spatial_key, table_key)
+    if builder.ctx is None and _device_coords(adata.obsm[spatial_key]) is None:
+        import copy as _copy
+
+        builder = _copy.copy(builder)  # the caller's builder keeps no context of this call
+        builder.ctx = default_context(device)
+    return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy, device=device)

@@ -227,6 +227,22 @@ __device__ __forceinline__ XT sqb_cvt(VT v) {
         return (XT)v;
 }
 
+// A product or sum rounded on its own (never contracted to an FMA), in float or double.
+template <typename T>
+__device__ __forceinline__ T mul_rn(T a, T b) {
+    if constexpr (std::is_same<T, float>::value)
+        return __fmul_rn(a, b);
+    else
+        return __dmul_rn(a, b);
+}
+template <typename T>
+__device__ __forceinline__ T add_rn(T a, T b) {
+    if constexpr (std::is_same<T, float>::value)
+        return __fadd_rn(a, b);
+    else
+        return __dadd_rn(a, b);
+}
+
 // The type a dispatch below hands to its callback: SqbType<T>::type.
 template <typename T>
 struct SqbType {

@@ -9,293 +9,26 @@
 //                            up to sc.tl.pca (:1336-1355) with _setdiag, _hop, _normalize and _aggregate (:1002-1054)
 //
 // Graph input (host or device CSR / CSC, int32 / int64 indices, float32 / float64 / int32 / int64 values) becomes a
-// device CSR in one of two orders: STORED (a CSR as given; a CSC transposed the way scipy's tocsr does it, rows by ascending
-// column then storage order) or CANONICAL (sorted columns, duplicates summed in the value type in storage order).  Values
-// are kept in float64 slots; a float32 graph's are float32 numbers and every operation on them rounds to float32.
+// device CSR in the STORED or CANONICAL form of caller_graph.cuh.  A float32 graph's values are float32 numbers and every
+// operation on them rounds to float32.
 //
 // Arithmetic is written as separate multiplies and adds (__fmul_rn / __fadd_rn, __dmul_rn / __dadd_rn): scipy's sparse
 // products do not contract to FMA, and the float32 results are bit-exact only in their order.
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "caller_graph.cuh"
 
 namespace {
 
-template <typename T>
-__device__ __forceinline__ T mul_rn(T a, T b) {
-    if constexpr (std::is_same<T, float>::value)
-        return __fmul_rn(a, b);
-    else
-        return __dmul_rn(a, b);
-}
-template <typename T>
-__device__ __forceinline__ T add_rn(T a, T b) {
-    if constexpr (std::is_same<T, float>::value)
-        return __fadd_rn(a, b);
-    else
-        return __dadd_rn(a, b);
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Graph loading
-// ---------------------------------------------------------------------------------------------------------------------
-struct Csr {
-    int64_t n = 0, e = 0;
-    DevBuf<uint32_t> ptr;
-    DevBuf<int32_t> col;
-    DevBuf<double> val;
-    explicit Csr(cudaStream_t s) : ptr(s), col(s), val(s) {}
-};
-
-// One warp per major index: row, column and value (as float64) of every stored entry.  Minor index outside [0, n): bit 2.
-template <typename IP, typename II, typename VT>
-__global__ void __launch_bounds__(256) niche_expand(const IP* __restrict__ ip, const II* __restrict__ ix, const VT* __restrict__ data,
-                                                    int64_t n, int csc, int32_t* __restrict__ row, int32_t* __restrict__ col,
-                                                    double* __restrict__ val, unsigned* __restrict__ err) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    unsigned bad = 0;
-    for (int64_t m = warp; m < n; m += nwarps) {
-        for (int64_t e = (int64_t)ip[m] + lane; e < (int64_t)ip[m + 1]; e += 32) {
-            const int64_t j = (int64_t)ix[e];
-            const bool ok = j >= 0 && j < n;
-            bad |= !ok;
-            const int32_t jj = ok ? (int32_t)j : 0;
-            row[e] = csc ? jj : (int32_t)m;
-            col[e] = csc ? (int32_t)m : jj;
-            val[e] = sqb_cvt<double>(data[e]);
-        }
-    }
-    if (bad) atomicOr(err, 2u);
-}
-
-// Sort keys: the row (STORED order of a CSC) or row << 32 | column (CANONICAL); payload the entry index.
-__global__ void __launch_bounds__(256) niche_keys(const int32_t* __restrict__ row, const int32_t* __restrict__ col, int64_t e, int canon,
-                                                  uint64_t* __restrict__ keys, uint32_t* __restrict__ ids) {
-    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < e; p += (int64_t)gridDim.x * blockDim.x) {
-        keys[p] = canon ? ((uint64_t)row[p] << 32) | (uint32_t)col[p] : (uint64_t)row[p];
-        ids[p] = (uint32_t)p;
-    }
-}
-
-// keep[p] = 1 at the head of every run of equal keys (every position when dedup == 0); the head's value becomes the run's
-// sum in the value type, added in storage order (the payload order of the stable sort).
-template <typename W>
-__global__ void __launch_bounds__(256) niche_runs(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ids,
-                                                  const double* __restrict__ val, int64_t e, int dedup, uint32_t* __restrict__ keep,
-                                                  double* __restrict__ run_val) {
-    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < e; p += (int64_t)gridDim.x * blockDim.x) {
-        const bool head = !dedup || p == 0 || keys[p - 1] != keys[p];
-        keep[p] = head;
-        if (!head) continue;
-        W s = (W)val[ids[p]];
-        if (dedup)
-            for (int64_t q = p + 1; q < e && keys[q] == keys[p]; ++q) s = add_rn<W>(s, (W)val[ids[q]]);
-        run_val[p] = (double)s;
-    }
-}
-
-__global__ void __launch_bounds__(256) niche_compact(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ rank,
-                                                     const uint32_t* __restrict__ ids, const int32_t* __restrict__ row,
-                                                     const int32_t* __restrict__ col, const double* __restrict__ run_val, int64_t e,
-                                                     int32_t* __restrict__ out_row, int32_t* __restrict__ out_col, double* __restrict__ out_val) {
-    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < e; p += (int64_t)gridDim.x * blockDim.x) {
-        if (!keep[p]) continue;
-        const uint32_t q = rank[p], id = ids[p];
-        out_row[q] = row[id];
-        out_col[q] = col[id];
-        out_val[q] = run_val[p];
-    }
-}
-
-// indptr of a CSR from the ascending rows of its e entries.
-__global__ void __launch_bounds__(256) niche_indptr(const int32_t* __restrict__ row, int64_t e, int64_t n, uint32_t* __restrict__ indptr) {
-    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p <= e; p += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t r = p < e ? row[p] : n;
-        const int64_t rp = p == 0 ? -1 : row[p - 1];
-        for (int64_t q = rp + 1; q <= r; ++q) indptr[q] = (uint32_t)p;
-    }
-}
-
-int exclusive_scan(sqb_ctx* c, const uint32_t* in, uint32_t* out, int64_t m, uint32_t* total) {
-    size_t bytes = 0;
-    SQB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, (int)m, c->stream));
-    DevBuf<uint8_t> tmp(c->stream);
-    SQB_TRY(tmp.alloc(bytes));
-    SQB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, in, out, (int)m, c->stream));
-    uint32_t tail[2] = {0, 0};
-    SQB_CUDA(cudaMemcpyAsync(&tail[0], out + m - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-    SQB_CUDA(cudaMemcpyAsync(&tail[1], in + m - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-    SQB_CUDA(cudaStreamSynchronize(c->stream));
-    *total = tail[0] + tail[1];
-    return SQB_OK;
-}
-
-// The caller's matrix (device pointers, already on the device) as a device CSR in STORED or CANONICAL order.
-template <typename IP, typename II, typename VT>
-int load_graph(sqb_ctx* c, int64_t n, int64_t nnz, const void* indptr, const void* indices, const void* data, int csc, bool canon,
-               bool w_f32, Csr& g, const char* where) {
-    const IP* ip = reinterpret_cast<const IP*>(indptr);
-    g.n = n;
-    SQB_TRY(g.ptr.alloc(n + 1));
-    SQB_TRY(sqb_check_indptr(c, SQB_K_MISC, ip, n, nnz, g.ptr.p, where));
-    if (nnz == 0) {
-        g.e = 0;
-        SQB_TRY(g.col.alloc(1));
-        SQB_TRY(g.val.alloc(1));
-        return SQB_OK;
-    }
-    DevBuf<int32_t> row(c->stream), col(c->stream);
-    DevBuf<double> val(c->stream);
-    DevBuf<unsigned> err(c->stream);
-    SQB_TRY(row.alloc(nnz));
-    SQB_TRY(col.alloc(nnz));
-    SQB_TRY(val.alloc(nnz));
-    SQB_TRY(err.alloc(1));
-    SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), c->stream));
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        niche_expand<IP, II, VT><<<sqb_grid_rows(c, n * 32, 256), 256, 0, c->stream>>>(
-            ip, reinterpret_cast<const II*>(indices), reinterpret_cast<const VT*>(data), n, csc, row.p, col.p, val.p, err.p);
-        SQB_POST_LAUNCH();
-    }
-    unsigned flag = 0;
-    SQB_CUDA(cudaMemcpyAsync(&flag, err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
-    SQB_CUDA(cudaStreamSynchronize(c->stream));
-    SQB_CHECK(!(flag & 2u), SQB_ERR_INVALID, "%s: index out of range [0, %lld)", where, (long long)n);
-    if (!csc && !canon) {  // a CSR in its stored order is used as given
-        g.e = nnz;
-        g.col = std::move(col);
-        g.val = std::move(val);
-        return SQB_OK;
-    }
-    DevBuf<uint64_t> keys(c->stream), keys_s(c->stream);
-    DevBuf<uint32_t> ids(c->stream), ids_s(c->stream), keep(c->stream), rank(c->stream);
-    DevBuf<double> run_val(c->stream);
-    SQB_TRY(keys.alloc(nnz));
-    SQB_TRY(keys_s.alloc(nnz));
-    SQB_TRY(ids.alloc(nnz));
-    SQB_TRY(ids_s.alloc(nnz));
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        niche_keys<<<sqb_grid_rows(c, nnz, 256), 256, 0, c->stream>>>(row.p, col.p, nnz, canon, keys.p, ids.p);
-        SQB_POST_LAUNCH();
-    }
-    int nbits = 1;
-    while (nbits < 31 && ((int64_t)1 << nbits) < n) ++nbits;
-    const int end_bit = canon ? 32 + nbits : nbits;
-    size_t bytes = 0;
-    SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys.p, keys_s.p, ids.p, ids_s.p, (int)nnz, 0, end_bit, c->stream));
-    DevBuf<uint8_t> tmp(c->stream);
-    SQB_TRY(tmp.alloc(bytes));
-    SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys.p, keys_s.p, ids.p, ids_s.p, (int)nnz, 0, end_bit, c->stream));
-    tmp.release();
-    keys.release();
-    ids.release();
-    SQB_TRY(keep.alloc(nnz));
-    SQB_TRY(rank.alloc(nnz));
-    SQB_TRY(run_val.alloc(nnz));
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        if (w_f32)
-            niche_runs<float><<<sqb_grid_rows(c, nnz, 256), 256, 0, c->stream>>>(keys_s.p, ids_s.p, val.p, nnz, canon, keep.p, run_val.p);
-        else
-            niche_runs<double><<<sqb_grid_rows(c, nnz, 256), 256, 0, c->stream>>>(keys_s.p, ids_s.p, val.p, nnz, canon, keep.p, run_val.p);
-        SQB_POST_LAUNCH();
-    }
-    uint32_t e = 0;
-    SQB_TRY(exclusive_scan(c, keep.p, rank.p, nnz, &e));
-    g.e = e;
-    DevBuf<int32_t> out_row(c->stream);
-    SQB_TRY(out_row.alloc(e));
-    SQB_TRY(g.col.alloc(e));
-    SQB_TRY(g.val.alloc(e));
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        niche_compact<<<sqb_grid_rows(c, nnz, 256), 256, 0, c->stream>>>(keep.p, rank.p, ids_s.p, row.p, col.p, run_val.p, nnz, out_row.p,
-                                                                          g.col.p, g.val.p);
-        SQB_POST_LAUNCH();
-    }
-    {
-        SqbLaunchScope scope(c, SQB_K_MISC);
-        niche_indptr<<<sqb_grid_rows(c, (int64_t)e + 1, 256), 256, 0, c->stream>>>(out_row.p, e, n, g.ptr.p);
-        SQB_POST_LAUNCH();
-    }
-    return SQB_OK;
-}
-
-// Value bytes of the graph dtype codes taken here (0 f32, 1 f64, 3 i32, 4 i64); 0 for the others.  Boolean graphs are
-// refused: scipy multiplies and adds them as logical and / or, which path sums do not reproduce.
-int graph_value_bytes(int code) {
-    switch (code) {
-        case 0: return 4;
-        case 1: return 8;
-        case 3: return 4;
-        case 4: return 8;
-    }
-    return 0;
-}
-
-struct GraphArgs {
-    int64_t n, nnz;
-    const void *indptr, *indices, *data;
-    int indptr_bits, index_bits, data_dtype, csc, device_input;
-    uintptr_t producer_stream;
-};
-
-int check_graph_args(const GraphArgs& a, const char* where) {
-    SQB_CHECK(a.n >= 1 && a.n < 0x7FFFFFFFLL, SQB_ERR_INVALID, "%s: n=%lld out of range [1, 2^31 - 1)", where, (long long)a.n);
-    SQB_CHECK(a.nnz >= 0 && a.nnz < (1LL << 31), SQB_ERR_INVALID, "%s: nnz=%lld out of range [0, 2^31)", where, (long long)a.nnz);
-    SQB_CHECK(a.indptr && ((a.indices && a.data) || a.nnz == 0), SQB_ERR_INVALID, "%s: null graph argument", where);
-    SQB_CHECK(a.nnz == 0 || graph_value_bytes(a.data_dtype), SQB_ERR_INVALID,
+// The graph checks of both entry points.  Boolean graphs are refused: scipy multiplies and adds them as logical and / or,
+// which path sums do not reproduce.
+int check_graph(const SqbGraphArgs& a, const char* where) {
+    SQB_TRY(sqb_check_graph_args(a, 31, where));
+    SQB_CHECK(a.nnz == 0 || (a.data_dtype != 5 && sqb_graph_value_bytes(a.data_dtype)), SQB_ERR_INVALID,
               "%s: data_dtype must be 0 (f32), 1 (f64), 3 (i32) or 4 (i64)", where);
-    SQB_CHECK((a.indptr_bits == 32 || a.indptr_bits == 64) && (a.index_bits == 32 || a.index_bits == 64), SQB_ERR_INVALID,
-              "%s: indptr_bits / index_bits must be 32 or 64", where);
     return SQB_OK;
-}
-
-// The caller's graph as a device CSR (host arrays are uploaded first; device arrays are read in place after the producer
-// stream).  Returns once the caller's arrays are no longer read.
-int graph_from_caller(sqb_ctx* c, const GraphArgs& a, bool canon, Csr& g, const char* where) {
-    const bool w_f32 = a.data_dtype == 0;
-    const auto run = [&](const void* ip, const void* ix, const void* dv) {
-        return sqb_dispatch_index(a.indptr_bits, a.index_bits, where, [&](auto tp, auto tx) {
-            using IP = typename decltype(tp)::type;
-            using II = typename decltype(tx)::type;
-            return sqb_dispatch_value(a.nnz == 0 ? 1 : a.data_dtype, where, "data_dtype", [&](auto tv) -> int {
-                using VT = typename decltype(tv)::type;
-                if constexpr (std::is_same<VT, __half>::value) {
-                    sqb_set_error("%s: float16 graph values are not supported", where);
-                    return SQB_ERR_INVALID;
-                } else {
-                    return load_graph<IP, II, VT>(c, a.n, a.nnz, ip, ix, dv, a.csc, canon, w_f32, g, where);
-                }
-            });
-        });
-    };
-    if (a.device_input)
-        return sqb_read_caller_buffers(c, a.producer_stream, [&]() -> int {
-            SQB_TRY(run(a.indptr, a.indices, a.data));
-            SQB_CUDA(cudaStreamSynchronize(c->stream));  // the caller's buffers are no longer read
-            return SQB_OK;
-        });
-    DevBuf<uint8_t> d_ip(c->stream), d_ix(c->stream), d_v(c->stream);
-    const size_t ip_bytes = (size_t)(a.n + 1) * (a.indptr_bits / 8), ix_bytes = (size_t)a.nnz * (a.index_bits / 8),
-                 v_bytes = (size_t)a.nnz * graph_value_bytes(a.data_dtype);
-    SQB_TRY(d_ip.alloc(ip_bytes));
-    SQB_TRY(d_ix.alloc(ix_bytes));
-    SQB_TRY(d_v.alloc(v_bytes));
-    SQB_TRY(sqb_h2d(c, d_ip.p, a.indptr, ip_bytes));
-    if (a.nnz > 0) {
-        SQB_TRY(sqb_h2d(c, d_ix.p, a.indices, ix_bytes));
-        SQB_TRY(sqb_h2d(c, d_v.p, a.data, v_bytes));
-    }
-    return run(d_ip.p, d_ix.p, d_v.p);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -621,7 +354,7 @@ __global__ void __launch_bounds__(kWarps * 32) niche_hop(const int32_t* __restri
 // a quarter of the free device memory, so the scratch never exceeds that whatever the graph.  hop_k's rows are sorted by
 // a segmented radix sort at the end.
 template <typename W>
-int next_hop(sqb_ctx* c, int64_t n, const uint32_t* h_ptr, const int32_t* h_col, const double* h_val, const Csr& a, const uint32_t* v_ptr,
+int next_hop(sqb_ctx* c, int64_t n, const uint32_t* h_ptr, const int32_t* h_col, const double* h_val, const SqbGraph& a, const uint32_t* v_ptr,
              const int32_t* v_col, const double* v_val, DevBuf<uint32_t>& o_hptr, DevBuf<int32_t>& o_hcol, DevBuf<uint32_t>& o_vptr,
              DevBuf<int32_t>& o_vcol, DevBuf<double>& o_vval) {
     DevBuf<int64_t> ub(c->stream);
@@ -709,8 +442,8 @@ int next_hop(sqb_ctx* c, int64_t n, const uint32_t* h_ptr, const int32_t* h_col,
     SQB_TRY(o_hptr.alloc(n + 1));
     SQB_TRY(o_vptr.alloc(n + 1));
     uint32_t nh = 0, nv = 0;
-    SQB_TRY(exclusive_scan(c, hcnt.p, o_hptr.p, n + 1, &nh));
-    SQB_TRY(exclusive_scan(c, vcnt.p, o_vptr.p, n + 1, &nv));
+    SQB_TRY(sqb_exclusive_scan(c, hcnt.p, o_hptr.p, n + 1, &nh));
+    SQB_TRY(sqb_exclusive_scan(c, vcnt.p, o_vptr.p, n + 1, &nv));
     DevBuf<int32_t> unsorted(c->stream);
     SQB_TRY(unsorted.alloc(nh));
     SQB_TRY(o_hcol.alloc(nh));
@@ -749,7 +482,7 @@ int spmm(sqb_ctx* c, const uint32_t* ptr, const int32_t* col, const double* val,
 
 // The aggregation of one graph over X (dense on the device): UTAG (mode 0) or the CellCharter blocks (modes 1 mean, 2 variance).
 template <typename W, typename TX, typename TO>
-int aggregate_run(sqb_ctx* c, Csr& g, const TX* X, int64_t m, int mode, int distance, TO* d_out, int64_t* out_hop_nnz) {
+int aggregate_run(sqb_ctx* c, SqbGraph& g, const TX* X, int64_t m, int mode, int distance, TO* d_out, int64_t* out_hop_nnz) {
     const int64_t n = g.n;
     // float32 accumulation only when both the graph's normalised values and X are float32 (scipy's upcast)
     using T1 = typename std::conditional<std::is_same<W, float>::value && std::is_same<TX, float>::value, float, double>::type;
@@ -784,8 +517,8 @@ int aggregate_run(sqb_ctx* c, Csr& g, const TX* X, int64_t m, int mode, int dist
     SQB_TRY(h_ptr.alloc(n + 1));
     SQB_TRY(v_ptr.alloc(n + 1));
     uint32_t nh = 0, nv = 0;
-    SQB_TRY(exclusive_scan(c, hcnt.p, h_ptr.p, n + 1, &nh));
-    SQB_TRY(exclusive_scan(c, vcnt.p, v_ptr.p, n + 1, &nv));
+    SQB_TRY(sqb_exclusive_scan(c, hcnt.p, h_ptr.p, n + 1, &nh));
+    SQB_TRY(sqb_exclusive_scan(c, vcnt.p, v_ptr.p, n + 1, &nv));
     SQB_TRY(h_col.alloc(nh));
     SQB_TRY(h_val.alloc(nh));
     SQB_TRY(v_col.alloc(nv));
@@ -852,40 +585,29 @@ int x_on_device(sqb_ctx* c, int64_t n, const XArgs& x, DevBuf<uint8_t>& dx, cons
     *out = X;
     if (x.format == 0) return sqb_h2d(c, X, x.x, (size_t)n * x.m * sizeof(TX));
     SQB_CUDA(cudaMemsetAsync(X, 0, (size_t)n * x.m * sizeof(TX), c->stream));
-    DevBuf<uint8_t> d_ip(c->stream), d_ix(c->stream), d_v(c->stream);
-    const void *ip = x.indptr, *ix = x.indices, *xv = x.x;
-    if (!x.device_input) {
-        const size_t ip_bytes = (size_t)(n + 1) * (x.indptr_bits / 8), ix_bytes = (size_t)x.nnz * (x.index_bits / 8),
-                     v_bytes = (size_t)x.nnz * sizeof(TX);
-        SQB_TRY(d_ip.alloc(ip_bytes));
-        SQB_TRY(d_ix.alloc(ix_bytes));
-        SQB_TRY(d_v.alloc(v_bytes));
-        SQB_TRY(sqb_h2d(c, d_ip.p, x.indptr, ip_bytes));
-        if (x.nnz) {
-            SQB_TRY(sqb_h2d(c, d_ix.p, x.indices, ix_bytes));
-            SQB_TRY(sqb_h2d(c, d_v.p, x.x, v_bytes));
-        }
-        ip = d_ip.p, ix = d_ix.p, xv = d_v.p;
-    }
-    return sqb_dispatch_index(x.indptr_bits, x.index_bits, where, [&](auto tp, auto tx) -> int {
-        using IP = typename decltype(tp)::type;
-        using II = typename decltype(tx)::type;
-        SQB_TRY(sqb_check_indptr(c, SQB_K_MISC, reinterpret_cast<const IP*>(ip), n, x.nnz, nullptr, where));
-        DevBuf<unsigned> err(c->stream);
-        SQB_TRY(err.alloc(1));
-        SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), c->stream));
-        {
-            SqbLaunchScope scope(c, SQB_K_MISC);
-            niche_densify<TX, IP, II><<<sqb_grid_rows(c, n, 256), 256, 0, c->stream>>>(
-                reinterpret_cast<const IP*>(ip), reinterpret_cast<const II*>(ix), reinterpret_cast<const TX*>(xv), n, x.m, X, err.p);
-            SQB_POST_LAUNCH();
-        }
-        unsigned flag = 0;
-        SQB_CUDA(cudaMemcpyAsync(&flag, err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
-        SQB_CUDA(cudaStreamSynchronize(c->stream));
-        SQB_CHECK(!flag, SQB_ERR_INVALID, "%s: X column index out of range [0, %lld)", where, (long long)x.m);
-        return SQB_OK;
-    });
+    const auto densify = [&](const void* ip, const void* ix, const void* xv) {
+        return sqb_dispatch_index(x.indptr_bits, x.index_bits, where, [&](auto tp, auto tx) -> int {
+            using IP = typename decltype(tp)::type;
+            using II = typename decltype(tx)::type;
+            SQB_TRY(sqb_check_indptr(c, SQB_K_MISC, reinterpret_cast<const IP*>(ip), n, x.nnz, nullptr, where));
+            DevBuf<unsigned> err(c->stream);
+            SQB_TRY(err.alloc(1));
+            SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), c->stream));
+            {
+                SqbLaunchScope scope(c, SQB_K_MISC);
+                niche_densify<TX, IP, II><<<sqb_grid_rows(c, n, 256), 256, 0, c->stream>>>(
+                    reinterpret_cast<const IP*>(ip), reinterpret_cast<const II*>(ix), reinterpret_cast<const TX*>(xv), n, x.m, X, err.p);
+                SQB_POST_LAUNCH();
+            }
+            unsigned flag = 0;
+            SQB_CUDA(cudaMemcpyAsync(&flag, err.p, sizeof(unsigned), cudaMemcpyDeviceToHost, c->stream));
+            SQB_CUDA(cudaStreamSynchronize(c->stream));
+            SQB_CHECK(!flag, SQB_ERR_INVALID, "%s: X column index out of range [0, %lld)", where, (long long)x.m);
+            return SQB_OK;
+        });
+    };
+    // a device X: sqb_niche_aggregate has waited for its producer stream already
+    return sqb_with_caller_csr(c, n, x.nnz, x.indptr, x.indptr_bits, x.indices, x.index_bits, x.x, sizeof(TX), x.device_input, 0, densify);
 }
 
 }  // namespace
@@ -896,8 +618,8 @@ extern "C" int sqb_niche_profile(sqb_ctx* c, int64_t n, int64_t nnz, const void*
                                  double* out) {
     static const char* where = "sqb_niche_profile";
     SQB_CHECK(c, SQB_ERR_INVALID, "%s: null ctx", where);
-    const GraphArgs ga{n, nnz, indptr, indices, data, indptr_bits, index_bits, data_dtype, csc, device_input, producer_stream};
-    SQB_TRY(check_graph_args(ga, where));
+    const SqbGraphArgs ga{n, nnz, indptr, indices, data, indptr_bits, index_bits, data_dtype, csc, device_input, producer_stream};
+    SQB_TRY(check_graph(ga, where));
     SQB_CHECK(codes && out, SQB_ERR_INVALID, "%s: null argument", where);
     SQB_CHECK(n_cls >= 1, SQB_ERR_INVALID, "%s: n_cls=%d must be at least 1", where, n_cls);
     SQB_CHECK(distance >= 1 && (distance == 1 || weights), SQB_ERR_INVALID, "%s: distance=%d must be >= 1 (with weights when > 1)", where,
@@ -906,8 +628,8 @@ extern "C" int sqb_niche_profile(sqb_ctx* c, int64_t n, int64_t nnz, const void*
         SQB_CHECK(codes[v] >= -1 && codes[v] < n_cls, SQB_ERR_INVALID, "%s: codes[%lld]=%d out of range [-1, %d)", where, (long long)v, codes[v],
                   n_cls);
     SQB_CUDA(cudaSetDevice(c->device));
-    Csr g(c->stream);
-    SQB_TRY(graph_from_caller(c, ga, true, g, where));
+    SqbGraph g(c->stream);
+    SQB_TRY(sqb_load_graph(c, ga, SqbGraphForm::CANONICAL, 0, g, where));
     const size_t cells = (size_t)n * n_cls;
     DevBuf<int32_t> d_codes(c->stream);
     DevBuf<double> P(c->stream), Q(c->stream), O(c->stream);
@@ -943,8 +665,8 @@ extern "C" int sqb_niche_aggregate(sqb_ctx* c, int64_t n, int64_t nnz, const voi
                                    int out_f32, void* out, int64_t* out_hop_nnz) {
     static const char* where = "sqb_niche_aggregate";
     SQB_CHECK(c, SQB_ERR_INVALID, "%s: null ctx", where);
-    const GraphArgs ga{n, nnz, indptr, indices, data, indptr_bits, index_bits, data_dtype, csc, device_input, producer_stream};
-    SQB_TRY(check_graph_args(ga, where));
+    const SqbGraphArgs ga{n, nnz, indptr, indices, data, indptr_bits, index_bits, data_dtype, csc, device_input, producer_stream};
+    SQB_TRY(check_graph(ga, where));
     SQB_CHECK(mode >= 0 && mode <= 2, SQB_ERR_INVALID, "%s: mode=%d must be 0 (utag), 1 (mean) or 2 (variance)", where, mode);
     SQB_CHECK(mode == 0 || (distance >= 1 && out_hop_nnz), SQB_ERR_INVALID, "%s: distance must be >= 1 with out_hop_nnz", where);
     SQB_CHECK(m >= 1 && out && (x || (x_format == 1 && x_nnz == 0)), SQB_ERR_INVALID, "%s: null argument or m < 1", where);
@@ -955,9 +677,9 @@ extern "C" int sqb_niche_aggregate(sqb_ctx* c, int64_t n, int64_t nnz, const voi
     SQB_CHECK(!out_f32 || (t1_f32 && (mode == 0 || distance == 1)), SQB_ERR_INVALID,
               "%s: a float32 output needs float32 graph values and X, and no hop beyond the first", where);
     SQB_CUDA(cudaSetDevice(c->device));
-    Csr g(c->stream);
+    SqbGraph g(c->stream);
     // UTAG reads the graph in storage order (normalize keeps it); CellCharter starts from its canonical form (tolil)
-    SQB_TRY(graph_from_caller(c, ga, mode != 0, g, where));
+    SQB_TRY(sqb_load_graph(c, ga, mode != 0 ? SqbGraphForm::CANONICAL : SqbGraphForm::STORED, 0, g, where));
     const XArgs xa{x, x_indptr, x_indices, x_nnz, m, x_format, x_indptr_bits, x_index_bits, x_f32, x_device, x_stream};
     const int64_t cols = mode == 0 ? m : (int64_t)(distance + 1) * m;
     const size_t out_bytes = (size_t)n * cols * (out_f32 ? 4 : 8);

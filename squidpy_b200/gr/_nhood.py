@@ -19,12 +19,13 @@ from typing import Any, NamedTuple
 import numpy as np
 
 from .._constants import Centrality, Key
-from .._device import DevGraph, DevSparse, array_device, device_graph, graph_args, graph_value_code
+from .._device import DevGraph, device_graph, graph_args, graph_value_code
 from .._dist import nccl_cuda, sequential_stats, shard_range, shared_seed, stats_device, world
-from .._lib import Context, check, default_context, load, pointer_device
+from .._lib import Context, check, default_context, load
 from .._rng import spawn_states
 from .._validators import assert_categorical_obs, assert_connectivity_key, assert_positive, extract_adata_if_sdata
-from ._utils import _save_data, as_csr, category_codes, logg
+from ._utils import _save_data, as_csr, caller_graph, category_codes, logg
+from ._utils import graph_device as _graph_device
 
 __all__ = ["nhood_enrichment", "NhoodEnrichmentResult", "NhoodPlan", "centrality_scores", "centrality_counts"]
 
@@ -197,14 +198,6 @@ class NhoodPlan:
             pass
 
 
-def _graph_device(d: DevSparse, device: int | None) -> int:
-    """The CUDA device holding a device graph; an explicit ``device`` must name it."""
-    on = array_device(d, pointer_device)
-    if device is not None and int(device) != on:
-        raise ValueError(f"`device={device}` does not match the device of the connectivity graph, cuda:{on}.")
-    return on
-
-
 def nhood_enrichment(
     adata: Any,
     cluster_key: str,
@@ -342,44 +335,32 @@ def centrality_counts(conn: Any, codes: np.ndarray, n_cls: int, measures: int, *
     in GPU memory (as ``nhood_enrichment`` takes it).  ``codes``: int32[n] cluster codes, -1 for none.  ``measures``: a
     mask of 1 (degree), 2 (closeness), 4 (clustering).  A CSC matrix is read as the CSR of its transpose, which is the
     same undirected graph."""
-    import scipy.sparse as sp
-
     codes = np.ascontiguousarray(codes, dtype=np.int32)
     n = codes.size
-    dev = device_graph(conn)
-    if dev is None:
-        g = conn if sp.issparse(conn) and conn.format in ("csr", "csc") else as_csr(conn)
-        if g.shape != (n, n):
-            raise ValueError(f"Expected the connectivity graph to be of shape `{(n, n)}`, found `{g.shape}`.")
-        spec = _HOST_VALUES.get(g.dtype)
+    g = caller_graph(conn, n, device)
+    if g.dev is None:
+        spec = _HOST_VALUES.get(g.host.dtype)
         if spec is None:
-            raise TypeError(f"Graph values of dtype `{g.dtype}` are not supported.")
+            raise TypeError(f"Graph values of dtype `{g.host.dtype}` are not supported.")
         dtype, code, int_bits = spec
-        indptr, indices = (np.ascontiguousarray(a) if a.dtype in (np.int32, np.int64) else np.ascontiguousarray(a, np.int64)
-                           for a in (g.indptr, g.indices))
-        data = g.data.view(np.int64) if g.dtype == np.uint64 else g.data
+        data = g.host.data.view(np.int64) if g.host.dtype == np.uint64 else g.host.data
         data = np.ascontiguousarray(data, dtype=dtype)
-        args = (n, indices.size, indptr.ctypes.data, 8 * indptr.itemsize, indices.ctypes.data, 8 * indices.itemsize, data.ctypes.data,
-                code, int_bits, 0)
-        stream = 0
+        data_ptr = data.ctypes.data
     else:
-        graph = graph_args(dev, n)
-        device = _graph_device(dev, device)
-        code = graph_value_code(dev.data, graph.nnz)
+        code = graph_value_code(g.dev.data, g.index_args[1])
         if code == 2:
             raise TypeError("Device graph values of dtype `float16` are not supported; use float32, float64, int32, int64 or bool.")
-        args = (n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None, graph.index_bits, dev.data.ptr or None, code,
-                32 if code == 3 else 64, 1)
-        stream = graph.stream
+        int_bits, data_ptr = 32 if code == 3 else 64, g.dev.data.ptr or None
+    args = (*g.index_args, data_ptr, code, int_bits, int(g.dev is not None))
     reach1 = np.zeros(n_cls, dtype=np.int64) if measures & 1 else None
     dist = np.zeros(n_cls, dtype=np.int64) if measures & 2 else None
     cc = np.empty(n, dtype=np.float64) if measures & 4 else None
     levels = C.c_int64(-1)
-    ctx = default_context(device)
+    ctx = default_context(g.device)
     with ctx.lock:
         check(load().sqb_centrality_scores(ctx.handle, *args, codes.ctypes.data, int(n_cls), int(measures),
                                            None if reach1 is None else reach1.ctypes.data, None if dist is None else dist.ctypes.data,
-                                           None if cc is None else cc.ctypes.data, C.byref(levels), stream))
+                                           None if cc is None else cc.ctypes.data, C.byref(levels), g.stream))
     return CentralityCounts(reach1, dist, cc, int(levels.value))
 
 

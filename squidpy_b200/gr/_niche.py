@@ -17,10 +17,10 @@ import numpy as np
 import pandas as pd
 
 from .._adata import AnnDataLite
-from .._device import DevArray, DevSparse, array_device, device_graph, device_matrix, graph_args, graph_value_code, matrix_args
+from .._device import DevArray, DevSparse, array_device, device_matrix, graph_value_code, matrix_args
 from .._lib import check, default_context, load, pointer_device
 from .._validators import assert_key_in_adata, extract_adata_if_sdata
-from ._utils import as_csr, logg
+from ._utils import caller_graph, logg
 
 __all__ = ["calculate_niche", "calculate_niche_neighborhood", "calculate_niche_utag", "calculate_niche_cellcharter", "niche_profile",
            "niche_aggregate"]
@@ -40,39 +40,27 @@ _BOOL_GRAPH = ("Boolean connectivity graphs are not supported: scipy combines th
 
 def _graph_abi(conn: Any, n: int, device: int | None) -> tuple[tuple, int | None, bool]:
     """``(graph arguments of sqb_niche_*, device, float32 values)`` of a host or device neighbour graph."""
-    import scipy.sparse as sp
-
-    dev = device_graph(conn)
-    if dev is None:
-        g = conn if sp.issparse(conn) and conn.format in ("csr", "csc") else as_csr(conn)
-        if g.shape != (n, n):
-            raise ValueError(f"Expected the connectivity graph to be of shape `{(n, n)}`, found `{g.shape}`.")
-        if g.dtype == np.float32 or g.dtype == np.float64:
-            data, code = np.ascontiguousarray(g.data), 0 if g.dtype == np.float32 else 1
-        elif g.dtype == np.bool_:
+    g = caller_graph(conn, n, device)
+    if g.dev is None:
+        if g.host.dtype == np.float32 or g.host.dtype == np.float64:
+            data, code = np.ascontiguousarray(g.host.data), 0 if g.host.dtype == np.float32 else 1
+        elif g.host.dtype == np.bool_:
             raise TypeError(_BOOL_GRAPH)
-        elif g.dtype.kind in "iu":
-            data, code = np.ascontiguousarray(g.data, dtype=np.int64), 4
+        elif g.host.dtype.kind in "iu":
+            data, code = np.ascontiguousarray(g.host.data, dtype=np.int64), 4
         else:
-            raise TypeError(f"Graph values of dtype `{g.dtype}` are not supported.")
-        indptr, indices = (np.ascontiguousarray(a) if a.dtype in (np.int32, np.int64) else np.ascontiguousarray(a, np.int64)
-                           for a in (g.indptr, g.indices))
-        keep = (indptr, indices, data)
-        args = (n, indices.size, indptr.ctypes.data, 8 * indptr.itemsize, indices.ctypes.data, 8 * indices.itemsize, data.ctypes.data, code,
-                int(g.format == "csc"), 0, 0)
-        return (args, keep), device, code == 0
-    graph = graph_args(dev, n)
-    on = array_device(dev, pointer_device)
-    if device is not None and int(device) != on:
-        raise ValueError(f"`device={device}` does not match the device of the connectivity graph, cuda:{on}.")
-    code = graph_value_code(dev.data, graph.nnz)
-    if code == 5:
-        raise TypeError(_BOOL_GRAPH)
-    if code == 2:
-        raise TypeError("Device graph values of dtype `float16` are not supported; use float32, float64, int32 or int64.")
-    args = (n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None, graph.index_bits, dev.data.ptr or None, code,
-            int(dev.format == "csc"), 1, graph.stream)
-    return (args, dev), on, code == 0
+            raise TypeError(f"Graph values of dtype `{g.host.dtype}` are not supported.")
+        data_ptr = data.ctypes.data
+    else:
+        code = graph_value_code(g.dev.data, g.index_args[1])
+        if code == 5:
+            raise TypeError(_BOOL_GRAPH)
+        if code == 2:
+            raise TypeError("Device graph values of dtype `float16` are not supported; use float32, float64, int32 or int64.")
+        data = g.dev.data
+        data_ptr = data.ptr or None
+    args = (*g.index_args, data_ptr, code, int(g.csc), int(g.dev is not None), g.stream)
+    return (args, (g, data)), g.device, code == 0
 
 
 def niche_profile(conn: Any, codes: np.ndarray, n_cls: int, distance: int = 1, weights: list[float] | None = None,

@@ -200,6 +200,12 @@ def test_boolean_device_graph_refused():
                                  torch.ones(A.nnz, dtype=torch.bool), size=A.shape, device="cuda")
     with pytest.raises(TypeError, match="Boolean connectivity graphs"):
         _niche.niche_profile(dA, np.zeros(A.shape[0], np.int32), 1, 2)
+    # a column index out of range, in the canonical (profile) and the stored (UTAG) order
+    bad = torch.sparse_csr_tensor(torch.tensor([0, 1, 1]), torch.tensor([5]), torch.tensor([1.0]), size=(2, 2)).cuda()
+    with pytest.raises(ValueError, match="out of range"):
+        _niche.niche_profile(bad, np.zeros(2, np.int32), 1)
+    with pytest.raises(ValueError, match="out of range"):
+        _niche.niche_aggregate(bad, np.ones((2, 3)), "utag")
 
 
 def test_cellcharter_knn15_long_rows():

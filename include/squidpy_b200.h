@@ -40,6 +40,8 @@
  *                                 src/squidpy/gr/_niche.py:1117-1169,1176-1214
  *   sqb_niche_aggregate        <- normalize(A, "l1") @ X of _UtagEmbedder (:1259-1260); _setdiag, _hop, _normalize, _aggregate
  *                                 and hstack(...).toarray() of _CellcharterEmbedder (:1002-1054,1336-1355)
+ *   sqb_mask_graph             <- _get_lines_coords + GeoDataFrame(LineString).within(polygon) + the masked assignments and
+ *                                 eliminate_zeros of mask_graph  src/squidpy/gr/_build.py:853-966
  */
 #ifndef SQUIDPY_B200_H
 #define SQUIDPY_B200_H
@@ -51,7 +53,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 15
+#define SQB_ABI_VERSION 16
 
 typedef enum {
     SQB_OK = 0,
@@ -507,6 +509,37 @@ int sqb_niche_aggregate(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr
                         const void* x_indptr, const void* x_indices, int64_t x_nnz, int x_format, int x_indptr_bits, int x_index_bits,
                         int x_f32, int64_t m, int x_device, uintptr_t x_stream, int mode, int distance, int out_f32, void* out,
                         int64_t* out_hop_nnz);
+
+/* ---- mask_graph ------------------------------------------------------------------------------------------------------
+ * Keeps or drops the stored entries of a spatial graph by a polygon (src/squidpy/gr/_build.py:853-966).  Entry (i, j) of the
+ * connectivities is the segment xy[i] -> xy[j]; it is within the polygon P when no point of it lies in P's exterior and some point
+ * of its open part in P's interior (shapely's LineString.within, DE-9IM T*F**F***); a zero-length segment is within iff its point
+ * is in P's interior.  Decided by exact orientation signs (mask_pred.h).  negative = 0 drops the entries that are not within,
+ * 1 those that are.  The distances lose the entries at the same (row, col) positions, and then both matrices every entry whose
+ * value is zero (scipy's eliminate_zeros; NaN is kept).  Values, their dtype and the order within each row are unchanged.
+ *   The graphs: n x n CSRs (indptr_bits / index_bits 32 or 64; data_dtype 0 f32, 1 f64, 3 i32, 4 i64, 5 bool), both on the host
+ *   (graph_device = 0) or both in device memory on the context's device (graph_device = 1, read in place after graph_stream, as
+ *   in sqb_autocorr_load_csr_device).  nnz < 2^31; an index outside [0, n) or a (row, col) stored twice is SQB_ERR_INVALID.
+ *   xy: n x 2 coordinates: host float64 C-contiguous (xy_device = 0, xy_dtype 1, strides 2 and 1), or a DEVICE pointer on the
+ *   context's device (xy_device = 1, read after xy_stream) of xy_dtype 0 f32 / 1 f64 with element strides stride_row /
+ *   stride_col.  Non-finite coordinates, or coordinates / polygon vertices neither 0 nor of magnitude in [2^-120, 2^120], are
+ *   SQB_ERR_INVALID.
+ *   The polygon: n_rings rings, ring r = the vertices ring_ptr[r] .. ring_ptr[r+1] of ring_xy (HOST, interleaved x, y), a hole of
+ *   the polygon before it when ring_hole[r] != 0, else the shell of a polygon; the polygons are the parts of a MultiPolygon.
+ *   Closing and repeated consecutive vertices are allowed; the polygon must be valid (shapely's is_valid), which is not checked.
+ * Returns a handle holding both masked CSRs and their entry counts.                                                         */
+typedef struct sqb_masked sqb_masked;
+int sqb_mask_graph(sqb_ctx* ctx, int64_t n, int64_t adj_nnz, const void* adj_indptr, int adj_indptr_bits, const void* adj_indices,
+                   int adj_index_bits, const void* adj_data, int adj_dtype, int64_t dst_nnz, const void* dst_indptr, int dst_indptr_bits,
+                   const void* dst_indices, int dst_index_bits, const void* dst_data, int dst_dtype, int graph_device, uintptr_t graph_stream,
+                   const void* xy, int xy_dtype, int64_t stride_row, int64_t stride_col, int xy_device, uintptr_t xy_stream, const double* ring_xy,
+                   const int64_t* ring_ptr, const uint8_t* ring_hole, int64_t n_rings, int negative, sqb_masked** out, int64_t* adj_nnz_out,
+                   int64_t* dst_nnz_out);
+/* Writes both masked CSRs (indptr n + 1 int32, indices int32, values in the input's dtype) into caller buffers in host or device
+ * memory.  consumer_stream: as in sqb_graph_export (0 for host buffers).  The buffers are complete when the call returns.     */
+int sqb_mask_export(sqb_masked* m, int32_t* adj_indptr, int32_t* adj_indices, void* adj_data, int32_t* dst_indptr, int32_t* dst_indices,
+                    void* dst_data, uintptr_t consumer_stream);
+int sqb_mask_free(sqb_masked* m);
 
 #ifdef __cplusplus
 }

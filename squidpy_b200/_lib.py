@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
 # phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -139,6 +139,12 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_niche_aggregate": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                       C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_int64, C.c_int, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "sqb_mask_graph": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int64,
+                                 C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_int, C.c_int64,
+                                 C.c_int64, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, c_void_pp,
+                                 C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "sqb_mask_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "sqb_mask_free": (C.c_int, [C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -3,6 +3,7 @@
 from ._build import (DelaunayBuilder, GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, delaunay_2d, knn_2d, radius_2d,
                      spatial_neighbors_delaunay, spatial_neighbors_from_builder, spatial_neighbors_grid, spatial_neighbors_knn,
                      spatial_neighbors_radius)
+from ._mask import mask_graph
 from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
 from ._niche import (calculate_niche, calculate_niche_cellcharter, calculate_niche_neighborhood, calculate_niche_spatialleiden,
                      calculate_niche_utag, niche_aggregate, niche_profile)
@@ -17,6 +18,7 @@ __all__ = [
     "spatial_neighbors_radius",
     "spatial_neighbors_delaunay",
     "spatial_neighbors_from_builder",
+    "mask_graph",
     "SpatialNeighborsResult",
     "DelaunayBuilder",
     "delaunay_2d",

@@ -53,7 +53,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 16
+#define SQB_ABI_VERSION 17
 
 typedef enum {
     SQB_OK = 0,
@@ -470,6 +470,40 @@ int sqb_graph_build_device(sqb_ctx* ctx, const void* xy, int xy_dtype, int64_t n
 int sqb_graph_export(sqb_graph* g, int32_t* adj_indptr, int32_t* adj_indices, float* adj_data, int32_t* dst_indptr,
                      int32_t* dst_indices, void* dst_data, uintptr_t consumer_stream);
 int sqb_graph_free(sqb_graph* g);
+
+/* ---- post-processing a caller's spatial graph in GPU memory, kept there --------------------------------------------------
+ * One post-processor of src/squidpy/gr/neighbors.py per call on a graph the caller built (a custom GraphBuilderCSR), with the
+ * steps sqb_graph_build_device uses.  The result equals the reference post-processor applied to host copies of the same
+ * matrices, after sort_indices(): the same stored entries, explicit zeros included, the same value dtypes and the same values
+ * bit for bit (spectral on a weighted adjacency: column sums in float64, rounded to float32).
+ *   The graph: n x n CSRs in DEVICE memory on the context's device, read in place after producer_stream (as in
+ *   sqb_autocorr_load_csr_device); indptr_bits / index_bits 32 or 64; nnz < 2^31; columns strictly increasing in every row
+ *   and inside [0, n) (else SQB_ERR_INVALID).  Connectivities float32; distances float64 if dst_f64, else float32.
+ *   op 0, DistanceIntervalPostprocessor((a, b)) (:441-447): adj.data[t] and dst.data[t] become 0 where dst.data[t] < a or
+ *     > b (by position: adj_nnz must equal dst_nnz), then every diagonal entry of adj is stored with its value from before,
+ *     0 where none was stored.  Float32 distances are compared with the bounds rounded to float32, as numpy does.
+ *   op 1, PercentilePostprocessor(a) (:450-458): threshold = np.percentile(dst.data, a) (method 'linear', in float32 for float32
+ *     distances); every adj position where dst stores a value > threshold becomes 0, stored explicitly where adj had no
+ *     entry; those distances become 0.  a in [0, 100]; an empty dst is SQB_ERR_INVALID and a threshold below 0 (scipy's
+ *     `dst > threshold` then marks every implicit entry) SQB_ERR_UNSUPPORTED.
+ *   op 2, TransformPostprocessor(transform) (:461-476): eliminate_zeros on both, then transform 0 none, 1 spectral, 2 cosine of
+ *     the connectivities (float32 results).
+ * Returns a sqb_graph handle (sqb_graph_export / sqb_graph_free) of n rows with the entry counts and the distances' dtype.
+ * Errors leave the context usable.                                                                                        */
+int sqb_graph_postprocess(sqb_ctx* ctx, int64_t n, int64_t adj_nnz, const void* adj_indptr, int adj_indptr_bits,
+                          const void* adj_indices, int adj_index_bits, const float* adj_data, int64_t dst_nnz,
+                          const void* dst_indptr, int dst_indptr_bits, const void* dst_indices, int dst_index_bits,
+                          const void* dst_data, int dst_f64, uintptr_t producer_stream, int op, double a, double b, int transform,
+                          sqb_graph** out, int64_t* adj_nnz_out, int64_t* dst_nnz_out, int* dst_f64_out);
+/* GraphBuilderCSR.combine (neighbors.py:137-154) of per-library device graphs: the block diagonal, its rows and columns put in
+ * the order of the observations.  Block b (block_n[b] >= 1 rows) is described by adj_blocks[6b .. 6b+6) and dst_blocks[6b ..
+ * 6b+6) (HOST int64): nnz, indptr pointer, indptr_bits, indices pointer, index_bits, data pointer, each a CSR as for
+ * sqb_graph_postprocess (float32 connectivities; distances float64 if dst_f64, else float32).  out_row (HOST int32, one per
+ * block row in block order) is the output row of every block row, a permutation of [0, total rows): the rank of its
+ * observation.  Explicit zeros are kept; columns come out ascending.  Returns a sqb_graph handle of *n_out rows.            */
+int sqb_graph_combine(sqb_ctx* ctx, int n_blocks, const int64_t* block_n, const int64_t* adj_blocks, const int64_t* dst_blocks,
+                      int dst_f64, uintptr_t producer_stream, const int32_t* out_row, sqb_graph** out, int64_t* n_out,
+                      int64_t* adj_nnz_out, int64_t* dst_nnz_out, int* dst_f64_out);
 
 /* ---- calculate_niche embeddings -----------------------------------------------------------------------------------
  * The graph (both entry points): an n x n CSR (csc = 0) or CSC (csc = 1) from the host (device_input = 0) or from device memory

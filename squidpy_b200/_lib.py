@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
 # phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -117,6 +117,11 @@ _SIGNATURES: dict[str, tuple] = {
                                          c_void_pp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
     "sqb_graph_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sqb_graph_free": (C.c_int, [C.c_void_p]),
+    "sqb_graph_postprocess": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_size_t, C.c_int, C.c_double, C.c_double, C.c_int,
+                                        c_void_pp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
+    "sqb_graph_combine": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_size_t, C.c_void_p, c_void_pp,
+                                    C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
     "sqb_cooc_counts": (
         C.c_int,
         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p],

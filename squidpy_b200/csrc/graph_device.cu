@@ -8,6 +8,10 @@
 //     _apply_percentile / _apply_transform                   :455-477                       eliminate_zeros, spectral / cosine)
 //   GraphBuilderCSR.combine                                  :138-156                       (library_key block diagonal)
 //   DelaunayBuilder.build_graph                              :318-332                       (Delaunay graph, delaunay.cu)
+// and, for a caller's graph already in device memory (sqb_graph_postprocess, sqb_graph_combine), the public post-processors
+//   DistanceIntervalPostprocessor / PercentilePostprocessor / TransformPostprocessor       :441-477
+//   GraphBuilderCSR.combine                                                              :138-156
+// one step per call, from the same steps as the builders' (DESIGN.md §3.4.1).
 // Every value equals the host path's bit for bit (squidpy_b200/gr/_build.py; DESIGN.md §3.4 has the argument per step):
 //  * entries are those of the host's CSR after eliminate_zeros: the host's explicit zeros (setdiag, pruning) only matter to
 //    the percentile, whose order statistics include them here too (the n diagonal zeros lead the sorted distances);
@@ -26,6 +30,9 @@
 
 #include <vector>
 
+#include <cub/device/device_segmented_sort.cuh>
+
+#include "caller_graph.cuh"
 #include "delaunay.cuh"
 
 enum { GD_KNN = 0, GD_GRID = 1, GD_RADIUS = 2, GD_DELAUNAY = 3 };
@@ -98,6 +105,16 @@ int sort_pairs(sqb_ctx* c, DevBuf<uint8_t>& tmp, const K* kin, K* kout, const V*
     SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, kin, kout, vin, vout, (int)m, 0, end_bit, c->stream));
     SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
     SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, kin, kout, vin, vout, (int)m, 0, end_bit, c->stream));
+    c->launches += 1;
+    return SQB_OK;
+}
+
+// ascending radix sort of m float64 values (cub orders the sign, so negative values sort first)
+int sort_keys(sqb_ctx* c, DevBuf<uint8_t>& tmp, const double* in, double* out, int64_t m) {
+    size_t bytes = 0;
+    SQB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, in, out, (int)m, 0, 64, c->stream));
+    SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
+    SQB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, bytes, in, out, (int)m, 0, 64, c->stream));
     c->launches += 1;
     return SQB_OK;
 }
@@ -193,11 +210,15 @@ __global__ void gd_knn_ptr_kernel(int64_t* __restrict__ ptr, int64_t n, int k) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x) ptr[i] = i * k;
 }
 
-// the distances the percentile sees besides the diagonal zeros: interval-pruned entries are zero
-__global__ void gd_masked_kernel(const double* __restrict__ d, int64_t m, int interval, double lo, double hi, double* __restrict__ out) {
+// the interval mask of _filter_by_radius_interval: `(dst.data < minn) | (dst.data > maxx)` (NaN is kept)
+__device__ __forceinline__ bool gd_outside(double v, double lo, double hi) { return v < lo || v > hi; }
+
+// the distances the percentile sees besides the diagonal zeros, as float64: interval-pruned entries are zero
+template <typename T>
+__global__ void gd_masked_kernel(const T* __restrict__ d, int64_t m, int interval, double lo, double hi, double* __restrict__ out) {
     for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) {
-        const double v = d[t];
-        out[t] = interval && (v < lo || v > hi) ? 0.0 : v;
+        const double v = (double)d[t];
+        out[t] = interval && gd_outside(v, lo, hi) ? 0.0 : v;
     }
 }
 
@@ -238,7 +259,7 @@ __global__ void gd_assemble_kernel(const int64_t* __restrict__ bptr, const int32
             if (p.cut_on && !(v < p.cut)) continue;  // GridBuilder: `dist < 1.3 * median` (neighbors.py:408-409)
             float a = 1.0f;
             double d = v;
-            if (p.interval && (v < p.lo || v > p.hi)) a = 0.0f, d = 0.0;
+            if (p.interval && gd_outside(v, p.lo, p.hi)) a = 0.0f, d = 0.0;
             if (d > p.thr) a = 0.0f, d = 0.0;
             emit(j, a, p.dst_mode == DST_DIST ? d : p.dst_mode == DST_ADJ ? (double)a : v);
         }
@@ -247,17 +268,18 @@ __global__ void gd_assemble_kernel(const int64_t* __restrict__ bptr, const int32
     }
 }
 
-__global__ void gd_colcount_kernel(const int32_t* __restrict__ idx, int64_t m, int32_t* __restrict__ cnt) {
-    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) atomicAdd(&cnt[idx[t]], 1);
+// column sums of the connectivities in float64: exact counts for a matrix of ones (below 2^53), weighted sums otherwise
+__global__ void gd_colsum_kernel(const int32_t* __restrict__ idx, const float* __restrict__ val, int64_t m, double* __restrict__ sum) {
+    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) atomicAdd(&sum[idx[t]], (double)val[t]);
 }
 
-// D^-1/2 A D^-1/2 of a matrix of ones: column sums are exact counts (below 2^24); every step rounded like numpy's float32
-__global__ void gd_spectral_kernel(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx, int64_t n, const int32_t* __restrict__ colcnt,
+// D^-1/2 A D^-1/2 with D the column sums rounded to float32; every step rounded like numpy's float32
+__global__ void gd_spectral_kernel(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx, int64_t n, const double* __restrict__ colsum,
                                    float* __restrict__ val) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float di = __fsqrt_rn(__fdiv_rn(1.0f, (float)colcnt[i]));
+        const float di = __fsqrt_rn(__fdiv_rn(1.0f, (float)colsum[i]));
         for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) {
-            const float dj = __fsqrt_rn(__fdiv_rn(1.0f, (float)colcnt[idx[t]]));
+            const float dj = __fsqrt_rn(__fdiv_rn(1.0f, (float)colsum[idx[t]]));
             val[t] = __fmul_rn(__fmul_rn(di, dj), val[t]);
         }
     }
@@ -405,6 +427,117 @@ __global__ void gd_block_fill_kernel(const int32_t* __restrict__ ptr, const int3
     }
 }
 
+// ---- a caller's graph (sqb_graph_postprocess, sqb_graph_combine) -------------------------------------------------------
+enum { GD_ERR_RANGE = 1, GD_ERR_ORDER = 2 };
+
+// The caller's columns as int32, one thread per row: an index outside [0, n) or a row whose columns do not strictly increase
+// raises its bit of *err.  The row pointers were checked by sqb_check_indptr.
+template <typename II>
+__global__ void gd_load_kernel(const uint32_t* __restrict__ ptr, const II* __restrict__ ix, int64_t n, int32_t* __restrict__ idx,
+                               unsigned* __restrict__ err) {
+    unsigned bad = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        int64_t prev = -1;
+        for (uint32_t t = ptr[i]; t < ptr[i + 1]; ++t) {
+            const int64_t j = (int64_t)ix[t];
+            if (j < 0 || j >= n) bad |= GD_ERR_RANGE;
+            else if (j <= prev) bad |= GD_ERR_ORDER;
+            idx[t] = (int32_t)j;
+            prev = j;
+        }
+    }
+    if (bad) atomicOr(err, bad);
+}
+
+// DistanceIntervalPostprocessor on the connectivities, one thread per row (count pass: oidx == nullptr).  adj.data[t] is zeroed
+// when dst.data[t] is outside the interval (the reference masks by position), then adj.setdiag(a_diag) stores every diagonal
+// entry with its value from before the mask, 0 where none was stored.
+template <typename T>
+__global__ void gd_interval_adj_kernel(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx, const float* __restrict__ val,
+                                       const T* __restrict__ dval, int64_t n, double lo, double hi, int32_t* __restrict__ cnt,
+                                       const int32_t* __restrict__ optr, int32_t* __restrict__ oidx, float* __restrict__ oval) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t o = oidx ? optr[i] : 0;
+        int32_t m = 0;
+        auto emit = [&](int32_t j, float v) {
+            if (oidx) oidx[o + m] = j, oval[o + m] = v;
+            ++m;
+        };
+        bool diag = false;
+        for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) {
+            const int32_t j = idx[t];
+            if (!diag && j >= i) {
+                diag = true;
+                if (j == i) {
+                    emit(j, val[t]);
+                    continue;
+                }
+                emit((int32_t)i, 0.0f);
+            }
+            emit(j, gd_outside((double)dval[t], lo, hi) ? 0.0f : val[t]);
+        }
+        if (!diag) emit((int32_t)i, 0.0f);
+        if (!oidx) cnt[i] = m;
+    }
+}
+
+// the distances of both post-processors in place: `dst.data[mask] = 0.0` (interval) and `dst[dst > threshold] = 0.0`
+template <typename T>
+__global__ void gd_dst_prune_kernel(T* __restrict__ v, int64_t m, int interval, double lo, double hi, double thr) {
+    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) {
+        const double x = (double)v[t];
+        if ((interval && gd_outside(x, lo, hi)) || x > thr) v[t] = (T)0;
+    }
+}
+
+// `adj[dst > threshold] = 0.0`, one thread per row (count pass: oidx == nullptr): the row's columns merged with the columns of
+// dst's row whose value exceeds the threshold; those positions are 0, stored explicitly where adj had no entry.
+template <typename T>
+__global__ void gd_pct_merge_kernel(const int32_t* __restrict__ aptr, const int32_t* __restrict__ aidx, const float* __restrict__ aval,
+                                    const int32_t* __restrict__ dptr, const int32_t* __restrict__ didx, const T* __restrict__ dval, int64_t n,
+                                    double thr, int32_t* __restrict__ cnt, const int32_t* __restrict__ optr, int32_t* __restrict__ oidx,
+                                    float* __restrict__ oval) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t o = oidx ? optr[i] : 0;
+        int32_t m = 0, p = aptr[i], q = dptr[i];
+        const int32_t pe = aptr[i + 1], qe = dptr[i + 1];
+        for (;;) {
+            while (q < qe && !((double)dval[q] > thr)) ++q;
+            const bool hp = p < pe, hq = q < qe;
+            if (!hp && !hq) break;
+            int32_t j;
+            float v;
+            if (hq && (!hp || didx[q] < aidx[p])) {
+                j = didx[q++], v = 0.0f;
+            } else {
+                j = aidx[p];
+                const bool hit = hq && didx[q] == j;
+                v = hit ? 0.0f : aval[p];
+                ++p, q += hit;
+            }
+            if (oidx) oidx[o + m] = j, oval[o + m] = v;
+            ++m;
+        }
+        if (!oidx) cnt[i] = m;
+    }
+}
+
+// eliminate_zeros, one thread per row (count pass: oidx == nullptr); NaN is kept
+template <typename T>
+__global__ void gd_nonzero_kernel(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx, const T* __restrict__ val, int64_t n,
+                                  int32_t* __restrict__ cnt, const int32_t* __restrict__ optr, int32_t* __restrict__ oidx, T* __restrict__ oval) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t o = oidx ? optr[i] : 0;
+        int32_t m = 0;
+        for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) {
+            if (val[t] == (T)0) continue;
+            if (oidx) oidx[o + m] = idx[t], oval[o + m] = val[t];
+            ++m;
+        }
+        if (!oidx) cnt[i] = m;
+    }
+}
+
 // ---- host steps --------------------------------------------------------------------------------------------------------
 struct sqb_graph {
     explicit sqb_graph(sqb_ctx* ctx) : c(ctx), adj(ctx->stream), dst(ctx->stream) {}
@@ -441,6 +574,17 @@ int assemble(sqb_ctx* c, const int64_t* bptr, const int32_t* bidx, const double*
     GD_LAUNCH(gd_assemble_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(bptr, bidx, bval, n, p, nullptr, nullptr, adj->ptr.p, adj->idx.p, adj->vf.p,
                                                                            dst->ptr.p, dst->idx.p, dst_f64 ? nullptr : dst->vf.p,
                                                                            dst_f64 ? dst->vd.p : nullptr));
+    return SQB_OK;
+}
+
+// D^-1/2 A D^-1/2 of the connectivities in place (symmetric_normalize_csr); an empty matrix is returned as it is
+int spectral(sqb_ctx* c, int64_t n, Csr* adj) {
+    if (adj->nnz == 0) return SQB_OK;
+    DevBuf<double> colsum(c->stream);
+    SQB_TRY(colsum.alloc(n));
+    SQB_CUDA(cudaMemsetAsync(colsum.p, 0, n * sizeof(double), c->stream));
+    GD_LAUNCH(gd_colsum_kernel<<<blocks_for(c, adj->nnz), 256, 0, c->stream>>>(adj->idx.p, adj->vf.p, adj->nnz, colsum.p));
+    GD_LAUNCH(gd_spectral_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, colsum.p, adj->vf.p));
     return SQB_OK;
 }
 
@@ -673,12 +817,8 @@ int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64
         SQB_TRY(bval.alloc(m));
         SQB_TRY(sorted.alloc(m));
         if (m > 0) {
-            GD_LAUNCH(gd_masked_kernel<<<blocks_for(c, m), 256, 0, c->stream>>>(dist.p, m, P.interval, ap.lo, ap.hi, bval.p));
-            size_t bytes = 0;
-            SQB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
-            SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
-            SQB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, bytes, bval.p, sorted.p, (int)m, 0, 64, c->stream));
-            c->launches += 1;
+            GD_LAUNCH(gd_masked_kernel<double><<<blocks_for(c, m), 256, 0, c->stream>>>(dist.p, m, P.interval, ap.lo, ap.hi, bval.p));
+            SQB_TRY(sort_keys(c, tmp, bval.p, sorted.p, m));
         }
         PctEnv env{c, sorted.p, n};
         SQB_TRY((f32 ? percentile_linear_f32 : percentile_linear)(P.percentile, m + n, &ap.thr, pct_get, &env));
@@ -689,12 +829,8 @@ int build_untransformed(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64
 // One graph (or one library's block) with its transform
 int build_block(sqb_ctx* c, const Coords& xy, const int32_t* rows, int64_t n, const Params& P, Csr* adj, Csr* dst) {
     SQB_TRY(build_untransformed(c, xy, rows, n, P, adj, dst));
-    if (P.transform == GD_SPECTRAL && adj->nnz > 0) {
-        DevBuf<int32_t> colcnt(c->stream);
-        SQB_TRY(colcnt.alloc(n));
-        SQB_CUDA(cudaMemsetAsync(colcnt.p, 0, n * sizeof(int32_t), c->stream));
-        GD_LAUNCH(gd_colcount_kernel<<<blocks_for(c, adj->nnz), 256, 0, c->stream>>>(adj->idx.p, adj->nnz, colcnt.p));
-        GD_LAUNCH(gd_spectral_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, colcnt.p, adj->vf.p));
+    if (P.transform == GD_SPECTRAL) {
+        SQB_TRY(spectral(c, n, adj));
     } else if (P.transform == GD_COSINE) {
         SQB_TRY(cosine(c, n, adj));
     }
@@ -728,6 +864,159 @@ int combine(sqb_ctx* c, int64_t n_out, const std::vector<Csr>& blocks, const std
             GD_LAUNCH(gd_block_fill_kernel<float><<<blocks_for(c, nb[b]), 256, 0, c->stream>>>(k.ptr.p, k.idx.p, k.vf.p, grow[b].p, nb[b], out->ptr.p,
                                                                                               out->idx.p, out->vf.p));
     }
+    return SQB_OK;
+}
+
+// f(values) with the distances' values as float* or double*
+template <typename F>
+int with_dst(const Csr& d, F&& f) {
+    return d.f64 ? f(d.vd.p) : f(d.vf.p);
+}
+
+// *g rewritten row by row: pass(cnt, optr, oidx, oval) launches a kernel that counts the entries of every row (oidx null) or
+// writes them at optr; the result replaces g's pointers, indices and values (member vals).
+template <typename V, typename F>
+int rewrite_rows(sqb_ctx* c, int64_t n, Csr* g, DevBuf<V> Csr::*vals, F&& pass) {
+    DevBuf<int32_t> cnt(c->stream), ptr(c->stream), idx(c->stream);
+    DevBuf<V> val(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(cnt.alloc(n + 1));
+    SQB_TRY(ptr.alloc(n + 1));
+    SQB_CUDA(cudaMemsetAsync(cnt.p + n, 0, sizeof(int32_t), c->stream));
+    GD_LAUNCH(pass(cnt.p, (const int32_t*)nullptr, (int32_t*)nullptr, (V*)nullptr));
+    SQB_TRY(exclusive_scan(c, tmp, cnt.p, ptr.p, n + 1));
+    int32_t m = 0;
+    SQB_TRY(read_back(c, &m, ptr.p + n, sizeof(int32_t)));
+    SQB_TRY(idx.alloc(m));
+    SQB_TRY(val.alloc(m));
+    GD_LAUNCH(pass((int32_t*)nullptr, (const int32_t*)ptr.p, idx.p, val.p));
+    g->ptr = std::move(ptr), g->idx = std::move(idx), g->*vals = std::move(val), g->nnz = m;
+    return SQB_OK;
+}
+
+// A caller's device CSR (checked by sqb_check_graph_args; data_dtype 0 float32 / 1 float64) as a Csr: columns strictly
+// increasing in every row and inside [0, n), or SQB_ERR_INVALID.
+int load_caller(sqb_ctx* c, const SqbGraphArgs& a, Csr* g, const char* where) {
+    SQB_TRY(sqb_check_graph_args(a, 31, where));
+    const int64_t n = a.n, nnz = a.nnz;
+    const size_t vbytes = a.data_dtype == 1 ? sizeof(double) : sizeof(float);
+    g->nnz = nnz, g->f64 = a.data_dtype == 1;
+    SQB_TRY(g->ptr.alloc(n + 1));
+    SQB_TRY(g->idx.alloc(nnz));
+    SQB_TRY(g->f64 ? g->vd.alloc(nnz) : g->vf.alloc(nnz));
+    DevBuf<unsigned> err(c->stream);
+    SQB_TRY(err.alloc(1));
+    SQB_CUDA(cudaMemsetAsync(err.p, 0, sizeof(unsigned), c->stream));
+    SQB_TRY(sqb_with_caller_csr(c, n, nnz, a.indptr, a.indptr_bits, a.indices, a.index_bits, a.data, vbytes, a.device_input, a.producer_stream,
+                                [&](const void* ip, const void* ix, const void* dv) {
+                                    return sqb_dispatch_index(a.indptr_bits, a.index_bits, where, [&](auto tp, auto tx) -> int {
+                                        using IP = typename decltype(tp)::type;
+                                        using II = typename decltype(tx)::type;
+                                        uint32_t* ptr = reinterpret_cast<uint32_t*>(g->ptr.p);  // nnz < 2^31
+                                        SQB_TRY(sqb_check_indptr(c, SQB_K_MISC, reinterpret_cast<const IP*>(ip), n, nnz, ptr, where));
+                                        if (nnz == 0) return SQB_OK;
+                                        GD_LAUNCH(gd_load_kernel<II><<<blocks_for(c, n), 256, 0, c->stream>>>(ptr, reinterpret_cast<const II*>(ix), n,
+                                                                                                            g->idx.p, err.p));
+                                        void* vals = g->f64 ? (void*)g->vd.p : (void*)g->vf.p;
+                                        SQB_CUDA(cudaMemcpyAsync(vals, dv, nnz * vbytes, cudaMemcpyDeviceToDevice, c->stream));
+                                        return SQB_OK;
+                                    });
+                                }));
+    unsigned flags = 0;
+    SQB_TRY(read_back(c, &flags, err.p, sizeof(unsigned)));
+    SQB_CHECK(!(flags & GD_ERR_RANGE), SQB_ERR_INVALID, "%s: index out of range [0, %lld)", where, (long long)n);
+    SQB_CHECK(!(flags & GD_ERR_ORDER), SQB_ERR_INVALID,
+              "%s: the columns of every row must be strictly increasing; call sum_duplicates() and sort_indices() first", where);
+    return SQB_OK;
+}
+
+// scipy's eliminate_zeros
+int eliminate_zeros(sqb_ctx* c, int64_t n, Csr* g) {
+    const auto run = [&](auto* v, auto member) -> int {
+        using V = std::remove_pointer_t<decltype(v)>;
+        return rewrite_rows<V>(c, n, g, member, [&](int32_t* cnt, const int32_t* optr, int32_t* oidx, V* oval) {
+            gd_nonzero_kernel<V><<<blocks_for(c, n), 256, 0, c->stream>>>(g->ptr.p, g->idx.p, v, n, cnt, optr, oidx, oval);
+        });
+    };
+    return g->f64 ? run(g->vd.p, &Csr::vd) : run(g->vf.p, &Csr::vf);
+}
+
+// DistanceIntervalPostprocessor (_filter_by_radius_interval): adj and dst hold equally many entries, masked by position
+int interval_step(sqb_ctx* c, int64_t n, double lo, double hi, Csr* adj, Csr* dst) {
+    SQB_CHECK(adj->nnz == dst->nnz, SQB_ERR_INVALID, "boolean index did not match indexed array along axis 0; size of axis is %lld but size of "
+              "corresponding boolean axis is %lld", (long long)adj->nnz, (long long)dst->nnz);
+    SQB_CHECK(adj->nnz + n < INT_MAX, SQB_ERR_UNSUPPORTED, "the graph has %lld entries; int32 indices hold at most 2^31 - 1", (long long)(adj->nnz + n));
+    if (!dst->f64) lo = (double)(float)lo, hi = (double)(float)hi;  // numpy compares float32 values with the Python bounds in float32
+    return with_dst(*dst, [&](auto* dv) -> int {
+        using T = std::remove_pointer_t<decltype(dv)>;
+        SQB_TRY(rewrite_rows<float>(c, n, adj, &Csr::vf, [&](int32_t* cnt, const int32_t* optr, int32_t* oidx, float* oval) {
+            gd_interval_adj_kernel<T><<<blocks_for(c, n), 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, adj->vf.p, dv, n, lo, hi, cnt, optr, oidx, oval);
+        }));
+        if (dst->nnz > 0) GD_LAUNCH(gd_dst_prune_kernel<T><<<blocks_for(c, dst->nnz), 256, 0, c->stream>>>(dv, dst->nnz, 1, lo, hi, INFINITY));
+        return SQB_OK;
+    });
+}
+
+// PercentilePostprocessor: the threshold np.percentile(dst.data, q) over every stored distance (explicit zeros included)
+int percentile_step(sqb_ctx* c, int64_t n, double q, Csr* adj, Csr* dst) {
+    const int64_t m = dst->nnz;
+    SQB_CHECK(m > 0, SQB_ERR_INVALID, "index -1 is out of bounds for axis 0 with size 0");
+    SQB_CHECK(adj->nnz + m < INT_MAX, SQB_ERR_UNSUPPORTED, "the graph has %lld entries; int32 indices hold at most 2^31 - 1", (long long)(adj->nnz + m));
+    DevBuf<double> vals(c->stream), sorted(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(vals.alloc(m));
+    SQB_TRY(sorted.alloc(m));
+    SQB_TRY(with_dst(*dst, [&](auto* dv) -> int {
+        using T = std::remove_pointer_t<decltype(dv)>;
+        GD_LAUNCH(gd_masked_kernel<T><<<blocks_for(c, m), 256, 0, c->stream>>>(dv, m, 0, 0.0, 0.0, vals.p));
+        return SQB_OK;
+    }));
+    SQB_TRY(sort_keys(c, tmp, vals.p, sorted.p, m));
+    PctEnv env{c, sorted.p, 0};
+    double thr = 0.0;
+    SQB_TRY((dst->f64 ? percentile_linear : percentile_linear_f32)(q, m, &thr, pct_get, &env));
+    SQB_CHECK(thr >= 0.0, SQB_ERR_UNSUPPORTED,
+              "the percentile threshold %g is not >= 0: `dst > threshold` would mark every entry the distances do not store", thr);
+    return with_dst(*dst, [&](auto* dv) -> int {
+        using T = std::remove_pointer_t<decltype(dv)>;
+        SQB_TRY(rewrite_rows<float>(c, n, adj, &Csr::vf, [&](int32_t* cnt, const int32_t* optr, int32_t* oidx, float* oval) {
+            gd_pct_merge_kernel<T><<<blocks_for(c, n), 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, adj->vf.p, dst->ptr.p, dst->idx.p, dv, n, thr, cnt,
+                                                                             optr, oidx, oval);
+        }));
+        GD_LAUNCH(gd_dst_prune_kernel<T><<<blocks_for(c, m), 256, 0, c->stream>>>(dv, m, 0, 0.0, 0.0, thr));
+        return SQB_OK;
+    });
+}
+
+// TransformPostprocessor: eliminate_zeros on both, then the transform of the connectivities
+int transform_step(sqb_ctx* c, int64_t n, int transform, Csr* adj, Csr* dst) {
+    SQB_TRY(eliminate_zeros(c, n, adj));
+    SQB_TRY(eliminate_zeros(c, n, dst));
+    if (transform == GD_SPECTRAL) return spectral(c, n, adj);
+    if (transform == GD_COSINE) return cosine(c, n, adj);
+    return SQB_OK;
+}
+
+// every row's columns in ascending order (with their values)
+int sort_rows(sqb_ctx* c, int64_t n, Csr* g) {
+    if (g->nnz == 0) return SQB_OK;
+    DevBuf<int32_t> idx(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(idx.alloc(g->nnz));
+    const auto run = [&](auto* v, auto member) -> int {
+        using V = std::remove_pointer_t<decltype(v)>;
+        DevBuf<V> val(c->stream);
+        SQB_TRY(val.alloc(g->nnz));
+        size_t bytes = 0;
+        SQB_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, bytes, g->idx.p, idx.p, v, val.p, (int)g->nnz, (int)n, g->ptr.p, g->ptr.p + 1, c->stream));
+        SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
+        SQB_CUDA(cub::DeviceSegmentedSort::SortPairs(tmp.p, bytes, g->idx.p, idx.p, v, val.p, (int)g->nnz, (int)n, g->ptr.p, g->ptr.p + 1, c->stream));
+        c->launches += 1;
+        g->*member = std::move(val);
+        return SQB_OK;
+    };
+    SQB_TRY(g->f64 ? run(g->vd.p, &Csr::vd) : run(g->vf.p, &Csr::vf));
+    g->idx = std::move(idx);
     return SQB_OK;
 }
 
@@ -800,6 +1089,89 @@ int sqb_graph_build_device(sqb_ctx* c, const void* xy, int xy_dtype, int64_t n, 
     }
     SQB_CUDA(cudaStreamSynchronize(c->stream));  // surfaces an asynchronous fault of the build here
     *n_out = g->n, *adj_nnz = g->adj.nnz, *dst_nnz = g->dst.nnz, *dst_f64 = g->dst.f64 ? 1 : 0;
+    *out = g.release();
+    return SQB_OK;
+}
+
+int sqb_graph_postprocess(sqb_ctx* c, int64_t n, int64_t adj_nnz, const void* adj_indptr, int adj_indptr_bits, const void* adj_indices,
+                          int adj_index_bits, const float* adj_data, int64_t dst_nnz, const void* dst_indptr, int dst_indptr_bits,
+                          const void* dst_indices, int dst_index_bits, const void* dst_data, int dst_f64, uintptr_t producer_stream, int op,
+                          double a, double b, int transform, sqb_graph** out, int64_t* adj_nnz_out, int64_t* dst_nnz_out, int* dst_f64_out) {
+    static const char* where = "sqb_graph_postprocess";
+    SQB_CHECK(c && out && adj_nnz_out && dst_nnz_out && dst_f64_out, SQB_ERR_INVALID, "%s: null argument", where);
+    *out = nullptr;
+    SQB_CHECK(op >= 0 && op <= 2, SQB_ERR_INVALID, "%s: op must be 0 (interval), 1 (percentile) or 2 (transform)", where);
+    SQB_CHECK(op != 2 || (transform >= GD_NONE && transform <= GD_COSINE), SQB_ERR_INVALID,
+              "%s: transform must be 0 (none), 1 (spectral) or 2 (cosine)", where);
+    SQB_CHECK(op != 1 || (a >= 0.0 && a <= 100.0), SQB_ERR_INVALID, "Percentiles must be in the range [0, 100]");
+    SQB_CUDA(cudaSetDevice(c->device));
+    std::unique_ptr<sqb_graph> g(new sqb_graph(c));
+    g->n = n;
+    const SqbGraphArgs aa{n, adj_nnz, adj_indptr, adj_indices, adj_data, adj_indptr_bits, adj_index_bits, 0, 0, 1, producer_stream};
+    const SqbGraphArgs da{n, dst_nnz, dst_indptr, dst_indices, dst_data, dst_indptr_bits, dst_index_bits, dst_f64 ? 1 : 0, 0, 1, producer_stream};
+    SQB_TRY(load_caller(c, aa, &g->adj, "sqb_graph_postprocess (connectivities)"));
+    SQB_TRY(load_caller(c, da, &g->dst, "sqb_graph_postprocess (distances)"));
+    if (op == 0)
+        SQB_TRY(interval_step(c, n, a, b, &g->adj, &g->dst));
+    else if (op == 1)
+        SQB_TRY(percentile_step(c, n, a, &g->adj, &g->dst));
+    else
+        SQB_TRY(transform_step(c, n, transform, &g->adj, &g->dst));
+    SQB_CUDA(cudaStreamSynchronize(c->stream));  // surfaces an asynchronous fault here
+    *adj_nnz_out = g->adj.nnz, *dst_nnz_out = g->dst.nnz, *dst_f64_out = g->dst.f64 ? 1 : 0;
+    *out = g.release();
+    return SQB_OK;
+}
+
+int sqb_graph_combine(sqb_ctx* c, int n_blocks, const int64_t* block_n, const int64_t* adj_blocks, const int64_t* dst_blocks, int dst_f64,
+                      uintptr_t producer_stream, const int32_t* out_row, sqb_graph** out, int64_t* n_out, int64_t* adj_nnz_out, int64_t* dst_nnz_out,
+                      int* dst_f64_out) {
+    static const char* where = "sqb_graph_combine";
+    SQB_CHECK(c && block_n && adj_blocks && dst_blocks && out_row && out && n_out && adj_nnz_out && dst_nnz_out && dst_f64_out, SQB_ERR_INVALID,
+              "%s: null argument", where);
+    *out = nullptr;
+    SQB_CHECK(n_blocks >= 1, SQB_ERR_INVALID, "%s: n_blocks must be positive", where);
+    int64_t total = 0;
+    for (int b = 0; b < n_blocks; ++b) {
+        SQB_CHECK(block_n[b] >= 1 && block_n[b] < 0x7FFFFFFFLL - total, SQB_ERR_INVALID, "%s: block %d has %lld rows", where, b, (long long)block_n[b]);
+        total += block_n[b];
+    }
+    // out_row: a permutation of [0, total); the columns of a block keep their order when its rows map in ascending order
+    std::vector<uint8_t> seen((size_t)total, 0);
+    bool ascending = true;
+    for (int b = 0, r0 = 0; b < n_blocks; r0 += (int)block_n[b], ++b)
+        for (int64_t r = 0; r < block_n[b]; ++r) {
+            const int32_t o = out_row[r0 + r];
+            SQB_CHECK(o >= 0 && o < total && !seen[o], SQB_ERR_INVALID, "%s: out_row must be a permutation of [0, %lld)", where, (long long)total);
+            seen[o] = 1;
+            ascending = ascending && (r == 0 || o > out_row[r0 + r - 1]);
+        }
+    SQB_CUDA(cudaSetDevice(c->device));
+    std::unique_ptr<sqb_graph> g(new sqb_graph(c));
+    g->n = total;
+    std::vector<Csr> ba, bd;
+    std::vector<DevBuf<int32_t>> grow;
+    std::vector<int64_t> nb(block_n, block_n + n_blocks);
+    for (int b = 0, r0 = 0; b < n_blocks; r0 += (int)block_n[b], ++b) {
+        ba.emplace_back(c->stream), bd.emplace_back(c->stream), grow.emplace_back(c->stream);
+        const int64_t* A = adj_blocks + 6 * b;  // nnz, indptr, indptr_bits, indices, index_bits, data
+        const int64_t* D = dst_blocks + 6 * b;
+        const SqbGraphArgs aa{nb[b], A[0], (const void*)A[1], (const void*)A[3], (const void*)A[5], (int)A[2], (int)A[4], 0, 0, 1, producer_stream};
+        const SqbGraphArgs da{nb[b], D[0], (const void*)D[1], (const void*)D[3], (const void*)D[5], (int)D[2], (int)D[4], dst_f64 ? 1 : 0, 0, 1,
+                              producer_stream};
+        SQB_TRY(load_caller(c, aa, &ba[b], "sqb_graph_combine (connectivities)"));
+        SQB_TRY(load_caller(c, da, &bd[b], "sqb_graph_combine (distances)"));
+        SQB_TRY(grow[b].alloc(nb[b]));
+        SQB_TRY(sqb_h2d(c, grow[b].p, out_row + r0, nb[b] * sizeof(int32_t)));
+    }
+    SQB_TRY(combine(c, total, ba, grow, nb, &g->adj));
+    SQB_TRY(combine(c, total, bd, grow, nb, &g->dst));
+    if (!ascending) {
+        SQB_TRY(sort_rows(c, total, &g->adj));
+        SQB_TRY(sort_rows(c, total, &g->dst));
+    }
+    SQB_CUDA(cudaStreamSynchronize(c->stream));
+    *n_out = total, *adj_nnz_out = g->adj.nnz, *dst_nnz_out = g->dst.nnz, *dst_f64_out = g->dst.f64 ? 1 : 0;
     *out = g.release();
     return SQB_OK;
 }

@@ -1,8 +1,9 @@
 """``squidpy_b200.gr`` — the spatial-statistics hot path of ``squidpy.gr`` on an H100."""
 
 from ._build import (DelaunayBuilder, GridBuilder, KNNBuilder, RadiusBuilder, SpatialNeighborsResult, delaunay_2d, knn_2d, radius_2d,
-                     spatial_neighbors_delaunay, spatial_neighbors_from_builder, spatial_neighbors_grid, spatial_neighbors_knn,
+                     spatial_neighbors, spatial_neighbors_delaunay, spatial_neighbors_from_builder, spatial_neighbors_grid, spatial_neighbors_knn,
                      spatial_neighbors_radius)
+from . import neighbors
 from ._mask import mask_graph
 from ._ligrec import ligrec, ligrec_analysis, ligrec_analysis_device
 from ._niche import (calculate_niche, calculate_niche_cellcharter, calculate_niche_neighborhood, calculate_niche_spatialleiden,
@@ -13,6 +14,7 @@ from ._ripley import nn_distance_hist, pair_counts, ripley
 from ._sepal import sepal, sepal_scores
 
 __all__ = [
+    "spatial_neighbors",
     "spatial_neighbors_knn",
     "spatial_neighbors_grid",
     "spatial_neighbors_radius",

@@ -1,8 +1,9 @@
 """Spatial neighbour graphs on the GPU — drop-ins for ``squidpy.gr.spatial_neighbors_knn / _grid / _radius``
 (``src/squidpy/gr/_build.py:484-549, 553-620, 701-786``) and the builder classes behind them
 (``src/squidpy/gr/neighbors.py``: ``KNNBuilder`` :157-209, ``RadiusBuilder`` :212-270, ``GridBuilder`` :335-419), plus
-``spatial_neighbors_delaunay`` / ``DelaunayBuilder`` (``_build.py:625-697``, ``neighbors.py:272-332``) and the public bridge
-``spatial_neighbors_from_builder`` (``_build.py:388-460``).
+``spatial_neighbors_delaunay`` / ``DelaunayBuilder`` (``_build.py:625-697``, ``neighbors.py:272-332``), the public bridge
+``spatial_neighbors_from_builder`` (``_build.py:388-460``), which also runs any ``GraphBuilder`` a caller writes, and the
+dispatcher ``spatial_neighbors`` (``_build.py:63-129, 132-329``).
 
 This is the step right before every hot-path call (SURVEY.md 8f-1): at 1M spots the scikit-learn KD-tree query costs
 seconds where the statistics now cost milliseconds.  The neighbour search runs on the H100 (``sqb_knn_2d`` /
@@ -23,18 +24,21 @@ from __future__ import annotations
 
 import ctypes as C
 import time
+import warnings
 from typing import Any, NamedTuple
 
 import numpy as np
-from scipy.sparse import block_diag, csr_matrix
+from scipy.sparse import csr_matrix
 
 from .._constants import CoordType, Key, Transform
-from .._device import DevArray, _torch_stream, array_device, device_matrix
+from .._device import DevArray, array_device, device_matrix
 from .._lib import Context, check, default_context, load, pointer_device
 from .._validators import assert_categorical_obs, assert_positive, assert_spatial_basis, extract_adata_if_sdata
+from ._postprocess import (_TRANSFORM_CODES, DistanceIntervalPostprocessor, GraphBuilder, GraphBuilderCSR, PercentilePostprocessor,
+                           TransformPostprocessor, _apply_transform, _filter_by_radius_interval, _percentile, export_graph, graph_pair_device)
 from ._utils import _save_data, logg
 
-__all__ = ["spatial_neighbors_knn", "spatial_neighbors_grid", "spatial_neighbors_radius", "spatial_neighbors_delaunay",
+__all__ = ["spatial_neighbors", "spatial_neighbors_knn", "spatial_neighbors_grid", "spatial_neighbors_radius", "spatial_neighbors_delaunay",
            "spatial_neighbors_from_builder", "SpatialNeighborsResult", "KNNBuilder", "GridBuilder", "RadiusBuilder", "DelaunayBuilder",
            "knn_2d", "radius_2d", "delaunay_2d"]
 
@@ -129,63 +133,23 @@ def _device_coords(coords) -> DevArray | None:
     return d
 
 
-_TRANSFORM_CODES = {Transform.NONE: 0, Transform.SPECTRAL: 1, Transform.COSINE: 2}
-
-
-# ---------------------------------------------------------------------------------------------------------
-# post-processing (host, O(nnz); follows neighbors.py:423-560)
-# ---------------------------------------------------------------------------------------------------------
-def _filter_by_radius_interval(adj: csr_matrix, dst: csr_matrix, radius: tuple[float, float]) -> None:
-    minn, maxx = radius
-    mask = (dst.data < minn) | (dst.data > maxx)
-    a_diag = adj.diagonal()
-    dst.data[mask] = 0.0
-    adj.data[mask] = 0.0
-    adj.setdiag(a_diag)
-
-
-def _percentile(adj: csr_matrix, dst: csr_matrix, percentile: float) -> tuple[csr_matrix, csr_matrix]:
-    threshold = np.percentile(dst.data, percentile)
-    adj[dst > threshold] = 0.0
-    dst[dst > threshold] = 0.0
-    return adj, dst
-
-
-def _transform_spectral(a: csr_matrix) -> csr_matrix:
-    """D^-1/2 A D^-1/2 with D = column sums (``symmetric_normalize_csr``, neighbors.py:530-549), float32 result."""
-    if not a.nnz:
-        return a
-    degrees = np.squeeze(np.array(np.sqrt(1.0 / a.sum(axis=0))))
-    rows = np.repeat(np.arange(a.shape[0]), np.diff(a.indptr))
-    res = (degrees[rows] * degrees[a.indices] * a.data).astype(np.float32)
-    return csr_matrix((res, a.indices, a.indptr), shape=a.shape)
-
-
-def _apply_transform(adj: csr_matrix, dst: csr_matrix, transform: Transform) -> tuple[csr_matrix, csr_matrix]:
-    # eliminate_zeros() of the reference (neighbors.py:463-464); a full pass only when there is something to drop
-    if np.count_nonzero(adj.data) != adj.data.size:
-        adj.eliminate_zeros()
-    if np.count_nonzero(dst.data) != dst.data.size:
-        dst.eliminate_zeros()
-    if transform == Transform.SPECTRAL:
-        return _transform_spectral(adj), dst
-    if transform == Transform.COSINE:
-        from sklearn.metrics.pairwise import cosine_similarity
-
-        return cosine_similarity(adj, dense_output=False), dst
-    if transform == Transform.NONE:
-        return adj, dst
-    raise NotImplementedError(f"Transform `{transform}` is not yet implemented.")
-
-
 # ---------------------------------------------------------------------------------------------------------
 # builders (same constructor arguments / uns_params / build contract as neighbors.py)
 # ---------------------------------------------------------------------------------------------------------
-class _Builder:
-    def __init__(self, transform=None, set_diag: bool = False, percentile: float | None = None, ctx: Context | None = None):
-        self.transform = Transform.NONE if transform is None else Transform(transform)
-        self.set_diag = set_diag
-        self.percentile = percentile
+def _postprocessor_list(interval, percentile, transform) -> list:
+    """The post-processors a built-in builder declares (neighbors.py:173-176, :228-233, :298-303, :357), in their order."""
+    steps = [] if interval is None else [DistanceIntervalPostprocessor(interval)]
+    if percentile is not None:
+        steps.append(PercentilePostprocessor(percentile))
+    return [*steps, TransformPostprocessor(Transform.NONE if transform is None else Transform(transform))]
+
+
+class _Builder(GraphBuilderCSR):
+    """The built-in builders: ``postprocessors()`` lists the reference's steps, while ``build`` runs the search and those
+    steps on the GPU for device coordinates, or fused on the host (``_build_host``)."""
+
+    def __init__(self, transform=None, set_diag: bool = False, percentile: float | None = None, ctx: Context | None = None, postprocessors=()):
+        super().__init__(transform, set_diag, percentile, postprocessors)
         self.ctx = ctx
 
     def build_graph(self, coords) -> tuple[csr_matrix, csr_matrix]:  # pragma: no cover
@@ -210,8 +174,6 @@ class _Builder:
     def build_device(self, d: DevArray, device: int | None = None, libraries: tuple[np.ndarray, np.ndarray] | None = None):
         """The graph of device coordinates ``d`` on their device (an explicit ``device`` must name it) as torch ``sparse_csr``
         CUDA tensors; ``libraries = (ptr int64, rows int32)`` builds every library's rows as its own block."""
-        import torch
-
         on = array_device(d, pointer_device)
         if device is not None and int(device) != on:
             raise ValueError(f"`device={device}` does not match the device of the spatial coordinates, cuda:{on}.")
@@ -220,25 +182,13 @@ class _Builder:
         lo, hi = interval if interval is not None else (0.0, 0.0)
         pct = np.nan if self.percentile is None else float(self.percentile)
         lp, lr, n_libs = (None, None, 0) if libraries is None else (libraries[0].ctypes.data, libraries[1].ctypes.data, libraries[0].size - 1)
-        lib = load()
         h, n_out, nnz_a, nnz_d, f64 = C.c_void_p(), C.c_int64(), C.c_int64(), C.c_int64(), C.c_int()
         with ctx.lock:
-            check(lib.sqb_graph_build_device(ctx.handle, d.ptr, int(d.dtype == np.float64), d.shape[0], d.strides[0], d.strides[1], d.stream, kind, k,
-                                             n_rings, float(radius), int(interval is not None), float(lo), float(hi), int(bool(self.set_diag)), pct,
-                                             _TRANSFORM_CODES[self.transform], lp, lr, n_libs, C.byref(h), C.byref(n_out), C.byref(nnz_a),
-                                             C.byref(nnz_d), C.byref(f64)))
-            try:
-                n, dev = n_out.value, torch.device("cuda", on)
-                parts = [torch.empty(n + 1, dtype=torch.int32, device=dev), torch.empty(nnz_a.value, dtype=torch.int32, device=dev),
-                         torch.empty(nnz_a.value, dtype=torch.float32, device=dev), torch.empty(n + 1, dtype=torch.int32, device=dev),
-                         torch.empty(nnz_d.value, dtype=torch.int32, device=dev),
-                         torch.empty(nnz_d.value, dtype=torch.float64 if f64.value else torch.float32, device=dev)]
-                check(lib.sqb_graph_export(h, *(t.data_ptr() or None for t in parts), _torch_stream(parts[0])))
-            finally:
-                lib.sqb_graph_free(h)
-        adj = torch.sparse_csr_tensor(parts[0], parts[1], parts[2], size=(n, n))
-        dst = torch.sparse_csr_tensor(parts[3], parts[4], parts[5], size=(n, n))
-        return adj, dst
+            check(load().sqb_graph_build_device(ctx.handle, d.ptr, int(d.dtype == np.float64), d.shape[0], d.strides[0], d.strides[1], d.stream, kind,
+                                                k, n_rings, float(radius), int(interval is not None), float(lo), float(hi), int(bool(self.set_diag)),
+                                                pct, _TRANSFORM_CODES[self.transform], lp, lr, n_libs, C.byref(h), C.byref(n_out), C.byref(nnz_a),
+                                                C.byref(nnz_d), C.byref(f64)))
+            return export_graph(h, on, n_out.value, nnz_a.value, nnz_d.value, bool(f64.value))
 
     def build(self, coords) -> tuple[csr_matrix, csr_matrix]:
         d = _device_coords(coords)
@@ -260,17 +210,6 @@ class _Builder:
                 adj, dst = _percentile(adj, dst, self.percentile)
             return _apply_transform(adj, dst, self.transform)
 
-    def combine(self, mats, ixs) -> tuple[csr_matrix, csr_matrix]:
-        """Per-library blocks -> one graph in the original observation order (``GraphBuilderCSR.combine``, neighbors.py:138-156)."""
-        adj = block_diag([m[0] for m in mats], format="csr")
-        dst = block_diag([m[1] for m in mats], format="csr")
-        ixs_arr = np.asarray(ixs)
-        if ixs_arr.size and np.any(np.diff(ixs_arr) < 0):
-            order = np.argsort(ixs_arr)
-            adj = adj[order, :][:, order]
-            dst = dst[order, :][:, order]
-        return adj, dst
-
 
 def _csr_from_rows(n: int, k: int, idx: np.ndarray, vals: np.ndarray, keep: np.ndarray | None = None) -> csr_matrix:
     """(n, k) row-major neighbour table with ascending indices per row -> canonical CSR (int32 indices / indptr)."""
@@ -291,7 +230,7 @@ class KNNBuilder(_Builder):
 
     def __init__(self, n_neighs: int = 6, transform=None, set_diag: bool = False, percentile: float | None = None, ctx: Context | None = None):
         assert_positive(n_neighs, name="n_neighs")
-        super().__init__(transform, set_diag, percentile, ctx)
+        super().__init__(transform, set_diag, percentile, ctx, _postprocessor_list(None, percentile, transform))
         self.n_neighs = n_neighs
 
     def uns_params(self) -> dict[str, Any]:
@@ -304,7 +243,7 @@ class KNNBuilder(_Builder):
         dist, idx = knn_2d(coords, self.n_neighs, ctx=self.ctx)
         n = idx.shape[0]
         adj = _csr_from_rows(n, self.n_neighs, idx, np.ones(idx.shape, dtype=np.float32))
-        dst = _csr_from_rows(n, self.n_neighs, idx, dist)
+        dst = _csr_from_rows(n, self.n_neighs, idx.copy(), dist)  # its own indices: eliminate_zeros on one must not move the other's
         self._diagonals(adj, dst)
         return adj, dst
 
@@ -313,7 +252,8 @@ class RadiusBuilder(_Builder):
     """Radius graph (``neighbors.py:212-270``); a tuple radius builds with the larger value and prunes to the interval."""
 
     def __init__(self, radius, transform=None, set_diag: bool = False, percentile: float | None = None, ctx: Context | None = None):
-        super().__init__(transform, set_diag, percentile, ctx)
+        interval = tuple(sorted(radius)) if isinstance(radius, tuple) else None
+        super().__init__(transform, set_diag, percentile, ctx, _postprocessor_list(interval, percentile, transform))
         self.radius = list(radius) if isinstance(radius, tuple) else radius
 
     def _interval(self):
@@ -347,7 +287,7 @@ class GridBuilder(_Builder):
         assert_positive(n_rings, name="n_rings")
         if delaunay:
             raise NotImplementedError("`delaunay=True` needs a Delaunay triangulation (Qhull); the GPU builders offer kNN, radius and grid graphs.")
-        super().__init__(transform, set_diag, None, ctx)
+        super().__init__(transform, set_diag, None, ctx, _postprocessor_list(None, None, transform))
         self.n_neighs, self.n_rings, self.delaunay = n_neighs, n_rings, delaunay
 
     def uns_params(self) -> dict[str, Any]:
@@ -396,7 +336,8 @@ class DelaunayBuilder(_Builder):
     def __init__(self, radius=None, transform=None, set_diag: bool = False, percentile: float | None = None, ctx: Context | None = None):
         if isinstance(radius, int | float):
             radius = (0.0, float(radius))
-        super().__init__(transform, set_diag, percentile, ctx)
+        interval = None if radius is None else tuple(sorted(radius))
+        super().__init__(transform, set_diag, percentile, ctx, _postprocessor_list(interval, percentile, transform))
         self.radius = list(radius) if isinstance(radius, tuple) else radius
 
     def _interval(self):
@@ -451,11 +392,44 @@ def _library_rows(adata, library_key: str | None) -> tuple[np.ndarray, np.ndarra
     return ptr, np.ascontiguousarray(rows[skip:])
 
 
-def _run(adata, builder: _Builder, *, spatial_key: str, library_key: str | None, key_added: str, copy: bool, device: int | None = None):
+def _device_rows(coords, d, rows: np.ndarray):
+    """Rows ``rows`` of device coordinates, gathered on their device as a torch CUDA tensor; never read on the host."""
+    import torch
+
+    t = torch.as_tensor(coords, device=torch.device("cuda", array_device(d, pointer_device)))
+    return t.index_select(0, torch.as_tensor(rows, dtype=torch.int64, device=t.device))
+
+
+def _build_checked(builder: GraphBuilder, coords):
+    adj, dst = builder.build(coords)
+    graph_pair_device(adj, dst)  # both on the host or both on one GPU
+    return adj, dst
+
+
+def _run_custom(adata, builder: GraphBuilder, *, spatial_key: str, library_key: str | None):
+    """A caller's builder: ``builder.build`` once per library and ``builder.combine``, as ``_run_spatial_neighbors`` does.
+    Device coordinates are split into libraries on their device."""
+    coords = adata.obsm[spatial_key]
+    if library_key is None:
+        return _build_checked(builder, coords)
+    assert_categorical_obs(adata, key=library_key)
+    codes = np.asarray(adata.obs[library_key].array.codes)
+    dev = device_matrix(coords)
+    mats, idxs = [], []
+    for code in range(len(adata.obs[library_key].cat.categories)):
+        idx = np.where(codes == code)[0]
+        mats.append(_build_checked(builder, _device_rows(coords, dev, idx) if dev is not None else np.ascontiguousarray(np.asarray(coords)[idx])))
+        idxs.extend(idx.tolist())
+    return builder.combine(mats, idxs)
+
+
+def _run(adata, builder: GraphBuilder, *, spatial_key: str, library_key: str | None, key_added: str, copy: bool, device: int | None = None):
     """``_run_spatial_neighbors`` (``_build.py:789-850``)."""
     start = time.perf_counter()
-    dev = _device_coords(adata.obsm[spatial_key])
-    if dev is not None:
+    dev = _device_coords(adata.obsm[spatial_key]) if isinstance(builder, _Builder) else None
+    if not isinstance(builder, _Builder):
+        adj, dst = _run_custom(adata, builder, spatial_key=spatial_key, library_key=library_key)
+    elif dev is not None:
         adj, dst = builder.build_device(dev, device, _library_rows(adata, library_key))
     elif library_key is not None:
         assert_categorical_obs(adata, key=library_key)
@@ -540,18 +514,78 @@ def spatial_neighbors_delaunay(data: Any, *, spatial_key: str = Key.obsm.spatial
     return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy, device=device)
 
 
-def spatial_neighbors_from_builder(data: Any, builder: _Builder, *, spatial_key: str = Key.obsm.spatial,
+def spatial_neighbors_from_builder(data: Any, builder: GraphBuilder, *, spatial_key: str = Key.obsm.spatial,
                                    elements_to_coordinate_systems: dict[str, str] | None = None, table_key: str | None = None,
                                    library_key: str | None = None, key_added: str = "spatial", copy: bool = False, n_jobs: int = 1,
                                    device: int | None = None) -> SpatialNeighborsResult | None:
-    """Spatial graph from a builder the caller constructed (``_build.py:388-460``): any of ``KNNBuilder``, ``RadiusBuilder``,
-    ``GridBuilder`` and ``DelaunayBuilder``."""
-    if not isinstance(builder, _Builder):
+    """Spatial graph from a builder the caller constructed (``_build.py:388-460``): one of ``KNNBuilder``, ``RadiusBuilder``,
+    ``GridBuilder`` and ``DelaunayBuilder``, or any ``GraphBuilder`` subclass.  A custom builder gets the coordinates as they are
+    stored (per library, a device array's rows are gathered on its device); device graphs it returns are post-processed and
+    combined on their GPU."""
+    if not isinstance(builder, GraphBuilder):
         raise TypeError(f"Expected a graph builder, found `{type(builder).__name__}`.")
     adata = _prepare(data, spatial_key, table_key)
-    if builder.ctx is None and _device_coords(adata.obsm[spatial_key]) is None:
+    if isinstance(builder, _Builder) and builder.ctx is None and _device_coords(adata.obsm[spatial_key]) is None:
         import copy as _copy
 
         builder = _copy.copy(builder)  # the caller's builder keeps no context of this call
         builder.ctx = default_context(device)
+    return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy, device=device)
+
+
+_DEPRECATION = ("Calling `spatial_neighbors` is deprecated and will be removed in squidpy v1.9.0. Use `spatial_neighbors_knn`, "
+                "`spatial_neighbors_radius`, `spatial_neighbors_delaunay`, `spatial_neighbors_grid`, or `spatial_neighbors_from_builder` instead.")
+
+
+def _resolve_graph_builder(*, coord_type, n_neighs, radius, delaunay, n_rings, percentile, transform, set_diag,
+                           has_spatial_uns: bool = False) -> _Builder:
+    """The builder ``spatial_neighbors`` dispatches to (``_build.py:63-129``)."""
+    n_neighs_was_set = n_neighs is not None
+    n_neighs = 6 if n_neighs is None else n_neighs
+    delaunay = False if delaunay is None else delaunay
+    n_rings = 1 if n_rings is None else n_rings
+    set_diag = False if set_diag is None else set_diag
+    assert_positive(n_rings, name="n_rings")
+    assert_positive(n_neighs, name="n_neighs")
+    transform = Transform.NONE if transform is None else Transform(transform)
+    if coord_type is None:
+        if radius is not None:
+            logg.warning(f"Graph creation with `radius` is only available for generic coordinates. Ignoring parameter `radius = {radius}`.")
+        coord_type = CoordType.GRID if has_spatial_uns else CoordType.GENERIC
+    else:
+        coord_type = CoordType(coord_type)
+    common = {"transform": transform, "set_diag": set_diag}
+    if coord_type == CoordType.GRID:
+        if percentile is not None:
+            raise ValueError("`percentile` is not supported for grid coordinates. It only applies to generic (non-grid) graphs.")
+        return GridBuilder(n_neighs=n_neighs, **common, n_rings=n_rings, delaunay=delaunay)
+    if delaunay:
+        if n_neighs_was_set:
+            warnings.warn("Parameter `n_neighs` is ignored when `delaunay=True` use `spatial_neighbors_delaunay` instead.", FutureWarning,
+                          stacklevel=3)
+        # a scalar radius is ignored here; DelaunayBuilder would read it as the interval (0.0, r)
+        return DelaunayBuilder(**common, radius=radius if isinstance(radius, tuple) else None, percentile=percentile)
+    if radius is not None:
+        if n_neighs_was_set:
+            warnings.warn("Parameter `n_neighs` is ignored when `radius` is set use `spatial_neighbors_radius` instead.", FutureWarning,
+                          stacklevel=3)
+        return RadiusBuilder(**common, radius=radius, percentile=percentile)
+    return KNNBuilder(n_neighs=n_neighs, **common, percentile=percentile)
+
+
+def spatial_neighbors(adata: Any, spatial_key: str = Key.obsm.spatial, elements_to_coordinate_systems: dict[str, str] | None = None,
+                      table_key: str | None = None, library_key: str | None = None, coord_type: str | CoordType | None = None,
+                      n_neighs: int | None = None, radius: float | tuple[float, float] | None = None, delaunay: bool | None = None,
+                      n_rings: int | None = None, percentile: float | None = None, transform: str | Transform | None = None,
+                      set_diag: bool = False, key_added: str = "spatial", copy: bool = False, n_jobs: int = 1, *,
+                      device: int | None = None) -> SpatialNeighborsResult | None:
+    """Spatial graph from coordinates, the mode resolved from the arguments (``_build.py:132-329``; deprecated in the reference
+    in favour of the ``spatial_neighbors_*`` functions): grid when ``coord_type`` is ``"grid"`` (or ``None`` with
+    ``adata.uns["spatial"]`` present), else Delaunay when ``delaunay``, else radius when ``radius`` is given, else kNN.  The graph
+    is the one the matching ``spatial_neighbors_*`` call builds; ``n_jobs`` is accepted and ignored."""
+    warnings.warn(_DEPRECATION, FutureWarning, stacklevel=2)
+    adata = _prepare(adata, spatial_key, table_key)
+    builder = _resolve_graph_builder(coord_type=coord_type, n_neighs=n_neighs, radius=radius, delaunay=delaunay, n_rings=n_rings,
+                                     percentile=percentile, transform=transform, set_diag=set_diag, has_spatial_uns=Key.obsm.spatial in adata.uns)
+    builder.ctx = _host_context(adata, spatial_key, device)
     return _run(adata, builder, spatial_key=spatial_key, library_key=library_key, key_added=key_added, copy=copy, device=device)

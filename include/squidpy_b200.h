@@ -22,7 +22,8 @@
  *   sqb_pair_counts_f64        <- KDTree(points, metric=...).two_point_correlation(points, r)  src/squidpy/gr/_ripley.py:218-223
  *   sqb_ligrec_counts          <- _score_permutations(data, clustering, generators, ...)  src/squidpy/gr/_ligrec.py:616-676
  *   sqb_sepal                  <- _diffusion(conc, use_hex, n_iter, sat, sat_idx, unsat, unsat_idx, dt, thresh)  src/squidpy/gr/_sepal.py:186-233
- *   sqb_dense_gather_device    <- X.toarray() / np.asarray(X) + DataFrame.fillna(0.0) + column selection  src/squidpy/gr/_ligrec.py:203-218,
+ *   sqb_sepal_idxs             <- g.eliminate_zeros() + the max_neighs check + _compute_idxs  src/squidpy/gr/_sepal.py:308-361
+ *   sqb_dense_gather_device   <- X.toarray() / np.asarray(X) + DataFrame.fillna(0.0) + column selection  src/squidpy/gr/_ligrec.py:203-218,
  *                                 vals[:, genes] of _diffusion_genes  src/squidpy/gr/_sepal.py:117-128,186-233
  *   sqb_ligrec_observed        <- data.groupby("clusters").mean() / the expression-fraction mask of _analysis  src/squidpy/gr/_ligrec.py:679-700
  *   sqb_ligrec_counts_dense    <- _score_permutations on a gathered device matrix  src/squidpy/gr/_ligrec.py:616-676
@@ -418,6 +419,27 @@ int sqb_window_ranges(sqb_ctx* ctx, const void* xy, int xy_dtype, int64_t n, con
 int sqb_sepal(sqb_ctx* ctx, const double* vals, int64_t n_genes, int64_t n, const int32_t* sat, int64_t n_sat,
               const int32_t* sat_idx, int max_neighs, const int32_t* unsat, const int32_t* unsat_idx, int64_t n_unsat,
               int n_iter, double dt, double thresh, double* out);
+/* The tables sqb_sepal reads (`_compute_idxs`, src/squidpy/gr/_sepal.py:308-361), built on the device.
+ *   The graph: an n x n CSR (csc = 0) or CSC (csc = 1, read as scipy's tocsr) from the host (device_input = 0) or from device
+ *   memory (device_input = 1: DEVICE pointers on the context's device, read in place after producer_stream, as in
+ *   sqb_autocorr_load_csr_device).  indptr_bits / index_bits 32 or 64; data_dtype 0 f32, 1 f64, 3 i32, 4 i64, 5 bool; nnz < 2^31.
+ *   Entries whose value is 0 are dropped in storage order (eliminate_zeros: NaN stays, -0.0 and False go); a node's degree is
+ *   its count of remaining entries, duplicates included.
+ *   *max_degree: the largest degree.  When it is not max_neighs (in [1, 1024]) the call returns here, nothing else written.
+ *   Otherwise, in HOST buffers of n, n x max_neighs, n and n entries: sat = the ascending nodes of degree max_neighs (*n_sat),
+ *   sat_idx = their remaining columns in storage order, unsat = the ascending other nodes (*n_unsat), unsat_idx = each one's
+ *   first remaining column that is saturated, or for an orphan (no such column) the saturated node j minimising
+ *   |x_o - x_j| + |y_o - y_j| in float64, numpy's argmin over the ascending saturated nodes (the first of equal distances, the
+ *   first NaN distance before any other).
+ *   xy: n x 2 coordinates, read only when orphans exist: host float64 C-contiguous (xy_device = 0, xy_dtype 1, strides 2 and 1),
+ *   or a DEVICE pointer on the context's device (xy_device = 1, read after xy_stream) of xy_dtype 0 f32 / 1 f64 with element
+ *   strides stride_row / stride_col.  *nonfinite = 1 when a coordinate of an orphan or of a saturated node was read and is NaN
+ *   or infinite (scikit-learn's pairwise_distances refuses those), else 0.
+ * Returns once the caller's arrays are no longer read; errors leave the context usable.                                  */
+int sqb_sepal_idxs(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices, int index_bits,
+                   const void* data, int data_dtype, int csc, int device_input, uintptr_t producer_stream, const void* xy, int xy_dtype,
+                   int64_t stride_row, int64_t stride_col, int xy_device, uintptr_t xy_stream, int max_neighs, int64_t* max_degree,
+                   int32_t* sat, int32_t* sat_idx, int32_t* unsat, int32_t* unsat_idx, int64_t* n_sat, int64_t* n_unsat, int* nonfinite);
 
 /* ---- spatial neighbour graphs (what runs right before every hot-path call) ------------------------------------------
  * Exact k nearest neighbours of every observation among the others (2-D float64 coordinates, interleaved x,y), the query

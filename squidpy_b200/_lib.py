@@ -99,6 +99,9 @@ _SIGNATURES: dict[str, tuple] = {
                                     C.c_void_p, C.c_void_p]),
     "sqb_sepal": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64,
                             C.c_int, C.c_double, C.c_double, C.c_void_p]),
+    "sqb_sepal_idxs": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                 C.c_size_t, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_size_t, C.c_int, C.POINTER(C.c_int64),
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
     "sqb_dense_gather_device": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_int,
                                           C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int,
                                           C.c_int, C.c_size_t, c_void_pp]),

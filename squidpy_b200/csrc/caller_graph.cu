@@ -208,8 +208,8 @@ int load(sqb_ctx* c, const SqbGraphArgs& a, const void* indptr, const void* indi
         SQB_POST_LAUNCH();
         return SQB_OK;
     };
-    // SYMMETRIC reads the values in its reducer, in their own type
-    SQB_TRY(sym ? expand(SqbType<double>()) : dispatch_values<false>(a.data_dtype, where, expand));
+    // SYMMETRIC reads the values in its reducer, in their own type; a bool value becomes 1.0 / 0.0
+    SQB_TRY(sym ? expand(SqbType<double>()) : dispatch_values<true>(a.data_dtype, where, expand));
     uint32_t e = (uint32_t)nnz;
     if (!as_stored) {
         DevBuf<uint64_t> keys_s(c->stream);

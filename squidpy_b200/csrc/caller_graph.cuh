@@ -52,7 +52,7 @@ int sqb_with_caller_csr(sqb_ctx* c, int64_t n, int64_t nnz, const void* indptr, 
 //   SYMMETRIC  A + Aᵀ without the diagonal and without values (indices only).  Each (row, column) sums A's entries, then
 //              Aᵀ's, then the two (scipy's csr_plus_csr), in A's dtype: integers wrap at int_bits, bool is a logical or,
 //              floats add in their own precision.  Only non-zero sums are kept (NaN is non-zero).
-// STORED and CANONICAL values are in float64 slots; a float32 graph's are float32 numbers.
+// STORED and CANONICAL values are in float64 slots; a float32 graph's are float32 numbers, a bool graph's 1.0 / 0.0.
 enum class SqbGraphForm { STORED, CANONICAL, SYMMETRIC };
 
 struct SqbGraph {

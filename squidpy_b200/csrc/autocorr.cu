@@ -47,7 +47,7 @@
 #include <climits>
 #include <thread>
 
-#include "common.cuh"
+#include "caller_graph.cuh"
 
 #define TILE 32
 
@@ -1438,37 +1438,6 @@ __global__ void __launch_bounds__(256) ac_w_s0_seq_kernel(const double* __restri
     if (threadIdx.x == 0) *out = s;
 }
 
-__global__ void ac_iota_kernel(int32_t* __restrict__ out, int64_t m) {
-    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) out[k] = (int32_t)k;
-}
-
-// column ranges [cbeg[j], cend[j]) of the entries sorted by column (both zeroed first: an empty column stays empty)
-__global__ void ac_col_bounds_kernel(const int32_t* __restrict__ key, int64_t m, int32_t* __restrict__ cbeg, int32_t* __restrict__ cend) {
-    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += (int64_t)gridDim.x * blockDim.x) {
-        const int32_t j = key[p];
-        if (p == 0 || key[p - 1] != j) cbeg[j] = (int32_t)p;
-        if (p == m - 1 || key[p + 1] != j) cend[j] = (int32_t)(p + 1);
-    }
-}
-
-// csum[j] = sequential float64 sum of column j in row order; colT (or null) the same sum in W's dtype (W.sum(0))
-template <typename T>
-__global__ void ac_col_sums_kernel(const int32_t* __restrict__ cbeg, const int32_t* __restrict__ cend, const int32_t* __restrict__ perm,
-                                   const double* __restrict__ wd, const T* __restrict__ w, int64_t n, double* __restrict__ csum,
-                                   T* __restrict__ colT) {
-    for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
-        double s = 0.0;
-        T t = (T)0;
-        for (int32_t p = cbeg[j]; p < cend[j]; ++p) {
-            const int32_t e = perm[p];
-            s = __dadd_rn(s, wd[e]);
-            t = t + w[e];
-        }
-        csum[j] = s;
-        if (colT) colT[j] = t;
-    }
-}
-
 // ---- numpy's pairwise summation ---------------------------------------------------------------------------
 // A block of at most 128 values: a plain loop below 8, else eight strided accumulators combined as
 // ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) and the tail added in order.  (numpy starts the short loop from -0.0 and np.sum adds the
@@ -1676,38 +1645,15 @@ static int ac_build_w(sqb_autocorr* h, const T* w, double* moments) {
         SQB_POST_LAUNCH();
     }
     // stable transpose: the entries sorted by column keep their row order
-    DevBuf<int32_t> keys(c->stream), iota(c->stream), perm(c->stream), cbeg(c->stream), cend(c->stream), rowof(c->stream);
+    DevBuf<int32_t> perm(c->stream), cbeg(c->stream), cend(c->stream), rowof(c->stream);
     DevBuf<T> colT(c->stream);
     DevBuf<uint8_t> tmp(c->stream);
-    SQB_TRY(cbeg.alloc(n));
-    SQB_TRY(cend.alloc(n));
-    SQB_TRY(perm.alloc(nnz > 0 ? nnz : 1));
     if (moments) SQB_TRY(colT.alloc(n));
-    SQB_CUDA(cudaMemsetAsync(cbeg.p, 0, n * sizeof(int32_t), c->stream));
-    SQB_CUDA(cudaMemsetAsync(cend.p, 0, n * sizeof(int32_t), c->stream));
-    if (nnz > 0) {
-        SQB_TRY(keys.alloc(nnz));
-        SQB_TRY(iota.alloc(nnz));
-        {
-            SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-            ac_iota_kernel<<<ac_grid(c, nnz), 256, 0, c->stream>>>(iota.p, nnz);
-            SQB_POST_LAUNCH();
-        }
-        int bits = 1;
-        while (bits < 31 && ((uint64_t)(n - 1) >> bits) != 0) ++bits;
-        size_t bytes = 0;
-        SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, h->d_wi.p, keys.p, iota.p, perm.p, (int)nnz, 0, bits, c->stream));
-        SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
-        SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, h->d_wi.p, keys.p, iota.p, perm.p, (int)nnz, 0, bits, c->stream));
-        c->launches += 1;
-        SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_col_bounds_kernel<<<ac_grid(c, nnz), 256, 0, c->stream>>>(keys.p, nnz, cbeg.p, cend.p);
-        SQB_POST_LAUNCH();
-    }
+    SQB_TRY(sqb_col_order(c, SQB_K_AUTOCORR_PREP, h->d_wi.p, nnz, n, perm, cbeg, cend));
     {
         SqbLaunchScope scope(c, SQB_K_AUTOCORR_PREP);
-        ac_col_sums_kernel<T><<<ac_grid(c, n), 256, 0, c->stream>>>(cbeg.p, cend.p, perm.p, h->d_wd.p, w, n, h->d_csum.p,
-                                                                     moments ? colT.p : nullptr);
+        sqb_col_sums_kernel<T><<<ac_grid(c, n), 256, 0, c->stream>>>(cbeg.p, cend.p, perm.p, h->d_wd.p, w, n, h->d_csum.p,
+                                                                      moments ? colT.p : nullptr);
         SQB_POST_LAUNCH();
     }
     // rows of at most 7 entries that all carry the same float32 weight (a row-normalised binary graph) take the compact format;

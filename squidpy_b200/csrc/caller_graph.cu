@@ -322,3 +322,50 @@ int sqb_exclusive_scan(sqb_ctx* c, const uint32_t* in, uint32_t* out, int64_t m,
     *total = tail[0] + tail[1];
     return SQB_OK;
 }
+
+namespace {
+
+__global__ void cgraph_iota(int32_t* __restrict__ out, int64_t m) {
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) out[k] = (int32_t)k;
+}
+
+// column ranges [cbeg[j], cend[j]) of the entries sorted by column (both zeroed first: an empty column stays empty)
+__global__ void cgraph_col_bounds(const int32_t* __restrict__ key, int64_t m, int32_t* __restrict__ cbeg, int32_t* __restrict__ cend) {
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t j = key[p];
+        if (p == 0 || key[p - 1] != j) cbeg[j] = (int32_t)p;
+        if (p == m - 1 || key[p + 1] != j) cend[j] = (int32_t)(p + 1);
+    }
+}
+
+}  // namespace
+
+int sqb_col_order(sqb_ctx* c, int kclass, const int32_t* idx, int64_t m, int64_t n, DevBuf<int32_t>& perm, DevBuf<int32_t>& cbeg,
+                  DevBuf<int32_t>& cend) {
+    SQB_TRY(cbeg.alloc(n));
+    SQB_TRY(cend.alloc(n));
+    SQB_TRY(perm.alloc(m > 0 ? m : 1));
+    SQB_CUDA(cudaMemsetAsync(cbeg.p, 0, n * sizeof(int32_t), c->stream));
+    SQB_CUDA(cudaMemsetAsync(cend.p, 0, n * sizeof(int32_t), c->stream));
+    if (m == 0) return SQB_OK;
+    DevBuf<int32_t> keys(c->stream), iota(c->stream);
+    DevBuf<uint8_t> tmp(c->stream);
+    SQB_TRY(keys.alloc(m));
+    SQB_TRY(iota.alloc(m));
+    {
+        SqbLaunchScope scope(c, kclass);
+        cgraph_iota<<<sqb_grid_rows(c, m, 256), 256, 0, c->stream>>>(iota.p, m);
+        SQB_POST_LAUNCH();
+    }
+    int bits = 1;
+    while (bits < 31 && ((uint64_t)(n - 1) >> bits) != 0) ++bits;
+    size_t bytes = 0;
+    SQB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, idx, keys.p, iota.p, perm.p, (int)m, 0, bits, c->stream));
+    SQB_TRY(tmp.alloc(bytes > 0 ? bytes : 1));
+    SQB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, idx, keys.p, iota.p, perm.p, (int)m, 0, bits, c->stream));
+    c->launches += 1;
+    SqbLaunchScope scope(c, kclass);
+    cgraph_col_bounds<<<sqb_grid_rows(c, m, 256), 256, 0, c->stream>>>(keys.p, m, cbeg.p, cend.p);
+    SQB_POST_LAUNCH();
+    return SQB_OK;
+}

@@ -71,3 +71,29 @@ int sqb_load_graph(sqb_ctx* c, const SqbGraphArgs& a, SqbGraphForm form, int int
 // out[i] = in[0] + ... + in[i - 1] for i < m, and *total = the sum of all m (one synchronisation).  cub's launches are not
 // counted in c->launches.
 int sqb_exclusive_scan(sqb_ctx* c, const uint32_t* in, uint32_t* out, int64_t m, uint32_t* total);
+
+// A stable transpose of the m column indices idx of a CSR with n columns: its entries sorted by column, row order kept within
+// a column.  perm[p] is the entry at sorted position p (at least one slot), [cbeg[j], cend[j]) the positions of column j
+// (0, 0 when it is empty).  The kernels count under launch class kclass.
+int sqb_col_order(sqb_ctx* c, int kclass, const int32_t* idx, int64_t m, int64_t n, DevBuf<int32_t>& perm, DevBuf<int32_t>& cbeg,
+                  DevBuf<int32_t>& cend);
+
+// Column sums in row order over sqb_col_order's permutation, each added from 0 one entry after another: csum[j] over the
+// float64 values wd and colT[j] over the values w in their own type, as scipy's W.sum(axis=0) adds them.  Either output may
+// be null (with its input); that sum is skipped.
+template <typename T>
+__global__ void sqb_col_sums_kernel(const int32_t* __restrict__ cbeg, const int32_t* __restrict__ cend, const int32_t* __restrict__ perm,
+                                    const double* __restrict__ wd, const T* __restrict__ w, int64_t n, double* __restrict__ csum,
+                                    T* __restrict__ colT) {
+    for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        double s = 0.0;
+        T t = (T)0;
+        for (int32_t p = cbeg[j]; p < cend[j]; ++p) {
+            const int32_t e = perm[p];
+            if (csum) s = __dadd_rn(s, wd[e]);
+            if (colT) t = t + w[e];
+        }
+        if (csum) csum[j] = s;
+        if (colT) colT[j] = t;
+    }
+}

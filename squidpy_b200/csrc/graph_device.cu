@@ -16,7 +16,8 @@
 //  * entries are those of the host's CSR after eliminate_zeros: the host's explicit zeros (setdiag, pruning) only matter to
 //    the percentile, whose order statistics include them here too (the n diagonal zeros lead the sorted distances);
 //  * percentile: numpy's `linear` method evaluated from the two order statistics around (m - 1) * q / 100;
-//  * spectral: column sums of ones are exact counts; deg = sqrt(1 / count) and deg[i] * deg[j] * w in float32, in that order;
+//  * spectral: scipy's float32 column sums (each column added in row order; of ones, exact counts below 2^24);
+//    deg = sqrt(1 / sum) and deg[i] * deg[j] * w in float32, in that order;
 //  * cosine: sklearn's row normalisation (float32 squares summed in double, float32 / double) and scipy's csr_matmat
 //    (products v * b added into each output column in row-walk order, float32, zero sums dropped): the products of a row
 //    are generated in walk order and stably sorted by column, so each column's sum runs in the same order;
@@ -268,32 +269,37 @@ __global__ void gd_assemble_kernel(const int64_t* __restrict__ bptr, const int32
     }
 }
 
-// column sums of the connectivities in float64: exact counts for a matrix of ones (below 2^53), weighted sums otherwise
-__global__ void gd_colsum_kernel(const int32_t* __restrict__ idx, const float* __restrict__ val, int64_t m, double* __restrict__ sum) {
-    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) atomicAdd(&sum[idx[t]], (double)val[t]);
-}
-
-// D^-1/2 A D^-1/2 with D the column sums rounded to float32; every step rounded like numpy's float32
-__global__ void gd_spectral_kernel(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx, int64_t n, const double* __restrict__ colsum,
+// D^-1/2 A D^-1/2 with D the float32 column sums; every step rounded like numpy's float32
+__global__ void gd_spectral_kernel(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx, int64_t n, const float* __restrict__ colsum,
                                    float* __restrict__ val) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float di = __fsqrt_rn(__fdiv_rn(1.0f, (float)colsum[i]));
+        const float di = __fsqrt_rn(__fdiv_rn(1.0f, colsum[i]));
         for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) {
-            const float dj = __fsqrt_rn(__fdiv_rn(1.0f, (float)colsum[idx[t]]));
+            const float dj = __fsqrt_rn(__fdiv_rn(1.0f, colsum[idx[t]]));
             val[t] = __fmul_rn(__fmul_rn(di, dj), val[t]);
         }
     }
 }
 
-// sklearn's inplace_csr_row_normalize_l2: float32 squares summed in double, every value divided by the double norm
-__global__ void gd_rownorm_kernel(const int32_t* __restrict__ ptr, int64_t n, const float* __restrict__ x, float* __restrict__ xn) {
+enum { GD_NONFINITE_NAN = 1, GD_NONFINITE_INF = 2 };
+
+// sklearn's inplace_csr_row_normalize_l2: float32 squares summed in double, every value divided by the double norm.  A NaN or
+// an infinity among the values raises its bit of *bad (sklearn's check_array refuses them).
+__global__ void gd_rownorm_kernel(const int32_t* __restrict__ ptr, int64_t n, const float* __restrict__ x, float* __restrict__ xn,
+                                  unsigned* __restrict__ bad) {
+    unsigned b = 0;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         double s = 0.0;
-        for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) s = __dadd_rn(s, (double)__fmul_rn(x[t], x[t]));
+        for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) {
+            const float v = x[t];
+            b |= isnan(v) ? GD_NONFINITE_NAN : isinf(v) ? GD_NONFINITE_INF : 0u;
+            s = __dadd_rn(s, (double)__fmul_rn(v, v));
+        }
         const bool zero = s == 0.0;
         s = __dsqrt_rn(s);
         for (int32_t t = ptr[i]; t < ptr[i + 1]; ++t) xn[t] = zero ? x[t] : __double2float_rn(__ddiv_rn((double)x[t], s));
     }
+    if (b) atomicOr(bad, b);
 }
 
 // (row, column) keys of a CSR's entries; transposed: (column, row)
@@ -577,13 +583,15 @@ int assemble(sqb_ctx* c, const int64_t* bptr, const int32_t* bidx, const double*
     return SQB_OK;
 }
 
-// D^-1/2 A D^-1/2 of the connectivities in place (symmetric_normalize_csr); an empty matrix is returned as it is
+// D^-1/2 A D^-1/2 of the connectivities in place (symmetric_normalize_csr); an empty matrix is returned as it is.  The column
+// sums are scipy's a.sum(axis=0) on the float32 CSR: float32, each column added from 0 in row order.
 int spectral(sqb_ctx* c, int64_t n, Csr* adj) {
     if (adj->nnz == 0) return SQB_OK;
-    DevBuf<double> colsum(c->stream);
+    DevBuf<int32_t> perm(c->stream), cbeg(c->stream), cend(c->stream);
+    DevBuf<float> colsum(c->stream);
     SQB_TRY(colsum.alloc(n));
-    SQB_CUDA(cudaMemsetAsync(colsum.p, 0, n * sizeof(double), c->stream));
-    GD_LAUNCH(gd_colsum_kernel<<<blocks_for(c, adj->nnz), 256, 0, c->stream>>>(adj->idx.p, adj->vf.p, adj->nnz, colsum.p));
+    SQB_TRY(sqb_col_order(c, SQB_K_MISC, adj->idx.p, adj->nnz, n, perm, cbeg, cend));
+    GD_LAUNCH(sqb_col_sums_kernel<float><<<blocks_for(c, n), 256, 0, c->stream>>>(cbeg.p, cend.p, perm.p, nullptr, adj->vf.p, n, nullptr, colsum.p));
     GD_LAUNCH(gd_spectral_kernel<<<blocks_for(c, n), 256, 0, c->stream>>>(adj->ptr.p, adj->idx.p, n, colsum.p, adj->vf.p));
     return SQB_OK;
 }
@@ -598,8 +606,15 @@ int cosine(sqb_ctx* c, int64_t n, Csr* adj) {
     DevBuf<uint8_t> tmp(c->stream);
     Csr out(c->stream);
     const unsigned gb = blocks_for(c, n);
+    DevBuf<unsigned> bad(c->stream);
+    SQB_TRY(bad.alloc(1));
+    SQB_CUDA(cudaMemsetAsync(bad.p, 0, sizeof(unsigned), c->stream));
     SQB_TRY(xn.alloc(m));
-    GD_LAUNCH(gd_rownorm_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, n, adj->vf.p, xn.p));
+    GD_LAUNCH(gd_rownorm_kernel<<<gb, 256, 0, c->stream>>>(adj->ptr.p, n, adj->vf.p, xn.p, bad.p));
+    unsigned flags = 0;
+    SQB_TRY(read_back(c, &flags, bad.p, sizeof(unsigned)));
+    SQB_CHECK(!(flags & GD_NONFINITE_NAN), SQB_ERR_INVALID, "Input contains NaN.");
+    SQB_CHECK(!(flags & GD_NONFINITE_INF), SQB_ERR_INVALID, "Input contains infinity or a value too large for dtype('float32').");
     // B = Xn^T as CSR with ascending columns (scipy converts the CSC transpose to sorted CSR)
     SQB_TRY(keys.alloc(m));
     SQB_TRY(bkeys.alloc(m));
@@ -973,10 +988,17 @@ int percentile_step(sqb_ctx* c, int64_t n, double q, Csr* adj, Csr* dst) {
     }));
     SQB_TRY(sort_keys(c, tmp, vals.p, sorted.p, m));
     PctEnv env{c, sorted.p, 0};
-    double thr = 0.0;
-    SQB_TRY((dst->f64 ? percentile_linear : percentile_linear_f32)(q, m, &thr, pct_get, &env));
-    SQB_CHECK(thr >= 0.0, SQB_ERR_UNSUPPORTED,
-              "the percentile threshold %g is not >= 0: `dst > threshold` would mark every entry the distances do not store", thr);
+    // numpy's percentile is NaN when any value is; the radix sort puts a NaN with its sign bit set first and any other NaN last
+    double thr = 0.0, first = 0.0, last = 0.0;
+    SQB_TRY(pct_get(&env, 0, &first));
+    SQB_TRY(pct_get(&env, m - 1, &last));
+    if (isnan(first) || isnan(last))
+        thr = NAN;
+    else
+        SQB_TRY((dst->f64 ? percentile_linear : percentile_linear_f32)(q, m, &thr, pct_get, &env));
+    // a NaN threshold (also numpy's interpolation between two infinities) marks nothing: `dst > nan` is all False
+    SQB_CHECK(!(thr < 0.0), SQB_ERR_UNSUPPORTED,
+              "the percentile threshold %g is below 0: `dst > threshold` would mark every entry the distances do not store", thr);
     return with_dst(*dst, [&](auto* dv) -> int {
         using T = std::remove_pointer_t<decltype(dv)>;
         SQB_TRY(rewrite_rows<float>(c, n, adj, &Csr::vf, [&](int32_t* cnt, const int32_t* optr, int32_t* oidx, float* oval) {

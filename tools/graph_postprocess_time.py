@@ -1,8 +1,10 @@
 """Wall-clock times of the public post-processors on a caller's graph: the kNN(6) graph of 1M uniform points, built on the GPU
 (torch sparse_csr), then ``PercentilePostprocessor(90)`` followed by ``TransformPostprocessor("cosine")`` on the GPU, against
-the same two steps in scipy on host copies of the same graph.  The two are run alternately, five times each after a warm-up,
-and each time ends in a device synchronise; the outputs are compared entry for entry.  The GPU's name and power limit are read
-in the same run.  Writes a JSON line to stdout and to ``--out``.
+the same two steps in scipy on host copies of the same graph.  ``--steps spectral`` instead times
+``TransformPostprocessor("spectral")`` on the same graph with float32 weights, whose column sums depend on the order they are
+added in.  The two are run alternately, five times each after a warm-up, and each time ends in a device synchronise; the
+outputs are compared entry for entry.  The GPU's name and power limit are read in the same run.  Writes a JSON line to stdout
+and to ``--out``.
 
     python tools/graph_postprocess_time.py --out results/graph_postprocess_time.json
 """
@@ -32,13 +34,18 @@ def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--steps", choices=["percentile-cosine", "spectral"], default="percentile-cosine")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     co = np.random.default_rng(0).uniform(0, 1000, (args.n, 2))
     adj, dst = nb.KNNBuilder(n_neighs=6).build(torch.tensor(co, device="cuda"))
+    if args.steps == "spectral":
+        w = torch.rand(adj.values().numel(), generator=torch.Generator().manual_seed(1)).add_(0.05).cuda()
+        adj = torch.sparse_csr_tensor(adj.crow_indices(), adj.col_indices(), w, size=adj.shape)
     to_host = lambda t: sp.csr_matrix((t.values().cpu().numpy(), t.col_indices().cpu().numpy(), t.crow_indices().cpu().numpy()), shape=tuple(t.shape))
     hadj, hdst = to_host(adj), to_host(dst)
-    steps = [nb.PercentilePostprocessor(90.0), nb.TransformPostprocessor(Transform.COSINE)]
+    steps = ([nb.TransformPostprocessor(Transform.SPECTRAL)] if args.steps == "spectral"
+             else [nb.PercentilePostprocessor(90.0), nb.TransformPostprocessor(Transform.COSINE)])
 
     def run(a, d):
         for s in steps:
@@ -64,7 +71,7 @@ def main() -> None:
         want.sort_indices()
         same &= bool(np.array_equal(got.indptr, want.indptr) and np.array_equal(got.indices, want.indices)
                      and np.array_equal(got.data.view(np.uint8), want.data.view(np.uint8)))
-    rec = {"gpu": gpu_info(), "n": args.n, "graph": "kNN(6), device-built", "steps": "percentile(90) + cosine", "nnz": int(adj.values().numel()),
+    rec = {"gpu": gpu_info(), "n": args.n, "graph": "kNN(6), device-built", "steps": "spectral, float32 weights" if args.steps == "spectral" else "percentile(90) + cosine", "nnz": int(adj.values().numel()),
            "device_s_median": float(np.median(dev_t)), "device_s": dev_t, "scipy_host_s_median": float(np.median(host_t)), "scipy_host_s": host_t,
            "equal_bit_for_bit": same}
     line = json.dumps(rec)

@@ -1,7 +1,8 @@
 """Multi-GPU plumbing: one process per GPU, ``torch.distributed`` (NCCL on GPUs, gloo on CPU for tests).
 
-The hot path shards embarrassingly — permutations for ``nhood_enrichment``, features for ``spatial_autocorr``, pair
-tiles for ``co_occurrence``/``ripley`` — so there is exactly ONE collective per call, on the final small tensor
+The hot path shards embarrassingly — permutations for ``nhood_enrichment`` and ``ligrec``, features for
+``spatial_autocorr`` and ``sepal``, pair tiles for ``co_occurrence``/``ripley`` — so there is exactly ONE collective per call,
+on the final small tensor
 (SURVEY.md section 8e).  Chunking follows the reference's own rule for splitting work over workers:
 contiguous chunks of ``ceil(n / n_workers)`` (``src/squidpy/_utils.py:225-231``).
 """
@@ -75,6 +76,18 @@ def all_gather_rows(local: np.ndarray, n_total: int) -> np.ndarray:
     dist.all_gather_into_tensor(out, t)
     full = out.cpu().numpy().view(local.dtype).reshape((ws * step,) + row_shape)
     return np.ascontiguousarray(full[:n_total])
+
+
+def broadcast_from_rank0(obj):
+    """Rank 0's ``obj`` (any picklable object) on every rank, in one broadcast; ``obj`` itself without a process group."""
+    _, ws = world()
+    if ws == 1:
+        return obj
+    import torch.distributed as dist
+
+    box = [obj]
+    dist.broadcast_object_list(box, src=0, device=_device_for_backend())
+    return box[0]
 
 
 def all_reduce_sum(local: np.ndarray) -> np.ndarray:

@@ -26,7 +26,7 @@ import pandas as pd
 
 from .._constants import ComplexPolicy, CorrAxis, Key
 from .._device import device_matrix
-from .._dist import shared_seed
+from .._dist import all_reduce_sum, shard_range, shared_seed, world
 from .._lib import Context, check, default_context, load
 from .._rng import spawn_states
 from .._validators import assert_categorical_obs, assert_positive, extract_adata_if_sdata
@@ -50,7 +50,9 @@ def ligrec_analysis(data: pd.DataFrame, interactions: np.ndarray, interaction_cl
                     n_perms: int = 1000, seed: int | None = None, *, ctx: Context | None = None) -> TempResult:
     """``_analysis`` (``_ligrec.py:679-776``): ``data`` has one integer-named column per gene plus a categorical column
     ``'clusters'`` whose categories are ``0 .. n_cls-1``; ``interactions`` holds column positions, ``interaction_clusters``
-    cluster codes."""
+    cluster codes.
+    Under an initialised ``torch.distributed`` process group (one process per GPU) the permutations are sharded over the ranks
+    and the permutation counts summed once over them; every rank gets the full result."""
     clustering = np.array(data["clusters"].values, dtype=np.int32)
     data = data.astype({c: np.float64 for c in data.columns if c != "clusters"})
     groups = data.groupby("clusters", observed=True)
@@ -89,25 +91,35 @@ def _decisions(mean_obs: np.ndarray, mask: np.ndarray, cluster_sizes: np.ndarray
 def _permutation_test(ctx: Context, clustering: np.ndarray, n_cls: int, inter: np.ndarray, cpairs: np.ndarray, inv_counts: np.ndarray,
                       mean_obs: np.ndarray, valid: np.ndarray, res_means: np.ndarray, n_perms: int, seed: int | None, counts_call) -> TempResult:
     """The permutation counts on a graph-less nhood handle whose base labels are ``clustering``; ``counts_call(lib, h, inv_counts,
-    mean_obs, valid_u8, counts)`` runs the counting entry point on the expression matrix of the caller's choice."""
+    mean_obs, valid_u8, counts)`` runs the counting entry point on the expression matrix of the caller's choice.
+
+    Under an initialised ``torch.distributed`` process group rank ``r`` counts only the permutations ``shard_range(n_perms, r,
+    world)`` (generators of one family: ``seed=None`` is drawn once on rank 0) and the int64 counts are summed over the ranks in
+    one all-reduce.  Integer sums are exact, so every rank gets the single-process result bit for bit."""
     n_cells = clustering.shape[0]
-    lib = load()
     counts = np.zeros((inter.shape[0], cpairs.shape[0]), dtype=np.int64)
-    valid_u8 = np.ascontiguousarray(valid, dtype=np.uint8)
-    mean_c = np.ascontiguousarray(mean_obs, dtype=np.float64)
-    with ctx.lock:
-        h = C.c_void_p()
-        empty_ptr = np.zeros(n_cells + 1, dtype=np.uint32)
-        # a graph-less handle: only the label shuffle of the nhood machinery is used (n_cls >= 2 is asserted by the caller)
-        check(lib.sqb_nhood_create(ctx.handle, n_cells, 0, empty_ptr.ctypes.data, None, max(n_cls, 2), C.byref(h)))
-        try:
-            lab = np.ascontiguousarray(clustering, dtype=np.uint32)
-            check(lib.sqb_nhood_set_base(h, lab.ctypes.data, None, 0))
-            states = spawn_states(seed, int(n_perms))
-            check(lib.sqb_nhood_permute_upload(h, states.ctypes.data, states.shape[0]))
-            counts_call(lib, h, inv_counts, mean_c, valid_u8, counts)
-        finally:
-            lib.sqb_nhood_destroy(h)
+    rank, ws = world()
+    lo, hi = shard_range(int(n_perms), rank, ws)
+    seed = shared_seed(seed)
+    logg.info("Counting ligrec permutations on cuda:%d (rank %d/%d, permutations %d..%d)", ctx.device, rank, ws, lo, hi)
+    if hi > lo:  # more ranks than permutations: this rank adds zeros (the handle refuses an empty upload)
+        lib = load()
+        valid_u8 = np.ascontiguousarray(valid, dtype=np.uint8)
+        mean_c = np.ascontiguousarray(mean_obs, dtype=np.float64)
+        with ctx.lock:
+            h = C.c_void_p()
+            empty_ptr = np.zeros(n_cells + 1, dtype=np.uint32)
+            # a graph-less handle: only the label shuffle of the nhood machinery is used (n_cls >= 2 is asserted by the caller)
+            check(lib.sqb_nhood_create(ctx.handle, n_cells, 0, empty_ptr.ctypes.data, None, max(n_cls, 2), C.byref(h)))
+            try:
+                lab = np.ascontiguousarray(clustering, dtype=np.uint32)
+                check(lib.sqb_nhood_set_base(h, lab.ctypes.data, None, 0))
+                states = spawn_states(seed, int(n_perms), lo, hi)
+                check(lib.sqb_nhood_permute_upload(h, states.ctypes.data, states.shape[0]))
+                counts_call(lib, h, inv_counts, mean_c, valid_u8, counts)
+            finally:
+                lib.sqb_nhood_destroy(h)
+    counts = all_reduce_sum(counts)
     pvalues = counts.astype(np.float64) / n_perms
     pvalues[~valid] = np.nan
     return TempResult(means=res_means, pvalues=pvalues)
@@ -117,7 +129,9 @@ def ligrec_analysis_device(x: Gathered, clustering: np.ndarray, n_cls: int, inte
                            threshold: float = 0.1, n_perms: int = 1000, seed: int | None = None) -> TempResult:
     """``ligrec_analysis`` on a matrix gathered on the device (observations x genes, float64, NaN written as 0): cluster
     ``clustering[i]`` in ``[0, n_cls)`` for observation ``i``, every cluster present.  The observed means are pandas' group
-    means bit for bit (``sqb_ligrec_observed``), so the result equals ``ligrec_analysis`` on the same values."""
+    means bit for bit (``sqb_ligrec_observed``), so the result equals ``ligrec_analysis`` on the same values.
+    Under an initialised ``torch.distributed`` process group (one process per GPU) the permutations are sharded over the ranks
+    and the permutation counts summed once over them; every rank gets the full result."""
     lib = load()
     ctx = x.ctx
     codes = np.ascontiguousarray(clustering, dtype=np.int32)
@@ -333,7 +347,9 @@ def ligrec(adata: Any, cluster_key: str, interactions: Any = None, complex_polic
            table_key: str | None = None, device: int | None = None) -> Mapping[str, pd.DataFrame] | None:
     """Permutation test of receptor-ligand interactions between clusters (``_ligrec.py:543-613``); returns / writes
     ``adata.uns[f'{cluster_key}_ligrec'] = {'means', 'pvalues', 'metadata'}`` (frames indexed by (source, target), columns
-    (cluster_1, cluster_2)).  ``n_jobs`` / ``show_progress_bar`` are accepted and ignored."""
+    (cluster_1, cluster_2)).  ``n_jobs`` / ``show_progress_bar`` are accepted and ignored.
+    Under an initialised ``torch.distributed`` process group (one process per GPU) the permutations are sharded over the ranks
+    and the permutation counts summed once over them; every rank gets the full result."""
     adata = extract_adata_if_sdata(adata, table_key=table_key)
     if not adata.shape[0]:
         raise ValueError("No cells are in `adata.obs_names`.")
@@ -362,7 +378,7 @@ def ligrec(adata: Any, cluster_key: str, interactions: Any = None, complex_polic
         logg.info("Running `%d` permutations on `%d` interactions and `%d` cluster combinations on the GPU", n_perms, len(pairs_df), len(clusters))
         with ctx.lock, Gathered(ctx, m, sel.rows, sel.gene_pos, OBS_MAJOR, nan_zero=True) as x:
             res_t = ligrec_analysis_device(x, sel.codes, sel.n_cls, sel.inter_, sel.clusters_, threshold=threshold, n_perms=int(n_perms),
-                                           seed=shared_seed(seed))
+                                           seed=seed)
         return _finish(adata, res_t, pairs_df, clusters, inter, corr_method, corr_axis, alpha, copy, cluster_key, key_added, start)
     from scipy.sparse import issparse
 
@@ -403,7 +419,7 @@ def ligrec(adata: Any, cluster_key: str, interactions: Any = None, complex_polic
 
     start = time.perf_counter()
     logg.info("Running `%d` permutations on `%d` interactions and `%d` cluster combinations on the GPU", n_perms, len(pairs_df), len(clusters))
-    res_t = ligrec_analysis(sub, inter_, clusters_, threshold=threshold, n_perms=int(n_perms), seed=shared_seed(seed), ctx=default_context(device))
+    res_t = ligrec_analysis(sub, inter_, clusters_, threshold=threshold, n_perms=int(n_perms), seed=seed, ctx=default_context(device))
     return _finish(adata, res_t, pairs_df, clusters, inter, corr_method, corr_axis, alpha, copy, cluster_key, key_added, start)
 
 

@@ -17,6 +17,7 @@ from scipy.sparse import csr_matrix, issparse
 
 from .._constants import Key
 from .._device import DevArray, DevMatrix, DevSparse, _contiguous_1d, device_matrix, on_host
+from .._dist import all_gather_rows, broadcast_from_rank0, shard_range, world
 from .._lib import Context, check, default_context, load, pointer_device
 from .._validators import assert_connectivity_key, assert_spatial_basis, extract_adata_if_sdata
 from ._gather import GENE_MAJOR, Gathered, device_context
@@ -209,7 +210,9 @@ def sepal(adata: Any, max_neighs: int, genes: str | Sequence[str] | None = None,
           device: int | None = None) -> pd.DataFrame | None:
     """Identify spatially variable genes with *Sepal* (see module docstring).  Returns / writes ``adata.uns['sepal_score']``: a
     DataFrame indexed by gene with the column ``sepal_score``, sorted descending.  ``n_jobs`` / ``show_progress_bar`` are accepted
-    and ignored."""
+    and ignored.
+    Under an initialised ``torch.distributed`` process group (one process per GPU) the genes are sharded over the ranks and the
+    scores all-gathered once; every rank gets the full result."""
     adata = extract_adata_if_sdata(adata, table_key=table_key)
     assert_connectivity_key(adata, connectivity_key)
     assert_spatial_basis(adata, key=spatial_key)
@@ -232,7 +235,11 @@ def sepal(adata: Any, max_neighs: int, genes: str | Sequence[str] | None = None,
         use_raw = False
     src = adata.raw if use_raw else adata
     if use_raw:
-        genes = list(set(src.var_names) & set(genes))
+        # set order follows the process's string hashing, which differs between ranks: every rank takes rank 0's order, so
+        # that a gene's position, and with it its shard, means the same gene everywhere
+        genes = broadcast_from_rank0(list(set(src.var_names) & set(genes)))
+    rank, ws = world()
+    lo, hi = shard_range(len(genes), rank, ws)
     whole = src.X if (layer is None or use_raw) else src.layers[layer]
     if device_matrix(whole) is not None:  # the genes are gathered by position on the array's device; X is not read on the host
         m, ctx = device_context(whole, device)
@@ -243,16 +250,19 @@ def sepal(adata: Any, max_neighs: int, genes: str | Sequence[str] | None = None,
             raise IndexError(f"Gene positions must lie in [-{m.shape[1]}, {m.shape[1]}).")
         positions = positions % m.shape[1]  # negative positions count from the end, as in X[:, genes]
         start = time.perf_counter()
-        logg.info("Calculating sepal score for `%d` genes on the GPU", len(genes))
-        score = _scores_device(m, ctx, positions, sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter),
+        logg.info("Calculating sepal score for `%d` genes on cuda:%d (rank %d/%d, genes %d..%d)", len(genes), ctx.device, rank, ws, lo, hi)
+        score = _scores_device(m, ctx, positions[lo:hi], sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter),
                                dt=dt, thresh=thresh, batch_genes=None)
     else:
         sub = src[:, genes]
         vals = sub.X if (layer is None or use_raw) else sub.layers[layer]
+        if ws > 1:
+            vals = vals[:, lo:hi]
+        ctx = default_context(device)
         start = time.perf_counter()
-        logg.info("Calculating sepal score for `%d` genes on the GPU", len(genes))
-        score = sepal_scores(vals, sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter), dt=dt, thresh=thresh,
-                             ctx=default_context(device))
+        logg.info("Calculating sepal score for `%d` genes on cuda:%d (rank %d/%d, genes %d..%d)", len(genes), ctx.device, rank, ws, lo, hi)
+        score = sepal_scores(vals, sat, sat_idx, unsat, unsat_idx, max_neighs=max_neighs, n_iter=int(n_iter), dt=dt, thresh=thresh, ctx=ctx)
+    score = all_gather_rows(score, len(genes))
     key_added = "sepal_score"
     sepal_score = pd.DataFrame(score, index=genes, columns=[key_added])
     if sepal_score[key_added].isna().any():

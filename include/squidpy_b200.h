@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define SQB_ABI_VERSION 17
+#define SQB_ABI_VERSION 18
 
 typedef enum {
     SQB_OK = 0,
@@ -193,19 +193,22 @@ int sqb_nhood_bytes_per_perm(sqb_nhood* h, int64_t* bytes);
  * Replaces _interaction_matrix(data, indices, indptr, cats, output) (src/squidpy/gr/_nhood.py:401,412-429) and the NaN
  * masking of interaction_matrix (:386-395).  codes[i] in [0, n_cls) or < 0 for an observation without label: stored
  * entries with an unlabelled end point are skipped (== restricting the graph to the labelled observations).
- * data == NULL (weights=False): out_counts[a*n_cls+b] = number of stored entries (i->j) with code(i)=a, code(j)=b (int64).
- * data != NULL (weights=True, data_dtype 0 = f32, 1 = f64): out_weighted[a*n_cls+b] = float64 sum of their values.       */
+ * data_dtype -1 (weights=False, data unused): out_counts[a*n_cls+b] = number of stored entries (i->j) with code(i)=a,
+ * code(j)=b (int64).  weights=True: data_dtype 3 = int32, 4 = int64, 5 = bool (one byte): out_counts = int64 sum of their
+ * values, wrapping modulo 2^64 like numba's int64; 0 = f32, 1 = f64: out_weighted = float64 sum in the reference's order
+ * (rows ascending, each row's entries in storage order), bit-identical to it and the same from run to run.            */
 int sqb_interaction_matrix(sqb_ctx* ctx, int64_t n, int64_t nnz, const uint32_t* indptr, const uint32_t* indices,
                            const void* data, int data_dtype, const int32_t* codes, int n_cls, double* out_weighted,
                            int64_t* out_counts);
 /* The same from a graph in device memory, read in place (no copy): indptr / indices / data are DEVICE pointers on the
- * context's device, indptr_bits / index_bits 32 or 64; codes and the outputs stay on the host.  weights=True is selected by
- * out_weighted != NULL (out_counts otherwise); data_dtype 0 = f32, 1 = f64, 2 = f16, 3 = int32, 4 = int64, 5 = bool (one
- * byte), every value summed in float64.  indptr is checked on the device before anything follows it; column indices outside
+ * context's device, indptr_bits / index_bits 32 or 64; codes and the outputs stay on the host.  csc != 0: the arrays are a
+ * CSC graph's, i.e. the CSR of its transpose; out is then the transpose of the graph's result, and float sums follow the
+ * order of the graph's tocsr() (rows ascending, columns ascending within a row, duplicates in storage order).  data_dtype
+ * and outputs as above, plus 2 = f16 (float64 sums).  indptr is checked on the device before anything follows it; column indices outside
  * [0, n) and codes >= n_cls are detected by the kernel (SQB_ERR_INVALID, no result).  producer_stream: as in
  * sqb_autocorr_load_csr_device.  Returns after the device has stopped reading the caller's buffers.                   */
 int sqb_interaction_matrix_device(sqb_ctx* ctx, int64_t n, int64_t nnz, const void* indptr, int indptr_bits, const void* indices,
-                                  int index_bits, const void* data, int data_dtype, const int32_t* codes, int n_cls,
+                                  int index_bits, int csc, const void* data, int data_dtype, const int32_t* codes, int n_cls,
                                   double* out_weighted, int64_t* out_counts, uintptr_t producer_stream);
 
 /* ---- centrality_scores -------------------------------------------------------------------------------------

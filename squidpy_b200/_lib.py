@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # $SQB_LIB_PATH: another build of the same C ABI (tools/apply_phases.py points it at the build with the region replay's
 # phase clocks, tools/native/libsquidpy_b200_clocks.so); the package itself only ever ships libsquidpy_b200.so
 LIB_PATH = os.environ.get("SQB_LIB_PATH") or os.path.join(_HERE, "libsquidpy_b200.so")
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 _lock = threading.Lock()
 _lib: C.CDLL | None = None
@@ -63,7 +63,7 @@ _SIGNATURES: dict[str, tuple] = {
     "sqb_nhood_permute_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "sqb_interaction_matrix": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                           C.c_int, C.c_void_p, C.c_void_p]),
-    "sqb_interaction_matrix_device": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+    "sqb_interaction_matrix_device": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                                  C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t]),
     "sqb_nhood_permute_sums": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sqb_nhood_permute_var_chain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -455,7 +455,10 @@ def interaction_matrix(
     """Compute the interaction matrix of the clusters (reference ``gr/_nhood.py:349-409``): entry (a, b) sums the stored
     entries (i -> j) of ``obsp[connectivity_key]`` with cluster(i) = a and cluster(j) = b, their values if ``weights`` else
     ones; observations with a NaN label are dropped from rows and columns; ``normalized`` divides every row by its sum.
-    dtype as in the reference (:398): int64 for bool / integer graphs, float64 otherwise.
+    dtype as in the reference (:398): int64 for bool / integer graphs, float64 otherwise.  Every result equals the
+    reference's bit for bit and does not change from run to run: integer and bool values are summed in int64 (wrapping modulo
+    2^64 as the reference's int64 sums do), float values in float64 in the reference's order (rows ascending, each row's
+    entries in storage order; for a CSC graph the order of its ``tocsr()``).
 
     Returns the matrix if ``copy=True``, otherwise writes ``adata.uns[f'{cluster_key}_interactions']``."""
     import pandas as pd
@@ -480,31 +483,27 @@ def interaction_matrix(
     n_cats = len(cats.cat.categories)
     int_graph = bool(pd.api.types.is_bool_dtype(value_dtype) or pd.api.types.is_integer_dtype(value_dtype))
 
+    # value code of the ABI: -1 counts; integer and bool values are summed in int64 (wrapping like the reference's int64
+    # output), float values in float64 in the reference's order
+    if not weights:
+        code, data = -1, None
+    elif dev is not None:
+        code = graph_value_code(graph.sparse.data, graph.nnz)
+    else:
+        dtype, code, _ = _HOST_VALUES.get(g.dtype, (np.float64, 1, 64))
+        data = np.ascontiguousarray(g.data.view(np.int64) if g.dtype == np.uint64 else g.data, dtype=dtype)
+    int_sums = code < 0 or code >= 3
+    out = np.zeros((n_cats, n_cats), dtype=np.int64 if int_sums else np.float64)
     ctx = default_context(device)
     lib = load()
-    if weights:
-        out = np.zeros((n_cats, n_cats), dtype=np.float64)
-        if dev is not None:
-            _interaction_device(lib, ctx, graph, codes, n_cats, out, None)
-        else:
-            indptr, indices = _as_u32(g.indptr), _as_u32(g.indices)
-            data = g.data
-            if data.dtype not in (np.float32, np.float64):
-                data = data.astype(np.float64)  # integer / bool weights are summed exactly in float64 (< 2^53)
-            data = np.ascontiguousarray(data)
-            check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
-                                             data.ctypes.data, 0 if data.dtype == np.float32 else 1, codes.ctypes.data, n_cats,
-                                             out.ctypes.data, None))
-        output = np.rint(out).astype(np.int64) if int_graph else out
+    if dev is not None:
+        _interaction_device(lib, ctx, graph, codes, n_cats, code, out)
     else:
-        cnt = np.zeros((n_cats, n_cats), dtype=np.int64)
-        if dev is not None:
-            _interaction_device(lib, ctx, graph, codes, n_cats, None, cnt)
-        else:
-            indptr, indices = _as_u32(g.indptr), _as_u32(g.indices)
-            check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
-                                             None, 0, codes.ctypes.data, n_cats, None, cnt.ctypes.data))
-        output = cnt if int_graph else cnt.astype(np.float64)
+        indptr, indices = _as_u32(g.indptr), _as_u32(g.indices)
+        check(lib.sqb_interaction_matrix(ctx.handle, g.shape[0], indices.size, indptr.ctypes.data, indices.ctypes.data,
+                                         None if data is None else data.ctypes.data, code, codes.ctypes.data, n_cats,
+                                         None if int_sums else out.ctypes.data, out.ctypes.data if int_sums else None))
+    output = out.astype(np.int64 if int_graph else np.float64, copy=False)  # counts of a float graph: float64
     if normalized:
         with np.errstate(divide="ignore", invalid="ignore"):
             output = output / output.sum(axis=1).reshape((-1, 1))  # _nhood.py:403-404
@@ -514,17 +513,14 @@ def interaction_matrix(
     return None
 
 
-def _interaction_device(lib, ctx: Context, graph: DevGraph, codes: np.ndarray, n_cats: int, out_w: np.ndarray | None,
-                        out_c: np.ndarray | None) -> None:
-    """Sums (``out_w``, float64) or counts (``out_c``, int64) of a device graph into the host matrix given, read in place by
-    ``sqb_interaction_matrix_device``; transposed back for a CSC graph."""
-    vals = graph.sparse.data
-    code = graph_value_code(vals, graph.nnz) if out_w is not None else 0
-    out = out_w if out_w is not None else out_c
+def _interaction_device(lib, ctx: Context, graph: DevGraph, codes: np.ndarray, n_cats: int, code: int, out: np.ndarray) -> None:
+    """``sqb_interaction_matrix_device`` on a device graph, read in place, into the host matrix ``out``: counts (``code`` -1)
+    and integer sums int64, float sums float64; transposed back for a CSC graph."""
+    int_out = code < 0 or code >= 3
     with ctx.lock:
         check(lib.sqb_interaction_matrix_device(ctx.handle, graph.n, graph.nnz, graph.indptr, graph.indptr_bits, graph.indices or None,
-                                                graph.index_bits, (vals.ptr or None) if out_w is not None else None, code,
-                                                codes.ctypes.data, n_cats, None if out_w is None else out_w.ctypes.data,
-                                                None if out_c is None else out_c.ctypes.data, graph.stream))
+                                                graph.index_bits, int(graph.transposed), (graph.sparse.data.ptr or None) if code >= 0 else None,
+                                                code, codes.ctypes.data, n_cats, None if int_out else out.ctypes.data,
+                                                out.ctypes.data if int_out else None, graph.stream))
     if graph.transposed:
         out[...] = out.T.copy()

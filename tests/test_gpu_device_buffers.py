@@ -139,21 +139,25 @@ def _interaction_device_error(array, match):
     return _raises(ValueError, match, lambda: sq.gr.interaction_matrix(_nh_adata(dev, g.shape[0], 3), "cl", copy=True))
 
 
-def _interaction_code_out_of_range():
-    """Codes come from a categorical in sq.gr.interaction_matrix, so a code >= n_cls only reaches the library directly."""
+def _interaction_code_beyond_n_cls(ordered: bool):
+    """Codes come from a categorical in sq.gr.interaction_matrix, so a code >= n_cls only reaches the library directly.
+    ``ordered``: float64 weights that no order-free sum reproduces, on the arrays of a CSC graph (the sorted, ordered path
+    and its buffers); otherwise counts."""
     g = synth.hex_graph(20, 20)
     n = g.shape[0]
     ip, ix = (torch.as_tensor(a.astype(np.int32)).cuda() for a in (g.indptr, g.indices))
+    vals = torch.as_tensor(np.random.default_rng(3).standard_normal(g.nnz) * 1e10).cuda()
     codes = np.zeros(n, np.int32)
     codes[7] = 3
-    out = np.zeros((3, 3), np.int64)
+    out = np.zeros((3, 3), np.float64 if ordered else np.int64)
 
     def call():
         torch.cuda.synchronize()  # the tensors are complete: no producer stream is named
         ctx = sq.default_context()
         with ctx.lock:
-            check(load().sqb_interaction_matrix_device(ctx.handle, n, g.nnz, ip.data_ptr(), 32, ix.data_ptr(), 32, None, 0, codes.ctypes.data,
-                                                       3, None, out.ctypes.data, 0))
+            check(load().sqb_interaction_matrix_device(ctx.handle, n, g.nnz, ip.data_ptr(), 32, ix.data_ptr(), 32, int(ordered),
+                                                       vals.data_ptr() if ordered else None, 1 if ordered else -1, codes.ctypes.data, 3,
+                                                       out.ctypes.data if ordered else None, None if ordered else out.ctypes.data, 0))
 
     return _raises(ValueError, "a code is >= n_cls", call)
 
@@ -262,7 +266,8 @@ CASES = {
     "nhood_device_index_out_of_range": lambda: _nhood_device_error(lambda g: {"indices": _big_index(g)}, "invalid CSR"),
     "interaction_device_indptr": lambda: _interaction_device_error(lambda g: {"indptr": _first_indptr(g)}, "indptr"),
     "interaction_device_index_out_of_range": lambda: _interaction_device_error(lambda g: {"indices": _big_index(g)}, "out of range"),
-    "interaction_device_code_out_of_range": _interaction_code_out_of_range,
+    "interaction_device_code_beyond_n_cls": lambda: _interaction_code_beyond_n_cls(False),
+    "interaction_device_ordered_code_beyond_n_cls": lambda: _interaction_code_beyond_n_cls(True),
     "ligrec_duplicate_cell": lambda: _ligrec_error("duplicate_cell"),
     "ligrec_index_out_of_range": lambda: _ligrec_error("index_out_of_range"),
     "ligrec_indptr": lambda: _ligrec_error("indptr"),

@@ -239,9 +239,9 @@ def test_builtin_builders_declare_the_reference_postprocessors():
     assert nb.GridBuilder(transform="spectral").postprocessors() == [nb.TransformPostprocessor(Transform.SPECTRAL)]
 
 
-def test_new_abi_symbols_are_declared():
+def test_abi_version_and_symbols_are_declared():
     assert "sqb_graph_postprocess" in _lib.EXPORTED_SYMBOLS and "sqb_graph_combine" in _lib.EXPORTED_SYMBOLS
-    assert _lib.ABI_VERSION == 17
+    assert _lib.ABI_VERSION == 18
     lib = _lib.load()
-    assert lib.sqb_abi_version() == 17
+    assert lib.sqb_abi_version() == 18
     assert hasattr(lib, "sqb_graph_postprocess") and hasattr(lib, "sqb_graph_combine")

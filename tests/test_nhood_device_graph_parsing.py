@@ -169,13 +169,13 @@ def test_nhood_csc_transposes_count_mean_and_std(no_scipy_graph, monkeypatch, fm
 
 @pytest.mark.parametrize("weights", [False, True])
 @pytest.mark.parametrize("fmt", ["csr", "csc"])
-def test_interaction_csc_transposes_the_result(no_scipy_graph, monkeypatch, fmt, weights):
+def test_interaction_passes_the_csc_flag_and_transposes_the_result(no_scipy_graph, monkeypatch, fmt, weights):
     block = np.array([[1, 2, 3], [4, 5, 6], [7, 8, 10]])
     calls = []
 
     class Lib:
-        def sqb_interaction_matrix_device(self, ctx, n, nnz, ip, ip_bits, ix, ix_bits, data, code, codes, n_cats, out_w, out_c, stream):
-            calls.append((n, nnz, ip_bits, ix_bits, data, code))
+        def sqb_interaction_matrix_device(self, ctx, n, nnz, ip, ip_bits, ix, ix_bits, csc, data, code, codes, n_cats, out_w, out_c, stream):
+            calls.append((n, nnz, ip_bits, ix_bits, csc, data, code))
             import ctypes
 
             dst = out_w if weights else out_c
@@ -185,7 +185,7 @@ def test_interaction_csc_transposes_the_result(no_scipy_graph, monkeypatch, fmt,
 
     monkeypatch.setattr(_nhood, "load", lambda: Lib())
     out = _nhood.interaction_matrix(_adata(FakeGraph(fmt, ip="<i8")), "cl", weights=weights, copy=True)
-    assert calls == [(6, 9, 64, 32, 0x3000 if weights else None, 0 if weights else 0)]
+    assert calls == [(6, 9, 64, 32, int(fmt == "csc"), 0x3000 if weights else None, 0 if weights else -1)]
     assert out.dtype == np.float64  # float32 graph values: float64 as on the host
     assert np.array_equal(out, block.T if fmt == "csc" else block)
 

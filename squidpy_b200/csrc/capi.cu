@@ -192,6 +192,20 @@ int sqb_ctx_create(int device, void* stream, sqb_ctx** out) {
     }
     cudaEventCreate(&c->ev0);
     cudaEventCreate(&c->ev1);
+    cudaEventCreate(&c->ev_in0);
+    cudaEventCreate(&c->ev_in1);
+    {
+        int least = 0, greatest = 0;
+        e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
+        if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->tail, cudaStreamNonBlocking, greatest);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
+        if (e != cudaSuccess) {
+            sqb_ctx_destroy(c);
+            sqb_set_error("sqb_ctx_create: second stream: %s", cudaGetErrorString(e));
+            return SQB_ERR_CUDA;
+        }
+    }
     {  // keep freed blocks of the stream-ordered allocator in the pool (handles are created and destroyed per API call)
         cudaMemPool_t pool = nullptr;
         if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
@@ -217,6 +231,14 @@ int sqb_ctx_destroy(sqb_ctx* c) {
     cudaSetDevice(c->device);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
+    if (c->ev_in0) cudaEventDestroy(c->ev_in0);
+    if (c->ev_in1) cudaEventDestroy(c->ev_in1);
+    if (c->ev_fork) cudaEventDestroy(c->ev_fork);
+    if (c->ev_join) cudaEventDestroy(c->ev_join);
+    if (c->tail) {
+        cudaStreamSynchronize(c->tail);
+        cudaStreamDestroy(c->tail);
+    }
     if (c->stream) cudaStreamSynchronize(c->stream);
     for (auto& s : c->scratch) s.release();
     for (int b = 0; b < sqb_ctx::kStage; ++b) {

@@ -126,6 +126,12 @@ struct sqb_ctx {
     double k_ms[SQB_K_NCLASS] = {0};
     int64_t k_n[SQB_K_NCLASS] = {0};
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    cudaEvent_t ev_in0 = nullptr, ev_in1 = nullptr;  // profile events of a launch timed inside another launch's scope
+    // Second stream at the device's greatest priority, owned by the context: the region replay's last round runs on it, so
+    // that the block scheduler places its CTAs before those of the transpose the context stream runs beside it (nhood.cu,
+    // launch_shuffle_part).  fork (fired once every CTA of the whole rounds has begun) / join order it with the context stream.
+    cudaStream_t tail = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     // Large scratch buffers that live as long as the context (GB-sized cudaMalloc/cudaFree per API call would
     // otherwise dominate the host-facing latency).  Work on one ctx is stream ordered, so handles can share them.
     DevBuf<uint8_t> scratch[4];
@@ -161,21 +167,24 @@ int sqb_wait_producer(sqb_ctx* c, uintptr_t producer);
 
 // Launch accounting.  In profile mode each launch is bracketed by events on the ctx stream and the elapsed
 // time accumulated per kernel class (the launch is synchronised; never used inside a timed bench region
-// except for the dedicated roofline pass).
+// except for the dedicated roofline pass).  A scope opened inside another one passes inner = true: it takes the second
+// pair of events, and its time overlaps the outer scope's.
 struct SqbLaunchScope {
     sqb_ctx* c;
     int kclass;
-    SqbLaunchScope(sqb_ctx* ctx, int k) : c(ctx), kclass(k) {
-        if (c->profile) cudaEventRecord(c->ev0, c->stream);
+    cudaEvent_t e0, e1;
+    SqbLaunchScope(sqb_ctx* ctx, int k, bool inner = false)
+        : c(ctx), kclass(k), e0(inner ? ctx->ev_in0 : ctx->ev0), e1(inner ? ctx->ev_in1 : ctx->ev1) {
+        if (c->profile) cudaEventRecord(e0, c->stream);
     }
     ~SqbLaunchScope() {
         c->launches += 1;
         c->k_n[kclass] += 1;
         if (c->profile) {
-            cudaEventRecord(c->ev1, c->stream);
-            cudaEventSynchronize(c->ev1);
+            cudaEventRecord(e1, c->stream);
+            cudaEventSynchronize(e1);
             float ms = 0.f;
-            cudaEventElapsedTime(&ms, c->ev0, c->ev1);
+            cudaEventElapsedTime(&ms, e0, e1);
             c->k_ms[kclass] += ms;
         }
     }

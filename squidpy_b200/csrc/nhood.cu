@@ -2567,6 +2567,7 @@ struct sqb_nhood {
     int count_single = 1;  // sqb_nhood_count: 1 = dedicated single-vector kernel, 0 = the batched kernels (test hook)
     int64_t shuffle_ctas = 0;          // persistent CTAs of the shuffle kernel (0 = occupancy x SM count)
     int shuffle_wfactor_x100 = 400;    // window = min(i/4, wfactor * sqrt(i)) raw values
+    int tail_overlap = 1;  // algo 9: transpose the finished groups under the replay's last round (0 = after it; measuring hook)
 };
 
 template <typename LT>
@@ -2845,25 +2846,63 @@ static int part_replay_shape(const sqb_nhood* h, int64_t np, PartShape* out) {
     return SQB_OK;
 }
 
+// persistent CTAs of the region replay: every CTA resident
+static int64_t part_apply_grid(const sqb_nhood* h, const PartShape& ps) {
+    return h->shuffle_ctas > 0 ? h->shuffle_ctas : (int64_t)ps.per_sm * h->ctx->sm_count;
+}
+
+// region replay of the np permutations whose label rows, J rows and count rows start at lab, J and cnt, on stream s; started
+// (or null): an event that fires once every CTA of the launch has begun (a launch-completion event, best effort: at the
+// latest when the launch completes)
 template <typename LT, int NT>
 static int launch_apply_part(sqb_nhood* h, LT* lab, const uint32_t* J, const uint16_t* cnt, int64_t nb_total, const PartShape& ps,
-                             int64_t np) {
-    sqb_ctx* c = h->ctx;
+                             int64_t np, cudaStream_t s, cudaEvent_t started) {
     const int nbmax = part_max_blocks(h);
     const size_t smem = part_tables_bytes(NT, (int)sizeof(LT), nbmax) + (size_t)ps.cap * sizeof(LT);
     SQB_TRY((part_apply_attributes<LT, NT>(smem)));
-    int64_t grid = h->shuffle_ctas;
-    if (grid <= 0) grid = (int64_t)ps.per_sm * c->sm_count;  // every CTA resident, persistent over the permutations
+    int64_t grid = part_apply_grid(h, ps);
     if (grid > np) grid = np;
-    nhood_apply_part_kernel<LT, NT><<<(unsigned)grid, NT, smem, c->stream>>>(
-        lab, J, cnt, reinterpret_cast<const LT*>(h->d_base.p), h->stride, np, h->nseg, h->d_seg_start.p, h->d_seg_len.p, nb_total,
-        ps.cap, sqb_part_bwords(nbmax));
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeLaunchCompletionEvent;
+    attr.val.launchCompletionEvent.event = started;
+    attr.val.launchCompletionEvent.flags = 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)grid);
+    cfg.blockDim = dim3(NT);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cfg.attrs = &attr;
+    cfg.numAttrs = started ? 1 : 0;
+    SQB_CUDA(cudaLaunchKernelEx(&cfg, nhood_apply_part_kernel<LT, NT>, lab, J, cnt, reinterpret_cast<const LT*>(h->d_base.p), h->stride,
+                                np, h->nseg, (const int64_t*)h->d_seg_start.p, (const int64_t*)h->d_seg_len.p, nb_total, ps.cap,
+                                sqb_part_bwords(nbmax)));
     return SQB_OK;
 }
 
-// shuffle_algo 9: partitioned swap targets + region replay (the label rows are not filled: the replay reads the base labels)
+// transpose (3) of the label groups [g0, g1) of a chunk of np permutations on the context stream; inner: timed inside the
+// scope of another launch
 template <typename LT>
-static int launch_shuffle_part(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, const PartShape& ps) {
+static int launch_transpose(sqb_nhood* h, const LT* lab, LT* labT, int64_t g0, int64_t g1, int64_t np, bool inner) {
+    sqb_ctx* c = h->ctx;
+    SqbLaunchScope scope(c, SQB_K_NHOOD_TRANSPOSE, inner);
+    dim3 grid((unsigned)ceil_div64(h->n, 256), (unsigned)(g1 - g0));
+    nhood_transpose_kernel<LT><<<grid, 256, 0, c->stream>>>(lab + g0 * 64 * h->stride, labT + g0 * (h->n + 1) * 64, h->n, h->stride,
+                                                            (int)(np - g0 * 64), h->has_order ? h->d_order.p : nullptr);
+    SQB_POST_LAUNCH();
+    return SQB_OK;
+}
+
+// shuffle_algo 9: partitioned swap targets + region replay (the label rows are not filled: the replay reads the base labels).
+// When the chunk is counted (labT given) and the replay's last round is partial, the replay is split there: the context stream
+// replays permutations [0, pa) in whole rounds of the grid, pa = floor(np / grid) * grid, and the last round [pa, np) runs as a
+// second launch on the context's high-priority stream.  That launch waits only until every CTA of the first has begun, so its
+// CTAs take the places of the first launch's CTAs as these finish, as one launch's CTAs would.  When the first launch
+// completes, the context stream transposes the groups of 64 permutations that [0, pa) completes, on the SMs the partial round
+// leaves half empty (DESIGN.md §3.1), and waits for the last round before anything else.  *g_done = the groups transposed here
+// (0 without the split).
+template <typename LT>
+static int launch_shuffle_part(sqb_nhood* h, LT* lab, LT* labT, const uint64_t* states, int64_t np, const PartShape& ps,
+                               int64_t* g_done) {
     sqb_ctx* c = h->ctx;
     int64_t nb_total = 0;
     for (int64_t m : h->h_seg_len) nb_total += (m + SQB_PART_L - 1) / SQB_PART_L;
@@ -2872,10 +2911,28 @@ static int launch_shuffle_part(sqb_nhood* h, LT* lab, const uint64_t* states, in
     uint32_t* J = reinterpret_cast<uint32_t*>(c->scratch[2].p);
     uint16_t* cnt = reinterpret_cast<uint16_t*>(c->scratch[3].p);
     SQB_TRY(launch_jgen<true>(h, J, states, np, cnt, nb_total, ps.cap));
+    auto apply = [&](int64_t q0, int64_t q1, cudaStream_t s, cudaEvent_t started) -> int {
+        LT* l = lab + q0 * h->stride;
+        const uint32_t* j = J + q0 * h->stride;
+        const uint16_t* k = cnt + q0 * nb_total * SQB_PART_RMAX;
+        const int rc = ps.nt == 512 ? launch_apply_part<LT, 512>(h, l, j, k, nb_total, ps, q1 - q0, s, started)
+                                    : launch_apply_part<LT, 1024>(h, l, j, k, nb_total, ps, q1 - q0, s, started);
+        SQB_TRY(rc);
+        SQB_POST_LAUNCH();
+        return SQB_OK;
+    };
     SqbLaunchScope scope(c, SQB_K_NHOOD_SHUFFLE);
-    if (ps.nt == 512) SQB_TRY((launch_apply_part<LT, 512>(h, lab, J, cnt, nb_total, ps, np)));
-    else SQB_TRY((launch_apply_part<LT, 1024>(h, lab, J, cnt, nb_total, ps, np)));
-    SQB_POST_LAUNCH();
+    const int64_t pa = np / part_apply_grid(h, ps) * part_apply_grid(h, ps);
+    const int64_t ga = pa / 64;
+    if (!labT || !h->tail_overlap || pa == np || ga == 0) return apply(0, np, c->stream, nullptr);
+    SQB_TRY(apply(0, pa, c->stream, c->ev_fork));
+    SQB_CUDA(cudaStreamWaitEvent(c->tail, c->ev_fork, 0));
+    SQB_TRY(apply(pa, np, c->tail, nullptr));
+    SQB_CUDA(cudaEventRecord(c->ev_join, c->tail));
+    const int rc = launch_transpose<LT>(h, lab, labT, 0, ga, np, true);
+    SQB_CUDA(cudaStreamWaitEvent(c->stream, c->ev_join, 0));  // on every path: the last round is ordered before what follows
+    SQB_TRY(rc);
+    *g_done = ga;
     return SQB_OK;
 }
 
@@ -2903,10 +2960,12 @@ static int launch_shuffle_two_kernel(sqb_nhood* h, LT* lab, const uint64_t* stat
     return SQB_OK;
 }
 
+// labT / *g_done: see launch_shuffle_part (the other replays transpose nothing)
 template <typename LT>
-static int launch_shuffle(sqb_nhood* h, LT* lab, const uint64_t* states, int64_t np, const PartShape& ps) {
+static int launch_shuffle(sqb_nhood* h, LT* lab, LT* labT, const uint64_t* states, int64_t np, const PartShape& ps, int64_t* g_done) {
     sqb_ctx* c = h->ctx;
-    if (ps.nt) return launch_shuffle_part<LT>(h, lab, states, np, ps);
+    *g_done = 0;
+    if (ps.nt) return launch_shuffle_part<LT>(h, lab, labT, states, np, ps, g_done);
     if (h->shuffle_algo == 7)
         return launch_shuffle_two_kernel<LT>(h, lab, states, np, h->shuffle_threads, h->shuffle_r, h->shuffle_low,
                                              (uint64_t)h->shuffle_stagger_us * 1000ull);
@@ -2992,16 +3051,11 @@ static int run_chunk(sqb_nhood* h, int64_t p0, int64_t np, bool do_count) {
                                                                   vec_per_row, np);
         SQB_POST_LAUNCH();
     }
-    SQB_TRY(launch_shuffle<LT>(h, lab, h->d_states.p + p0 * 4, np, ps));
+    int64_t g_done = 0;  // label groups the shuffle already transposed
+    SQB_TRY(launch_shuffle<LT>(h, lab, do_count ? labT : nullptr, h->d_states.p + p0 * 4, np, ps, &g_done));
     if (!do_count) return SQB_OK;
     const int PB = (int)sqb_labT_pb(np);
-    {
-        SqbLaunchScope scope(c, SQB_K_NHOOD_TRANSPOSE);
-        dim3 grid((unsigned)ceil_div64(h->n, 256), (unsigned)(PB / 64));
-        nhood_transpose_kernel<LT><<<grid, 256, 0, c->stream>>>(lab, labT, h->n, h->stride, (int)np,
-                                                                h->has_order ? h->d_order.p : nullptr);
-        SQB_POST_LAUNCH();
-    }
+    SQB_TRY(launch_transpose<LT>(h, lab, labT, g_done, PB / 64, np, false));
     SQB_TRY(launch_count<LT>(h, labT, PB, (int)np, h->d_counts.p + p0 * (int64_t)h->n_cls * h->n_cls));
     return SQB_OK;
 }
@@ -3421,6 +3475,9 @@ int sqb_nhood_set_option(sqb_nhood* h, const char* key, int64_t value) {
     } else if (!strcmp(key, "count_algo")) {
         SQB_CHECK(value >= 0 && value <= 2, SQB_ERR_INVALID, "count_algo must be 0, 1 or 2");
         h->count_algo = (int)value;
+    } else if (!strcmp(key, "tail_overlap")) {
+        SQB_CHECK(value == 0 || value == 1, SQB_ERR_INVALID, "tail_overlap must be 0 or 1");
+        h->tail_overlap = (int)value;
     } else {
         sqb_set_error("sqb_nhood_set_option: unknown key '%s'", key);
         return SQB_ERR_INVALID;
